@@ -1,8 +1,8 @@
-# Builds libtsgpu.so (product, sm_100a only), the CPU oracle and the test-only SIMT build.
+# Builds libtsgpu.so (product, sm_90a only), the CPU oracle and the test-only SIMT build.
 PKG := tiered-storage-for-apache-kafka_b200
 CSRC := $(PKG)/csrc
 NVCC ?= nvcc
-NVCCFLAGS := -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC,-Wall -Xptxas -v \
+NVCCFLAGS := -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC,-Wall -Xptxas -v \
              --expt-relaxed-constexpr
 HDRS := $(wildcard $(CSRC)/*.cuh $(CSRC)/*.h $(CSRC)/*.hpp $(CSRC)/*.inc) include/tsgpu.h
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — segment transform throughput (BASELINE.json metric) on N B200s, one process per GPU.
+"""bench.py — segment transform throughput (BASELINE.json metric) on N H100s, one process per GPU.
 
 A "step" = one pass of the hot path over one synthetic segment (default: 1 GiB, 4 MiB chunks, Zstd + AES-256-GCM,
 i.e. BASELINE.json configs[3], which is the configuration the metric is quoted on and fits one GPU).
@@ -53,6 +53,9 @@ def parse():
     ap.add_argument("--window-mib", type=int, default=16)
     ap.add_argument("--config", type=int, default=None, choices=[0, 1, 2, 3, 4],
                     help="shorthand for BASELINE.json configs[N] (0: 256 MiB no transform, 1: zstd, 2: aes, 3: zstd+aes, 4: ranged fetch)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float64 sizes, "
+                         "a fixed seeded float32 sample of the bytes; at most 64 MB in all), to compare two builds")
     a = ap.parse_args()
     if a.config is not None:
         if a.config == 0:
@@ -61,6 +64,8 @@ def parse():
             a.workload, a.direction = "zstd+aes", "fetch"
         else:
             a.workload = {1: "zstd", 2: "aes", 3: "zstd+aes"}[a.config]
+    if a.dump_outputs and (a.impl != "tsgpu" or a.workload == "none"):
+        ap.error("--dump-outputs needs the GPU path (--impl tsgpu and a workload other than none)")
     return a
 
 
@@ -83,15 +88,15 @@ def config_of(args, n_gpus):
         "segment_bytes": args.segment_mib * MIB, "chunk_bytes": args.chunk_mib * MIB,
         "transform": args.workload, "corpus": args.corpus, "zstd_mode": args.zstd_mode if "zstd" in args.workload else None,
         "parallelism": "segments sharded across %d GPU(s), no data-path collective" % n_gpus,
-        "l2_policy": "inputs (segment >= 1 GiB) larger than the 126 MB L2; no explicit flush",
+        "l2_policy": "inputs (segment >= 1 GiB) larger than the 50 MB L2; no explicit flush",
     }
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.index = index
@@ -131,7 +136,7 @@ class ClockSampler:
         # taken under the same load right before it (warm-up runs the identical step) are used and counted separately
         inside = [r for (t, r) in self.rows if self.t0 is not None and self.t0 <= t <= (self.t1 or t)]
         rows = inside if inside else [r for (t, r) in self.rows][-5:]
-        sm, mx, reasons = [], [], set()
+        sm, mx, plim, reasons = [], [], [], set()
         for r in rows:
             f = [x.strip() for x in r.split(",")]
             if len(f) < 9:
@@ -140,11 +145,16 @@ class ClockSampler:
                 sm.append(float(f[1])); mx.append(float(f[2]))
             except ValueError:
                 continue
+            if len(f) > 9:
+                try:
+                    plim.append(float(f[9]))
+                except ValueError:
+                    pass
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm), "samples_inside_timed_region": len(inside)}
+                "power_limit_w": max(plim) if plim else None, "reasons": sorted(reasons), "samples": len(sm), "samples_inside_timed_region": len(inside)}
 
 
 def load_peaks():
@@ -154,7 +164,33 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, not measured)"
+
+
+DUMP_BYTES = 63_000_000            # the arrays; with the .npy headers the files stay under 64 MB (and 64 MiB)
+DUMP_SEED = 20240917
+
+
+def dump_outputs(out_dir, torch, flat, starts, lengths, named):
+    """Writes `named` (name -> array of sizes / status words, as float64) and, from each of the rows
+    flat[starts[i] : starts[i] + lengths[i]] (a uint8 device tensor), the bytes at the same fixed seeded fractions of the
+    row's length (float32, one row per chunk; -1 where a row is empty) to out_dir/<name>.npy.  The sample positions depend
+    only on the seed and on the lengths, so two builds that compute the same sizes are compared byte for byte."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float64) for k, v in named.items()}
+    rows = len(starts)
+    per_row = max(1, (DUMP_BYTES - sum(a.nbytes for a in arrays.values())) // 4 // max(1, rows))
+    per_row = min(per_row, int(max(lengths)) if rows else 1)
+    frac = np.sort(np.random.default_rng(DUMP_SEED).random(per_row))
+    dev = flat.device
+    ln = torch.as_tensor(np.asarray(lengths, dtype=np.int64), device=dev)
+    off = (torch.as_tensor(frac, device=dev)[None, :] * ln[:, None].double()).long()
+    idx = torch.as_tensor(np.asarray(starts, dtype=np.int64), device=dev)[:, None] + off
+    sample = flat[idx.clamp(max=flat.numel() - 1).reshape(-1)].reshape(rows, per_row).float()
+    arrays["bytes_sample"] = torch.where(ln[:, None] > 0, sample, torch.full_like(sample, -1.0)).cpu().numpy()
+    assert sum(a.nbytes for a in arrays.values()) <= DUMP_BYTES
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
 
 
 def make_segment(args, segment_id):
@@ -346,7 +382,7 @@ def main_fetch(args):
     d_dst = torch.zeros(wch * cs, dtype=torch.uint8, device=dev)
     d_osz = torch.zeros(wch, dtype=torch.int32, device=dev); d_st = torch.zeros(wch, dtype=torch.int32, device=dev)
     stream = torch.cuda.current_stream().cuda_stream
-    flush = torch.empty(256 * MIB, dtype=torch.uint8, device=dev)      # > 126 MB L2: written between timed windows
+    flush = torch.empty(256 * MIB, dtype=torch.uint8, device=dev)      # > 50 MB L2: written between timed windows
 
     def step_device(i):
         d_slots, d_sizes = wins[i % len(wins)]
@@ -379,10 +415,14 @@ def main_fetch(args):
         ok = ok and int(d_st.abs().sum().item()) == 0
     barrier()
     sampler.end()
+    clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        osz = d_osz.cpu().numpy()
+        dump_outputs(args.dump_outputs, torch, d_dst, [k * cs for k in range(wch)], osz,
+                     {"original_sizes": osz, "status": d_st.cpu().numpy()})
     ok = ok and bool(np.array_equal(d_dst.cpu().numpy(), src_np[f * cs:(f + wch) * cs]))      # last window, checked after timing
     ms = sum(a.elapsed_time(b) for a, b in evs)
     launches = ctx.launch_count() - l0
-    clocks = sampler.stop() if rank == 0 else None
     t = torch.tensor([ms], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -452,7 +492,7 @@ def main_fetch(args):
             "warmup": args.warmup, "ms_per_step": ms_max / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "u8", "data": "synthetic", "config": dict(config_of(args, world),
                 l2_policy="256 MiB written between timed windows (L2 flush), outside the per-window events"),
-            "frames_written_by": args.frames, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
+            "gpu": torch.cuda.get_device_name(local), "frames_written_by": args.frames, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
             "roofline": roofline, "cpu_baseline": cpu, "kernels_ms_per_step": kernels, "verified": {"windows_bit_exact": bool(ok)}}))
     if not ok:
         raise SystemExit("bench.py: a fetched window differs from the segment")
@@ -584,6 +624,9 @@ def main_tsgpu(args):
     value = world * seg * args.steps / GIB / (ms_max / 1000.0)
     sizes = d_sizes.cpu().numpy().astype(np.int64)
     transformed_total = int(sizes.sum())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, d_slots, [i * stride + 4 for i in range(nch)], sizes,
+                     {"transformed_sizes": sizes})
 
     # ---- verify what was timed (after the timed region): the slots the LAST timed step left behind go back through the
     # device detransform and must equal the segment byte for byte; a seeded sample of chunks is also decoded by the CPU
@@ -626,23 +669,8 @@ def main_tsgpu(args):
             alg = seg + transformed_total
         peak, how = load_peaks()
         achieved = alg / 1e9 / (ms_k / 1000.0)
-        traffic, traffic_capture = None, None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            try:
-                # keys are kernel names ("zstd_enc_blocks"); values {"bytes": per-launch DRAM read + write, "capture": file}
-                tj = json.load(open(tpath))
-                ent = tj.get(name, tj.get(name.rsplit("_", 1)[0]))
-                here = "%s|%s|%s|%d" % (args.workload, args.zstd_mode, args.corpus, args.segment_mib)
-                if isinstance(ent, dict) and ent.get("bench_config") == here:      # only a capture taken at THIS configuration
-                    traffic, traffic_capture = ent.get("bytes"), ent.get("capture")
-            except Exception:
-                traffic = None
         roofline = {"bound": "hbm", "kernel": name, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                    "frac": achieved / peak, "traffic": traffic, "peak_source": how,
-                    "traffic_source": None if traffic is None else
-                    "STATIC: dram__bytes_read.sum + dram__bytes_write.sum of one launch at this configuration from the ncu --set "
-                    "full capture %s (not measured in this run)" % traffic_capture,
+                    "frac": achieved / peak, "traffic": None, "peak_source": how,
                     "algorithmic_bytes_per_launch": alg, "kernel_ms": ms_k,
                     "note": "integer/LDS-bound kernels: see DESIGN.md for the ALU/shared-memory ceilings"}
 
@@ -723,8 +751,8 @@ def main_tsgpu(args):
             "dtype": "u8", "data": "synthetic", "config": config_of(args, world),
             "compression_ratio": seg / max(1, transformed_total - (28 * nch if flags & 2 else 0)) if flags & 1 else None,
             "transformed_bytes_per_segment": transformed_total,
-            "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline,
-            "cpu_baseline": cpu, "kernels_ms_per_step": kernels, "verified": verified,
+            "gpu": torch.cuda.get_device_name(local), "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
+            "roofline": roofline, "cpu_baseline": cpu, "kernels_ms_per_step": kernels, "verified": verified,
         }
         print(json.dumps(line))
     ctx.close()

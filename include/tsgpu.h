@@ -1,11 +1,11 @@
 /*
- * tsgpu.h — C-ABI of libtsgpu.so: the B200-native chunk-transform pipeline behind Aiven's
+ * tsgpu.h — C-ABI of libtsgpu.so: the H100-native (sm_90a) chunk-transform pipeline behind Aiven's
  * tiered-storage RemoteStorageManager operator surface.
  *
  * The reference has no FFI of its own (pure Java); its boundary for this path is the pair of Java interfaces
  *   TransformChunkEnumeration    core/M/transform/TransformChunkEnumeration.java:28-42
  *   DetransformChunkEnumeration  core/M/transform/DetransformChunkEnumeration.java:28-29
- * (core/M = /root/reference/core/src/main/java/io/aiven/kafka/tieredstorage).  A thin JNI class (jni/, see
+ * (core/M = <reference>/core/src/main/java/io/aiven/kafka/tieredstorage).  A thin JNI class (jni/, see
  * INTEGRATION.md) implements those interfaces by handing a *batch* of chunks to the calls below and serving
  * one byte[] per nextElement().  Each entry point names the reference code it replaces.
  *
@@ -27,8 +27,8 @@ extern "C" {
 #define TSGPU_FLAG_ZSTD 1u     /* compression.enabled  (RemoteStorageManagerConfig.java:132-138) */
 #define TSGPU_FLAG_AES  2u     /* encryption.enabled   (RemoteStorageManagerConfig.java:147-153) */
 /* Modifier of TSGPU_FLAG_ZSTD on the transform side (ignored by detransform): compress for size rather than for speed.
- * Default: independent 8 KiB blocks, ~3.1 : 1 on Kafka-like text at ~14.7 ms per GiB on a B200 — the segment pipeline stays
- * PCIe-bound.  Dense: 64 KiB regions sharing one window and one set of entropy tables, ~3.5 : 1 at ~27 ms per GiB and
+ * Default: independent 8 KiB blocks, ~3.1 : 1 on Kafka-like text, about twice as fast as dense.  Dense: 64 KiB regions
+ * sharing one window and one set of entropy tables, ~3.5 : 1 and
  * byte-identical frames on every run.  Both are plain zstd frames with Frame_Content_Size; libzstd and this library read both.
  * TSGPU_ZSTD_MODE=dense in the environment makes dense the default of a context. */
 #define TSGPU_FLAG_ZSTD_DENSE 4u

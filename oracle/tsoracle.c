@@ -1,6 +1,6 @@
 /*
  * tsoracle.c — CPU oracle (TEST INFRASTRUCTURE ONLY; see tsoracle.h for scope, citations and pinning).
- * Paths cited as core/M/... = /root/reference/core/src/main/java/io/aiven/kafka/tieredstorage/...
+ * Paths cited as core/M/... = <reference>/core/src/main/java/io/aiven/kafka/tieredstorage/...
  */
 #define _GNU_SOURCE
 #include "tsoracle.h"

@@ -4,7 +4,7 @@
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference leg may
  * load this library.  The product (libtsgpu.so) never links, loads or calls anything in oracle/.
  *
- * What it restates (reference paths relative to /root/reference/core/src/main/java/io/aiven/kafka/tieredstorage/):
+ * What it restates (reference paths relative to <reference>/core/src/main/java/io/aiven/kafka/tieredstorage/):
  *   - transform/CompressionChunkEnumeration.java:49-62   one zstd frame per chunk, level 3, contentSize=true,
  *                                                        pledgedSrcSize, fresh ctx per chunk
  *   - transform/EncryptionChunkEnumeration.java:65-84    IV(12) || AES-256-GCM(ct) || TAG(16), AAD per segment

@@ -37,7 +37,7 @@ cap gcm_main gcm_main 1 -- python bench.py --steps 1 --warmup 1 --no-e2e --no-cp
 SKIPK=3 cap zstd_dec_blk 'zstd_dec_blk_literals|zstd_dec_blk_sequences|zstd_dec_indep_execute' 3 -- python tests/perf/bench_detransform.py 256
 cap zstd_dec_regions zstd_dec_regions 1 -- python bench.py --direction fetch --frames own --zstd-mode dense --segment-mib 256 --window-mib 256 --steps 1 --warmup 1 --no-e2e --no-cpu-baseline
 SKIPK=0 cap zstd_dec_libzstd 'zstd_dec_par_entropy|zstd_dec_par_execute' 2 -- python bench.py --direction fetch --frames libzstd --steps 1 --warmup 0 --no-e2e --no-cpu-baseline --segment-mib 64
-# compute-sanitizer over the smoke invocation (both compressors, every decode path, AES both ways): logs go under profiles/
+# compute-sanitizer over the smoke invocation (both compressors, every decode path, AES both ways): logs go to the output directory
 timeout 420 compute-sanitizer --tool memcheck --log-file $O/${R}_sanitizer_memcheck.log python -c "import __graft_entry__ as g; g.smoke()" > $O/${R}_sanitizer_memcheck.out 2>&1; echo "memcheck exit $?" >> $O/${R}_sanitizer_memcheck.out
 timeout 420 compute-sanitizer --tool racecheck --log-file $O/${R}_sanitizer_racecheck.log python -c "import __graft_entry__ as g; g.smoke()" > $O/${R}_sanitizer_racecheck.out 2>&1; echo "racecheck exit $?" >> $O/${R}_sanitizer_racecheck.out
 for f in $O/${R}_sanitizer_memcheck.log $O/${R}_sanitizer_racecheck.log; do tail -n 3 $f; done

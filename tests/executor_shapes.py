@@ -1,4 +1,4 @@
-"""Inputs shared by the emulator and the B200 tests of the frame executor."""
+"""Inputs shared by the emulator and the GPU tests of the frame executor."""
 import numpy as np
 
 

@@ -98,7 +98,7 @@ def main():
         f.write("\n")
     print("wrote", len(frames["frames"]), "frames,", sum(len(x["frame_b64"]) for x in frames["frames"]), "base64 bytes")
     # dense-mode frames of THIS library are a function of the input (DESIGN.md 4.2): digests of what the emulated kernels write,
-    # so that (a) an unintended change of the compressed bytes shows up and (b) the B200 can be checked against the emulator
+    # so that (a) an unintended change of the compressed bytes shows up and (b) the GPU can be checked against the emulator
     import subprocess
     simt = os.path.join(ROOT, "tests", "simt", "libtsgpu_simt.so")
     subprocess.check_call(["make", "-s", "-C", ROOT, "tests/simt/libtsgpu_simt.so"])

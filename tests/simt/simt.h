@@ -2,7 +2,7 @@
  * simt.h — TEST-ONLY SIMT emulator.  NOT part of the product; libtsgpu.so never includes this file.
  *
  * The build container has nvcc but no GPU, and GPU time (gpurun) is scarce.  To debug kernel *logic*
- * (bit-stream formats, table construction, index arithmetic) before going to a B200, the device
+ * (bit-stream formats, table construction, index arithmetic) before going to an H100, the device
  * headers under tiered-storage-for-apache-kafka_b200/csrc/ are written in a restricted CUDA subset
  * that this header can also compile with plain g++: every CUDA thread of a block becomes a fiber
  * (hand-rolled x86-64 context switch), warp collectives and barriers are rendezvous points, blocks

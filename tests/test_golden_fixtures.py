@@ -1,6 +1,6 @@
 """The committed fixtures under tests/golden/ (made by tests/golden/make_golden.py): golden vectors transcribed from the
 reference's tests + public AES known answers, and libzstd-written frames.  CPU leg: the oracle and the SIMT-emulated
-product code both reproduce them; the `-m gpu` leg repeats the product checks on a B200 through the C-ABI."""
+product code both reproduce them; the `-m gpu` leg repeats the product checks on an H100 through the C-ABI."""
 import base64
 import hashlib
 import json
@@ -116,10 +116,8 @@ def test_emulated_dense_frames_are_the_committed_ones():
 
 
 @pytest.mark.gpu
-@pytest.mark.xfail(strict=False, reason="emulator-vs-hardware byte identity of dense-mode frames: added after the round's last GPU "
-                                        "lease, so its first run on a B200 is the driver's; an XPASS is the expected outcome")
 def test_gpu_dense_frames_equal_the_emulators():
-    # the B200 writes byte for byte what the emulator writes for the same input: the CPU-side kernel tests and the hardware
+    # the GPU writes byte for byte what the emulator writes for the same input: the CPU-side kernel tests and the hardware
     # run the same algorithm (round trips are asserted unconditionally inside _dense_digests)
     ctx = tsgpu.Context(max_chunk_bytes=1 << 19, max_batch=4)
     try:

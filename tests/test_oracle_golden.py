@@ -1,5 +1,5 @@
 """Pins the CPU oracle on every golden vector / exact expectation the reference's own tests hold for the
-hot path (SURVEY.md §8c).  Citations: core/T = /root/reference/core/src/test/java/io/aiven/kafka/tieredstorage."""
+hot path (SURVEY.md §8c).  Citations: core/T = <reference>/core/src/test/java/io/aiven/kafka/tieredstorage."""
 import base64
 
 import numpy as np

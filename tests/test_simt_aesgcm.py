@@ -1,6 +1,6 @@
 """Runs the REAL AES-GCM kernel sources under the test-only SIMT emulator (tests/simt/) through the C-ABI and
 checks them bit-exact against the oracle.  This is a logic check on the GPU-less build box; the -m gpu tests
-are the parity gate on a B200."""
+are the parity gate on an H100."""
 import os
 import subprocess
 

@@ -1,7 +1,7 @@
 """Runs the REAL zstd compressor/decompressor kernel sources under the test-only SIMT emulator (tests/simt/)
 through the C-ABI and checks them against the oracle (system libzstd): our frames decode with libzstd, libzstd's
 level-3 frames decode with ours, Frame_Content_Size is present, corrupt input is an error and never a crash.
-Logic check for the GPU-less build box; the -m gpu tests repeat this on a B200 at full sizes."""
+Logic check for the GPU-less build box; the -m gpu tests repeat this on an H100 at full sizes."""
 import json
 import os
 import subprocess
@@ -264,7 +264,7 @@ def test_simt_matches_that_end_at_the_block_end(ctx, mode):
 
 def test_simt_straight_line_extension_is_the_same_parse(tmp_path):
     # The per-lane match extension of the speed-mode compressor exists as a loop (ZB_TUNE_STRAIGHT=0, the code until round 2)
-    # and as straight-line branch-free code (=1, the product: profiles/r02_ab.md).  It is a restructuring, not a different
+    # and as straight-line branch-free code (=1, the product: faster on the GPU, see the ZB_TUNE_STRAIGHT note).  It is a restructuring, not a different
     # parse: with the emulator's fixed lane order both builds must emit identical frames.
     libs = {}
     for v in (0, 1):

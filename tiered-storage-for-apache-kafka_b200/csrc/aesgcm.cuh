@@ -1,4 +1,4 @@
-// aesgcm.cuh — batched AES-256-GCM for sm_100a (kernels K3/K4 of SURVEY.md §2a).
+// aesgcm.cuh — batched AES-256-GCM for sm_90a (kernels K3/K4 of SURVEY.md §2a).
 //
 // Replaces, per chunk, javax.crypto Cipher("AES/GCM/NoPadding").doFinal as called from
 //   core/M/transform/EncryptionChunkEnumeration.java:65-80   (layout IV(12) || CT || TAG(16))

@@ -4,7 +4,7 @@
 //   TransformedChunksSerializer      core/M/manifest/index/serde/TransformedChunksSerializer.java:30-52
 //   Fixed/VariableSizeChunkIndex JSON core/M/manifest/index/{FixedSizeChunkIndex,VariableSizeChunkIndex}.java,
 //                                    type tag core/M/manifest/index/ChunkIndex.java:36-42
-// (core/M = /root/reference/core/src/main/java/io/aiven/kafka/tieredstorage).
+// (core/M = <reference>/core/src/main/java/io/aiven/kafka/tieredstorage).
 #pragma once
 #include <stdint.h>
 #include <string>

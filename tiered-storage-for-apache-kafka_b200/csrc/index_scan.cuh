@@ -1,6 +1,6 @@
 // index_scan.cuh — K5: exclusive prefix sum of transformed chunk sizes -> transformed positions.
 // Replaces the serial loop of AbstractChunkIndex.materializeChunks
-// (/root/reference/core/src/main/java/io/aiven/kafka/tieredstorage/manifest/index/AbstractChunkIndex.java:52-72).
+// (<reference>/core/src/main/java/io/aiven/kafka/tieredstorage/manifest/index/AbstractChunkIndex.java:52-72).
 // One warp; 32 sizes per step through a shuffle scan with a 64-bit running carry (n = 256 for a 1 GiB segment).
 #pragma once
 #include "ts_common.cuh"

@@ -1,4 +1,4 @@
-// ts_common.cuh — shared device-side helpers for the sm_100a chunk-transform kernels.
+// ts_common.cuh — shared device-side helpers for the sm_90a chunk-transform kernels.
 //
 // The device headers are written in a restricted CUDA subset so that tests/simt/ (a TEST-ONLY fiber
 // emulator, never linked into libtsgpu.so) can also compile them with g++ to check kernel logic on

@@ -38,7 +38,7 @@ static int fail(int code, const char* fmt, ...) {
 #define CHECK_LAUNCH(what) do { const char* e_ = rt::last_error(); if (e_) return fail(TSGPU_E_CUDA, "launch %s: %s", what, e_); } while (0)
 
 extern "C" const char* tsgpu_last_error(void) { return g_err; }
-extern "C" const char* tsgpu_version(void) { return "tsgpu 0.1 (sm_100a)"; }
+extern "C" const char* tsgpu_version(void) { return "tsgpu 0.1 (sm_90a)"; }
 
 static inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 static inline uint64_t frame_bound(uint64_t n) { return n + (n >> 8) + 64; }   // >= header + 3 bytes per 8 KiB block

@@ -1,4 +1,4 @@
-// zstd_dec.cuh — batched Zstandard decompression for sm_100a (kernel K2 of SURVEY.md §2a).
+// zstd_dec.cuh — batched Zstandard decompression for sm_90a (kernel K2 of SURVEY.md §2a).
 //
 // Replaces Zstd.decompressedSize + Zstd.decompress as called per chunk from
 //   core/M/transform/DecompressionChunkEnumeration.java:38-46

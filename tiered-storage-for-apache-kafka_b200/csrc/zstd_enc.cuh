@@ -1,4 +1,4 @@
-// zstd_enc.cuh — batched Zstandard compression for sm_100a (kernel K1 of SURVEY.md §2a).
+// zstd_enc.cuh — batched Zstandard compression for sm_90a (kernel K1 of SURVEY.md §2a).
 //
 // Replaces ZstdCompressCtx.compress as called per chunk from
 //   core/M/transform/CompressionChunkEnumeration.java:49-62 (new ctx, default level, setPledgedSrcSize,
@@ -6,7 +6,7 @@
 // Parity bar (SURVEY.md §8c): libzstd decodes every frame to the original bytes and
 // ZSTD_getFrameContentSize(frame) == original size.  Compressed bytes are not expected to equal libzstd's.
 //
-// B200-first decomposition: a chunk is cut into REGIONS of 64 KiB that never reference each other, one CTA (8 warps) per
+// GPU-first decomposition: a chunk is cut into REGIONS of 64 KiB that never reference each other, one CTA (8 warps) per
 // region; a region is 8 zstd blocks of 8 KiB, one warp each.  A 1 GiB segment is 16,384 independent regions / 131,072
 // warps instead of 256 sequential frames.  Inside a region
 //   * matches reach back across the whole region (one 64 KiB window in shared memory): every slice has its own running
@@ -115,8 +115,8 @@ __device__ __forceinline__ void ze_put_bits(uint32_t* words, uint32_t o, uint64_
 // Hash-table insert where the HIGHEST position of the warp's step wins a shared slot — the hardware would keep an
 // arbitrary one, which made frames differ between runs; retried uploads must produce identical objects.  Lanes re-store
 // until no lower position is left in a slot: one round when the step has no slot collision, one more per extra peer.
-// (match.any would find the peers in one instruction but serialises on the number of distinct values: measured 20 ms per
-// GiB on random data; 32-bit slots would allow atomicMax but halve the table at equal shared memory: -1.7 % ratio.)
+// (match.any would find the peers in one instruction but serialises on the number of distinct values, which is slow on
+// random data; 32-bit slots would allow atomicMax but halve the table at equal shared memory: -1.7 % ratio.)
 #ifdef TSGPU_SIMT
 static inline unsigned __match_any_sync(unsigned, unsigned v) {
     simt::Warp& w = simt::g_blk->warps[simt::g_cur->warp];
@@ -318,7 +318,7 @@ __device__ __forceinline__ uint32_t ze_frame_header_size(uint32_t n) {
 // Decoupled look-back (Merrill & Garland's single-pass scan): a unit publishes its own SIZE as soon as it is known, then
 // walks back over its predecessors' words, 32 at a time, adding sizes until it meets one that already carries an inclusive
 // PREFIX; then it publishes its own prefix.  Nothing waits for a chain of prefixes to propagate unit by unit — a first
-// version did (each unit waited for its predecessor's prefix) and the 512-hop chain per chunk cost 13 ms per GiB.
+// version did (each unit waited for its predecessor's prefix) and the 512-hop chain per chunk nearly doubled the kernel's time.
 // Word: bits 62-63 = 0 empty / 1 size / 2 inclusive prefix, bits 0-61 the value.  Called by a whole warp.
 constexpr unsigned long long ZE_LB_SIZE = 1ull << 62, ZE_LB_PREFIX = 2ull << 62, ZE_LB_VALUE = (1ull << 62) - 1;
 __device__ __forceinline__ unsigned long long ze_lb_load(const unsigned long long* w) {

@@ -4,8 +4,8 @@
 // different trade: every 8 KiB block is self-contained (own Huffman tree, own FSE tables, no match leaves the block), so a
 // 1 GiB segment is 131,072 independent warps with no barrier between them, 20 warps per SM.  That is the round-1 kernel with
 // the streamlined FSE chains and the backwards growth of taken matches ("catch up"); it compresses the K corpus ~3.1 : 1 at
-// ~14.7 ms per GiB, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at ~27 ms per GiB (one 64 KiB window and one set
-// of tables per 8 blocks).  TSGPU_FLAG_ZSTD picks this kernel, TSGPU_FLAG_ZSTD | TSGPU_FLAG_ZSTD_DENSE the region kernel;
+// ~16.7 ms per GiB on an H100, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
+// window and one set of tables per 8 blocks).  TSGPU_FLAG_ZSTD picks this kernel, TSGPU_FLAG_ZSTD | TSGPU_FLAG_ZSTD_DENSE the region kernel;
 // the decoder reads both through the same region path (zstd_dec.cuh).
 //   zstd_enc_blocks_kernel    one WARP per block: block staged in shared memory; 32 positions hashed and verified per step
 //                             against a per-warp hash table, greedy left-to-right selection by ballot/ffs, match extension
@@ -22,20 +22,20 @@ namespace ts {
 constexpr int ZB_HLOG = 10;                    // per-warp hash table: 2^10 x u16 (position + 1)
 constexpr uint32_t ZB_HSIZE = 1u << ZB_HLOG;
 // ZB_TUNE_* exist for A/B runs on the GPU (scripts/ab_variants.sh builds one library per setting); the defaults are the product
-#ifndef ZB_TUNE_WPB
+#ifndef ZB_TUNE_WPB       // H100: 8 warps per CTA 19.0 ms per GiB, 4 warps 16.6, 2 warps 16.5 (within noise of 4)
 #define ZB_TUNE_WPB 4
 #endif
 #ifndef ZB_TUNE_LANE_EXT
 #define ZB_TUNE_LANE_EXT 12
 #endif
-#ifndef ZB_TUNE_BACK      // 1: taken matches grow backwards over up to 4 literals ("catch up"): +3.6 % ratio for +0.76 ms per GiB (measured)
+#ifndef ZB_TUNE_BACK      // 1: taken matches grow backwards over up to 4 literals ("catch up"): +3.6 % ratio for ~0.5 ms per GiB (H100)
 #define ZB_TUNE_BACK 1
 #endif
 #ifndef ZB_TUNE_STRAIGHT  // 1: per-lane match extension as straight-line code over 12 bytes instead of a divergent loop:
-#define ZB_TUNE_STRAIGHT 1 //   16.21 -> 14.72 ms per GiB on the B200 (the loop was 16 % of the kernel's stall samples; profiles/r02_ab.md)
+#define ZB_TUNE_STRAIGHT 1 //   18.1 -> 16.6 ms per GiB on an H100
 #endif
 #ifndef ZB_TUNE_EXTLDS    // 1: the warp-wide extension of long matches reads shared memory with LDS word pairs instead of generic loads
-#define ZB_TUNE_EXTLDS 0  //    (measured on the B200: 14.92 instead of 14.72 ms per GiB — off; profiles/r02_ab.md)
+#define ZB_TUNE_EXTLDS 0  //    (H100: within 1 % of the generic loads, 16.5 vs 16.6 ms per GiB — off)
 #endif
 constexpr int ZB_WPB = ZB_TUNE_WPB;            // warps (= blocks in flight) per CTA
 constexpr uint32_t ZB_LANE_EXT = ZB_TUNE_LANE_EXT;   // bytes a lane extends its own match beyond the first 4
@@ -541,7 +541,7 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
 #if ZB_TUNE_BACK
         // how many of the 4 bytes before the position also match (straight-line, all lanes: two loads, two funnel shifts):
         // a taken match grows backwards over the literals before it, libzstd's "catch up".  (A first version did this in a
-        // branch of the lanes with a verified candidate, through ld_u32_unaligned: 1.55 ms per GiB instead of 0.76.)
+        // branch of the lanes with a verified candidate, through ld_u32_unaligned, and was slower.)
         const uint32_t am = p >= 4 ? wp[-1] : 0u, cm = cand >= 4 ? wc[-1] : 0u;
         const uint32_t bkr = min((uint32_t)__clz((int)(__funnelshift_r(am, a0, shp) ^ __funnelshift_r(cm, c0, shc))) >> 3, min(cand, 4u));
 #else

@@ -1,7 +1,7 @@
 // zstd_format.h — RFC 8878 constants and FSE table construction shared by the compressor and decompressor.
 //
 // The reference reaches this format through com.github.luben:zstd-jni:1.5.6-9 (libzstd 1.5.6), which is not in
-// /root/reference; the call sites are core/M/transform/CompressionChunkEnumeration.java:52-61 and
+// the reference repository; the call sites are core/M/transform/CompressionChunkEnumeration.java:52-61 and
 // core/M/transform/DecompressionChunkEnumeration.java:41-45.  Everything here restates the published format
 // (RFC 8878 §3.1.1.3-§3.1.1.5, §4.1): code tables, default distributions, FSE spread/state tables.
 #pragma once

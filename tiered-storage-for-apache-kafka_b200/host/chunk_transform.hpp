@@ -6,9 +6,9 @@
 //   core/M/manifest/index/{AbstractChunkIndexBuilder,FixedSizeChunkIndexBuilder,VariableSizeChunkIndexBuilder}.java,
 //   core/M/manifest/index/{AbstractChunkIndex,FixedSizeChunkIndex,VariableSizeChunkIndex}.java, core/M/Chunk.java,
 //   core/M/fetch/FetchChunkEnumeration.java
-// (core/M = /root/reference/core/src/main/java/io/aiven/kafka/tieredstorage).
+// (core/M = <reference>/core/src/main/java/io/aiven/kafka/tieredstorage).
 //
-// Difference that makes it B200-native: the reference pulls ONE chunk through the decorator chain per
+// Difference that makes it GPU-native: the reference pulls ONE chunk through the decorator chain per
 // nextElement(); here the outermost enumeration pulls a BATCH of original chunks from the base enumeration,
 // hands the whole batch to tsgpu_transform / tsgpu_detransform once, and then serves the results one at a time.
 // The decorators only contribute their flag, key material and transformedChunkSize() arithmetic.

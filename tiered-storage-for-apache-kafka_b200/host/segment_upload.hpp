@@ -9,7 +9,7 @@
 // (M = src/main/java/io/aiven/kafka/tieredstorage.)
 //
 // The record-batch layout and its checksums live in kafka-clients 3.6.0 (build.gradle:110), which is not vendored in
-// /root/reference; they are restated here from the published Kafka message format:
+// the reference repository; they are restated here from the published Kafka message format:
 //   v2:  baseOffset i64 | batchLength i32 | partitionLeaderEpoch i32 | magic i8 (=2) | crc u32 (CRC-32C of everything
 //        after it) | attributes i16 (bits 0-2 = compression codec) | ... 61 bytes of header in all
 //   v0/v1: offset i64 | size i32 | crc u32 (CRC-32 of everything after it) | magic i8 | attributes i8 (bits 0-2) | ...
@@ -153,7 +153,7 @@ inline std::vector<UploadPart> multipartPlan(uint64_t objectBytes, uint64_t part
     return parts;
 }
 
-// RemoteStorageManager.uploadSegmentLog, B200 shape: the whole segment goes through ONE tsgpu_transform call (batches are
+// RemoteStorageManager.uploadSegmentLog, GPU shape: the whole segment goes through ONE tsgpu_transform call (batches are
 // pipelined inside), the packed object lands in a pinned buffer, and the uploader is handed finished parts of that
 // buffer — it never pulls a stream through the transform.  The rate limiter is charged per part, as the reference's
 // stream is charged per read(buf, off, len).
