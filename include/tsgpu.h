@@ -59,10 +59,8 @@ const char* tsgpu_version(void);
  * A host-buffer call (tsgpu_transform / tsgpu_detransform) cuts its chunks into batches of `max_batch` and keeps up to
  * 8 of them in flight per device (work slots, allocated on first use; each has a compute stream and a copy-out stream).
  * With 4 MiB chunks `max_batch = 4` measured best through PCIe; device-resident callers pass whole segments.
- * Environment (read once by tsgpu_create; tuning only): TSGPU_SLOTS=1..16 slots per device, TSGPU_SPLIT_OUT=0 puts the
- * copies-out back on the compute stream, TSGPU_ZSTD_MODE=dense makes TSGPU_FLAG_ZSTD_DENSE the context's default.
- * (Round 1's opt-in variants are gone: the per-block entropy stage for libzstd-shaped frames is the only general decode
- * path now, the two-launch compressor was deleted.)
+ * Environment (read once by tsgpu_create; tuning only): TSGPU_SLOTS=1..16 slots per device, TSGPU_ZSTD_MODE=dense makes
+ * TSGPU_FLAG_ZSTD_DENSE the context's default.
  * --------------------------------------------------------------------------------------------------------- */
 int  tsgpu_create(const int* device_ids, int n_devices, uint32_t max_chunk_bytes, uint32_t max_batch,
                   tsgpu_ctx** out);

@@ -12,9 +12,9 @@ src = corpus.gen_segment(kind, 0, seg, cs)
 h_src = torch.empty(seg, dtype=torch.uint8).pin_memory(); h_src.numpy()[:] = src
 key, aad, ivs = corpus.fixed_key_material(nch)
 import os
-for flags, slots, split, mb in ((3, 16, 1, 4), (3, 16, 1, 8), (3, 16, 1, 2), (3, 16, 1, 16), (3, 16, 0, 4), (7, 16, 1, 4), (1, 16, 1, 4), (2, 16, 1, 4), (2, 16, 1, 8)):
+for flags, slots, mb in ((3, 16, 4), (3, 16, 8), (3, 16, 2), (3, 16, 16), (7, 16, 4), (1, 16, 4), (2, 16, 4), (2, 16, 8)):
     if True:
-        os.environ['TSGPU_SLOTS'] = str(slots); os.environ['TSGPU_SPLIT_OUT'] = str(split)
+        os.environ['TSGPU_SLOTS'] = str(slots)
         ctx = tsgpu.Context(max_chunk_bytes=cs, max_batch=mb)
         cap = int(ctx.lib.tsgpu_transform_bound(flags, seg, cs)) + 64
         h_dst = torch.empty(cap, dtype=torch.uint8).pin_memory(); d = h_dst.numpy()
@@ -22,7 +22,7 @@ for flags, slots, split, mb in ((3, 16, 1, 4), (3, 16, 1, 8), (3, 16, 1, 2), (3,
         torch.cuda.synchronize(); t0 = time.perf_counter()
         for _ in range(4): out, sizes = ctx.transform(flags, h_src.numpy(), cs, key, aad, ivs, dst=d)
         torch.cuda.synchronize(); dt = (time.perf_counter() - t0) / 4
-        print('flags', flags, 'slots', slots, 'split', split, 'batch', mb, 'e2e %.1f GiB/s' % (1.0 / dt), 'out MiB', sum(sizes) // MIB, flush=True)
+        print('flags', flags, 'slots', slots, 'batch', mb, 'e2e %.1f GiB/s' % (1.0 / dt), 'out MiB', sum(sizes) // MIB, flush=True)
         ctx.close(); del h_dst
 # raw copy ceilings
 d_buf = torch.empty(seg, dtype=torch.uint8, device='cuda')

@@ -48,6 +48,7 @@ namespace {
 
 constexpr int NSLOT_MAX = 16;       // work slots per device; tsgpu_ctx::nslot of them are used
 constexpr uint32_t MAX_AAD = 4096;
+constexpr uint32_t KNOWN_FLAGS = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE;
 
 struct Desc {            // device-side descriptor block of one work slot (all arrays sized for max_batch)
     uint64_t* a_off; uint64_t* b_off; uint64_t* c_off;
@@ -62,7 +63,7 @@ struct Work {
     rt::event_t ev_dev_desc{}, ev_dev_done{};   // device API: descriptor upload of / end of the previous call on this slot
     bool dev_pending = false;
     bool out_pending = false;              // a copy-out on out_stream still reads this slot's final buffer
-    bool busy = false, ready = false;
+    bool ready = false;
     bool claimed = false;                  // owned by a call in progress (guarded by tsgpu_ctx::mu)
     Aes256RoundKeys key_rk{};      // the key this slot's GcmKeyCtx (H powers, Shoup table) was built for
     bool key_valid = false;        //   ... consecutive calls with one segment's data key skip the set-up kernel
@@ -78,8 +79,6 @@ struct Work {
     ZstdBlkScratch zblk{};         // block kernel (default), allocated on first use
     ZstdDecScratch zdec{};
     uint32_t* h_sizes = nullptr;   // pinned: sizes/status coming back
-    // bookkeeping of the batch currently owning this slot
-    uint32_t c0 = 0, nb = 0;
 };
 
 struct Lane { int device = 0; Work w[NSLOT_MAX]; };
@@ -96,7 +95,6 @@ struct tsgpu_ctx {
     uint64_t frame_stride = 0, slot_stride = 0;
     LaunchProf prof;
     uint32_t nslot = 16;           // work slots per device (TSGPU_SLOTS overrides); one call takes at most 8 of them
-    bool split_out = true;         // copies-out ride their own stream (the slot's next batch starts behind an event, not behind them)
 };
 
 static void carve_desc(uint8_t* base, uint32_t nb, Desc& d, size_t* total) {
@@ -195,17 +193,14 @@ extern "C" int tsgpu_create(const int* device_ids, int n_devices, uint32_t max_c
     if (!c) return fail(TSGPU_E_NOMEM, "out of memory");
     c->chunk_cap = max_chunk_bytes; c->max_batch = max_batch;
     if (const char* e = getenv("TSGPU_SLOTS")) { int v = atoi(e); if (v >= 1 && v <= NSLOT_MAX) c->nslot = (uint32_t)v; }       // tuning knobs
-    if (const char* e = getenv("TSGPU_SPLIT_OUT")) c->split_out = atoi(e) != 0;
     if (const char* e = getenv("TSGPU_ZSTD_MODE")) c->dense_default = strcmp(e, "dense") == 0;
     c->frame_stride = align_up(frame_bound(max_chunk_bytes), 16) + 16;
     c->slot_stride = tsgpu_slot_stride(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES, max_chunk_bytes);
     c->lanes.resize(ids.size());
-    for (size_t l = 0; l < ids.size(); l++) {
+    for (size_t l = 0; l < ids.size(); l++) {           // slot 0 now, the others on first use (claim_slots)
         c->lanes[l].device = ids[l];
-        for (int s = 0; s < 1; s++) {                   // further slots are allocated on first use (work_ready)
-            int rc = work_init(c, c->lanes[l].w[s], ids[l]);
-            if (rc) { tsgpu_destroy(c); return rc; }
-        }
+        int rc = work_init(c, c->lanes[l].w[0], ids[l]);
+        if (rc) { tsgpu_destroy(c); return rc; }
     }
     for (size_t l = 0; l < ids.size(); l++) {           // opt in to > 48 KiB dynamic shared memory, per device
         rt::set_device(ids[l]);
@@ -233,11 +228,27 @@ extern "C" void* tsgpu_host_alloc(size_t bytes) {
 extern "C" void tsgpu_host_free(void* p) { rt::free_host(p); }
 extern "C" uint64_t tsgpu_launch_count(const tsgpu_ctx* c) { return c ? c->prof.launches.load() : 0; }
 
-// ------------------------------------------------------------------------------------------ zstd stage (compress)
-// Two kernels, one contract (zstd_enc_blk.cuh: independent 8 KiB blocks, fastest; zstd_enc.cuh: 64 KiB regions with shared
-// tables and history, densest).  Their scratch is allocated the first time a slot runs the mode.
-static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, const uint8_t* in_base, const uint64_t* d_in_off,
-                      const uint32_t* d_in_len, uint32_t nb, uint32_t cs, uint8_t* out_base, const uint64_t* d_out_off, uint32_t* d_out_len) {
+// ------------------------------------------------------------------------------------------ stages
+// A batch's chunks in one device buffer: chunk i is len[i] bytes at base + off[i] (off/len are device arrays).
+namespace {
+struct ChunksIn { const uint8_t* base; const uint64_t* off; const uint32_t* len; };
+struct ChunksOut {
+    uint8_t* base; uint64_t* off; uint32_t* len;
+    operator ChunksIn() const { return {base, off, len}; }
+};
+// Per-chunk limits of the decrypt / decompress kernels.  Sizes of transformed chunks come from outside (a manifest): the
+// kernels refuse a chunk that would overrun a buffer and report it in the status array.
+struct DxBounds {
+    uint32_t max_in;     // largest transformed chunk (sizes the GCM grid)
+    uint32_t aes_room;   // plaintext bytes the GCM stage may write per chunk
+    uint32_t zstd_in;    // frame bytes the zstd stage may read per chunk
+    uint32_t zstd_out;   // original bytes per chunk
+};
+}
+
+// zstd compress.  Two kernels, one contract (zstd_enc_blk.cuh: independent 8 KiB blocks, fastest; zstd_enc.cuh: 64 KiB
+// regions with shared tables and history, densest).  Their scratch is allocated the first time a slot runs the mode.
+static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, ChunksIn in, uint32_t nb, uint32_t cs, ChunksOut out) {
     const bool dense = (flags & TSGPU_FLAG_ZSTD_DENSE) || c->dense_default;
     int rc;
     if (dense) {
@@ -245,37 +256,38 @@ static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, co
             const char* e = zstd_enc_scratch_alloc(w.zenc, c->chunk_cap, c->max_batch);
             if (e) { zstd_enc_scratch_free(w.zenc); return fail(TSGPU_E_CUDA, "zstd enc scratch: %s", e); }
         }
-        rc = zstd_compress_batch(w.zenc, st, in_base, d_in_off, d_in_len, nb, cs, out_base, d_out_off, d_out_len, c->prof);
+        rc = zstd_compress_batch(w.zenc, st, in.base, in.off, in.len, nb, cs, out.base, out.off, out.len, c->prof);
     } else {
         if (!w.zblk.seqs) {
             const char* e = zstd_blk_scratch_alloc(w.zblk, c->chunk_cap, c->max_batch);
             if (e) { zstd_blk_scratch_free(w.zblk); return fail(TSGPU_E_CUDA, "zstd enc scratch: %s", e); }
         }
-        rc = zstd_compress_batch_blocks(w.zblk, st, in_base, d_in_off, d_in_len, nb, cs, out_base, d_out_off, d_out_len, c->prof);
+        rc = zstd_compress_batch_blocks(w.zblk, st, in.base, in.off, in.len, nb, cs, out.base, out.off, out.len, c->prof);
     }
     if (rc) return fail(rc, "zstd compress: %s", zstd_last_error());
     return TSGPU_OK;
 }
 
-// ------------------------------------------------------------------------------------------ AES-GCM stage
-// Runs key set-up (once per call and work slot), the main kernel over (ranges x chunks) and the finalize kernel.
+// AES-GCM: key set-up, the main kernel over (ranges x chunks) and the finalize kernel.  IVs (ENC) and AAD come from the
+// slot's descriptor block.  The slot keeps the key tables of the last key it ran: consecutive calls with one segment's data
+// key skip the set-up kernel.  Host and device calls share slot 0's tables; that is safe because device calls are ordered
+// behind each other by events (dev_call_begin) and a host call takes the slot only once device work on it has completed.
 template <bool ENC>
-static int gcm_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Aes256RoundKeys& rk, bool key_ready,
-                     const uint8_t* in_base, const uint64_t* d_in_off, const uint32_t* d_in_len,
-                     uint8_t* out_base, const uint64_t* d_out_off, uint32_t* d_out_len,
-                     const uint8_t* d_ivs, const uint8_t* d_aad, uint32_t aad_len, uint32_t* d_status,
-                     uint32_t n_chunks, uint32_t max_payload, uint4* d_partials, uint32_t max_ranges, uint32_t out_cap = 0xffffffffu) {
+static int gcm_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Aes256RoundKeys& rk, ChunksIn in, ChunksOut out,
+                     uint32_t aad_len, uint32_t* d_status, uint32_t n_chunks, uint32_t max_payload, uint32_t out_cap) {
+    const bool key_ready = w.key_valid && memcmp(&w.key_rk, &rk, sizeof rk) == 0;
+    w.key_rk = rk; w.key_valid = false;                      // valid again once the whole stage has been enqueued
     if (!key_ready) {
         TS_LAUNCH_P(c->prof, "gcm_key_setup", gcm_key_setup_kernel, dim3(1), dim3(GH_T), 0, st, rk, w.d_keyctx);
         CHECK_LAUNCH("gcm_key_setup_kernel");
     }
     GcmBatch B;
-    B.in_base = in_base; B.in_off = d_in_off; B.in_len = d_in_len;
-    B.out_base = out_base; B.out_off = d_out_off; B.out_len = d_out_len;
-    B.ivs = d_ivs; B.aad = d_aad; B.aad_len = aad_len;
-    B.partials = d_partials; B.max_ranges = max_ranges; B.status = d_status; B.n_chunks = n_chunks; B.out_cap = out_cap;
+    B.in_base = in.base; B.in_off = in.off; B.in_len = in.len;
+    B.out_base = out.base; B.out_off = out.off; B.out_len = out.len;
+    B.ivs = ENC ? w.dd.ivs : nullptr; B.aad = w.dd.aad; B.aad_len = aad_len;
+    B.partials = w.d_partials; B.max_ranges = w.max_ranges; B.status = d_status; B.n_chunks = n_chunks; B.out_cap = out_cap;
     uint32_t ranges = (uint32_t)(((uint64_t)max_payload + 15) / 16 + GH_RANGE_BLOCKS - 1) / GH_RANGE_BLOCKS;
-    if (ranges > max_ranges) return fail(TSGPU_E_ARG, "chunk too large for this context");
+    if (ranges > w.max_ranges) return fail(TSGPU_E_ARG, "chunk too large for this context");
     if (ranges) {
         TS_LAUNCH_P(c->prof, ENC ? "gcm_main_enc" : "gcm_main_dec", gcm_main_kernel<ENC>, dim3(ranges, n_chunks), dim3(GH_T),
                     GCM_SMEM_BYTES, st, rk, w.d_keyctx, B);
@@ -284,6 +296,7 @@ static int gcm_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Aes256RoundKe
     TS_LAUNCH_P(c->prof, ENC ? "gcm_finalize_enc" : "gcm_finalize_dec", gcm_finalize_kernel<ENC>, dim3((n_chunks + 3) / 4),
                 dim3(128), 0, st, rk, w.d_keyctx, B);
     CHECK_LAUNCH("gcm_finalize_kernel");
+    w.key_valid = true;
     return TSGPU_OK;
 }
 
@@ -291,6 +304,46 @@ static int gcm_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Aes256RoundKe
 // out_stream; the first kernel that overwrites the buffer they are read from waits for them here.
 static int wait_copies_out(Work& w, rt::stream_t st) {
     if (w.out_pending) { RT(rt::stream_wait_event(st, w.ev_done)); w.out_pending = false; }
+    return TSGPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------ stage chains
+// Used by the host-buffer and the device-resident calls alike; the caller has filled and uploaded the descriptor block.
+// Between the two stages the chunks sit in the slot's frame buffer (16-byte aligned slots of frame_stride).
+
+// [zstd ->] [AES-GCM encrypt]: nb chunks of at most cs bytes from `src` into `dst`.
+static int transform_enqueue(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, uint32_t nb, uint32_t cs,
+                             const Aes256RoundKeys& rk, uint32_t aad_len, ChunksIn src, ChunksOut dst) {
+    const bool aes = flags & TSGPU_FLAG_AES;
+    uint32_t max_payload = cs;
+    if (flags & TSGPU_FLAG_ZSTD) {
+        const ChunksOut frames = aes ? ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len} : dst;
+        int rc = zstd_stage(c, w, st, flags, src, nb, cs, frames);
+        if (rc) return rc;
+        src = frames; max_payload = (uint32_t)frame_bound(cs);
+    }
+    if (aes) return gcm_stage<true>(c, w, st, rk, src, dst, aad_len, w.dd.status, nb, max_payload, 0xffffffffu);
+    return TSGPU_OK;
+}
+
+// [AES-GCM decrypt ->] [zstd]: nb chunks from `src` into `dst`.  packed: dst.off is written on the device as the running sum
+// of the original sizes (chunks back to back) instead of being read as given.
+static int detransform_enqueue(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, uint32_t nb, const Aes256RoundKeys& rk,
+                               uint32_t aad_len, ChunksIn src, ChunksOut dst, uint32_t* d_status, const DxBounds& lim, bool packed) {
+    const bool zstd = flags & TSGPU_FLAG_ZSTD;
+    if (flags & TSGPU_FLAG_AES) {
+        const ChunksOut plain = zstd ? ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len} : dst;
+        if (!zstd) { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }                        // dst is the final buffer
+        int rc = gcm_stage<false>(c, w, st, rk, src, plain, aad_len, d_status, nb, lim.max_in, lim.aes_room);
+        if (rc) return rc;
+        src = plain;
+    }
+    if (zstd) {
+        { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
+        int rc = zstd_decompress_batch(w.zdec, st, src.base, src.off, src.len, nb, lim.zstd_out, dst.base, dst.off, dst.len,
+                                       d_status, packed, c->prof, lim.zstd_in);
+        if (rc) return fail(rc, "zstd decompress: %s", zstd_last_error());
+    }
     return TSGPU_OK;
 }
 
@@ -363,21 +416,71 @@ static int claim_slots(tsgpu_ctx* c, uint32_t want, SlotClaim& claim, int only_d
     return TSGPU_OK;
 }
 
-// ------------------------------------------------------------------------------------------ transform (host)
+// ------------------------------------------------------------------------------------------ batches (host-buffer calls)
 namespace {
-struct XfBatch {            // one in-flight transform batch
-    Work* w; uint32_t c0, nb;
-    const uint8_t* final_base; uint64_t final_stride; uint32_t final_head;
-};
+struct Batch { Work* w; uint32_t c0, nb; };      // chunks [c0, c0 + nb) of a call, in flight on slot w
 }
 
+// Cuts n chunks into batches of max_batch and deals them round-robin over the slots it claims.  issue(batch) enqueues a
+// batch on its slot's stream and ends with the D2H of its sizes (ev_sizes); drain(batch) runs once those sizes are on the
+// host, in batch order, and sends the batch's bytes home (copy_out).  Returns with every claimed slot idle.
+template <class Issue, class Drain>
+static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain) {
+    const uint32_t nbatches = (n + c->max_batch - 1) / c->max_batch;
+    SlotClaim claim;
+    { int rcc = claim_slots(c, nbatches, claim); if (rcc) return rcc; }
+    const uint32_t nwork = (uint32_t)claim.slots.size();
+    std::vector<Batch> inflight(nbatches);
+    uint32_t drained = 0;
+    auto drain_next = [&]() -> int {
+        const Batch& bt = inflight[drained++];
+        RT(rt::set_device(bt.w->device));
+        RT(rt::event_sync(bt.w->ev_sizes));
+        return drain(bt);
+    };
+    int rc = TSGPU_OK;
+    for (uint32_t b = 0; b < nbatches && rc == TSGPU_OK; b++) {
+        // From b = nwork on a slot is reused: its previous batch is drained first (sizes read on the host, copies-out
+        // enqueued on the slot's out_stream); the new batch's copy-in and first kernels start right away and only the
+        // kernel that overwrites the buffer being copied out waits for those copies (wait_copies_out) — the host never
+        // waits here, which keeps all slots' queues full.
+        if (b >= nwork) { rc = drain_next(); if (rc) break; }
+        const uint32_t c0 = b * c->max_batch;
+        inflight[b] = Batch{claim.slots[b % nwork], c0, std::min(c->max_batch, n - c0)};
+        rc = issue(inflight[b]);
+    }
+    while (rc == TSGPU_OK && drained < nbatches) rc = drain_next();
+    for (Work* w : claim.slots) {                    // always leave the claimed slots idle
+        rt::set_device(w->device);
+        const char* e = rt::stream_sync(w->stream);
+        if (!e) e = rt::stream_sync(w->out_stream);
+        if (e && rc == TSGPU_OK) rc = fail(TSGPU_E_CUDA, "stream_sync: %s", e);
+        w->out_pending = false;
+    }
+    return rc;
+}
+
+// A drained batch's `total` bytes at `from` go to dst + dst_off on the slot's copy-out stream (the sizes event has
+// completed: there is nothing to order them behind).
+static int copy_out(Work& w, const uint8_t* from, uint64_t total, uint8_t* dst, uint64_t dst_cap, uint64_t& dst_off) {
+    if (dst_off + total > dst_cap) return fail(TSGPU_E_SHORT, "dst too small");
+    if (total) RT(rt::d2h(dst + dst_off, from, total, w.out_stream));
+    dst_off += total;
+    RT(rt::event_record(w.ev_done, w.out_stream));
+    w.out_pending = true;
+    return TSGPU_OK;
+}
+
+// ------------------------------------------------------------------------------------------ transform (host)
+// One batch: copy in, fill the descriptors, enqueue the stages, pack the transformed chunks, D2H of their sizes.
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
-static int transform_issue(tsgpu_ctx* c, Work& w, uint32_t flags, const uint8_t* src, const uint64_t* off, const uint32_t* len,
-                           uint32_t cs, uint32_t c0, uint32_t nb, const Aes256RoundKeys& rk,
-                           const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, XfBatch& xb) {
+static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const uint8_t* src, const uint64_t* off,
+                           const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
+                           const uint8_t* ivs) {
+    Work& w = *bt.w;
+    const uint32_t c0 = bt.c0, nb = bt.nb;
     RT(rt::set_device(w.device));
     rt::stream_t st = w.stream;
-    w.busy = true;                                       // from here on the caller must drain this slot's streams before returning
     const uint64_t byte0 = off[c0];
     const uint64_t byte1 = off[c0 + nb - 1] + len[c0 + nb - 1];
     RT(rt::h2d(w.d_orig, src + byte0, byte1 - byte0, st));
@@ -388,45 +491,28 @@ static int transform_issue(tsgpu_ctx* c, Work& w, uint32_t flags, const uint8_t*
         w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
         w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
     }
-    if (flags & TSGPU_FLAG_AES) {
+    const bool aes = flags & TSGPU_FLAG_AES;
+    if (aes) {
         memcpy(w.hd.ivs, ivs + (size_t)c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
         if (aad_len) memcpy(w.hd.aad, aad, aad_len);
     }
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
-
-    const uint8_t* cur_base = w.d_orig; const uint64_t* cur_off = w.dd.a_off; const uint32_t* cur_len = w.dd.a_len;
-    uint32_t cur_max = cs;
-    xb.final_base = w.d_orig; xb.final_stride = cs; xb.final_head = 0;
-    if (flags & TSGPU_FLAG_ZSTD) {
-        int rc = zstd_stage(c, w, st, flags, cur_base, cur_off, cur_len, nb, cs, w.d_frames, w.dd.b_off, w.dd.b_len);
-        if (rc) return rc;
-        cur_base = w.d_frames; cur_off = w.dd.b_off; cur_len = w.dd.b_len; cur_max = (uint32_t)frame_bound(cs);
-        xb.final_base = w.d_frames; xb.final_stride = c->frame_stride; xb.final_head = 0;
-    }
-    if (flags & TSGPU_FLAG_AES) {
-        const bool key_ready = w.key_valid && memcmp(&w.key_rk, &rk, sizeof rk) == 0;
-        w.key_rk = rk; w.key_valid = false;                  // valid again once the stage has been enqueued
-        int rc = gcm_stage<true>(c, w, st, rk, key_ready, cur_base, cur_off, cur_len, w.d_xf, w.dd.c_off, w.dd.c_len,
-                                 w.dd.ivs, w.dd.aad, aad_len, w.dd.status, nb, cur_max, w.d_partials, w.max_ranges);
-        if (rc) return rc;
-        w.key_valid = true;
-        cur_len = w.dd.c_len;
-        xb.final_base = w.d_xf; xb.final_stride = c->slot_stride; xb.final_head = TSGPU_SLOT_HEAD;
-    }
+    // encrypted chunks land in the transformed slots; zstd alone leaves its frames in the frame slots
+    const ChunksOut fin = aes ? ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len} : ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len};
+    { int rc = transform_enqueue(c, w, st, flags, nb, cs, rk, aad_len, ChunksIn{w.d_orig, w.dd.a_off, w.dd.a_len}, fin); if (rc) return rc; }
     // the transformed chunks, back to back, so the batch leaves in one copy (the previous batch's copy-out may still be
     // reading d_pack: this is the first kernel of the batch that has to wait for it)
     { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
     {
         PackArgs P;
-        P.base = xb.final_base; P.stride = xb.final_stride; P.head = xb.final_head; P.len = cur_len; P.n = nb; P.out = w.d_pack;
+        P.base = fin.base; P.stride = aes ? c->slot_stride : c->frame_stride; P.head = aes ? TSGPU_SLOT_HEAD : 0;
+        P.len = fin.len; P.n = nb; P.out = w.d_pack;
         const uint64_t longest = (flags & TSGPU_FLAG_ZSTD) ? frame_bound(cs) + 28 : (uint64_t)cs + 28;
         TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
         CHECK_LAUNCH("pack_chunks_kernel");
     }
-    RT(rt::d2h(w.h_sizes, cur_len, 4ull * nb, st));
+    RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
-    xb.w = &w; xb.c0 = c0; xb.nb = nb;
-    w.busy = true;
     return TSGPU_OK;
 }
 
@@ -439,7 +525,7 @@ static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
     if (!n_chunks || !transformed_sizes) return fail(TSGPU_E_ARG, "transformed_sizes/n_chunks cannot be null");
     if (src_len && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
-    if (flags & ~(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
+    if (flags & ~KNOWN_FLAGS) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if ((flags & TSGPU_FLAG_AES) && (!key || !ivs)) return fail(TSGPU_E_ARG, "key and ivs are required for encryption");
     if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
     if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
@@ -503,75 +589,38 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
     Aes256RoundKeys rk{};
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
 
-    const uint32_t nbatches = (n + c->max_batch - 1) / c->max_batch;
-    SlotClaim claim;
-    { int rcc = claim_slots(c, nbatches, claim); if (rcc) return rcc; }
-    const uint32_t nwork = (uint32_t)claim.slots.size();
-    std::vector<XfBatch> inflight(nbatches);
     uint64_t dst_off = 0;
-    int rc = TSGPU_OK;
-    auto work_of = [&](uint32_t b) -> Work& { return *claim.slots[b % nwork]; };
-    auto drain = [&](uint32_t b) -> int {        // sizes of batch b are ready -> copy its chunks out, in order
-        XfBatch& xb = inflight[b];
-        Work& w = *xb.w;
-        RT(rt::set_device(w.device));
-        RT(rt::event_sync(w.ev_sizes));
-        rt::stream_t os = c->split_out ? w.out_stream : w.stream;    // the sizes event has completed: nothing to order on out_stream
-        uint64_t total = 0;
-        for (uint32_t i = 0; i < xb.nb; i++) { transformed_sizes[xb.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
-        if (dst_off + total > dst_cap) return fail(TSGPU_E_SHORT, "dst too small");
-        if (total) RT(rt::d2h(dst + dst_off, w.d_pack, total, os));  // one copy per batch: the chunks were packed on the device
-        dst_off += total;
-        RT(rt::event_record(w.ev_done, os));
-        w.out_pending = c->split_out;
-        return TSGPU_OK;
-    };
-    uint32_t drained = 0;
-    for (uint32_t b = 0; b < nbatches && rc == TSGPU_OK; b++) {
-        if (b >= nwork) {
-            // The slot is reused.  Its previous batch has been drained (sizes read on the host, copies-out enqueued on
-            // the slot's out_stream); the new batch's copy-in and first kernels start right away and only the kernel
-            // that overwrites the buffer being copied out waits for those copies (wait_copies_out) — the host never
-            // waits here, which keeps all slots' queues full.
-            if (drained <= b - nwork) { rc = drain(drained++); if (rc) break; }
-        }
-        uint32_t c0 = b * c->max_batch, nb = std::min(c->max_batch, n - c0);
-        rc = transform_issue(c, work_of(b), flags, src, off.data(), len.data(), cs, c0, nb, rk, aad, aad_len, ivs, inflight[b]);
-    }
-    while (rc == TSGPU_OK && drained < nbatches) rc = drain(drained++);
-    for (Work* wp : claim.slots) if (wp->busy) {                 // always leave the claimed slots idle
-        Work& w = *wp;
-        rt::set_device(w.device);
-        const char* e = rt::stream_sync(w.stream);
-        if (!e) e = rt::stream_sync(w.out_stream);
-        if (e && rc == TSGPU_OK) rc = fail(TSGPU_E_CUDA, "stream_sync: %s", e);
-        w.busy = false; w.out_pending = false;
-    }
+    const int rc = run_batches(c, n,
+        [&](const Batch& bt) { return transform_issue(c, bt, flags, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
+        [&](const Batch& bt) {
+            Work& w = *bt.w;
+            uint64_t total = 0;
+            for (uint32_t i = 0; i < bt.nb; i++) { transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
+            return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);     // one copy per batch: packed on the device
+        });
     if (rc) return rc;
     *n_chunks = n;
     return TSGPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------ detransform (host)
-namespace {
-struct DxBatch { Work* w; uint32_t c0, nb; uint64_t in_bytes; };
-}
-
-static int detransform_issue(tsgpu_ctx* c, Work& w, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
-                             uint32_t c0, uint32_t nb, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
-                             DxBatch& db) {
+// One batch: bound the sizes, copy the chunks in, fill the descriptors, enqueue the stages, D2H of sizes and status.
+// `src`: the batch's first transformed chunk.
+static int detransform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
+                             const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len) {
+    Work& w = *bt.w;
+    const uint32_t c0 = bt.c0, nb = bt.nb;
     RT(rt::set_device(w.device));
     rt::stream_t st = w.stream;
-    w.busy = true;
+    // Sizes come from a manifest, i.e. from outside: bound them per mode BEFORE any kernel writes (the GCM kernel
+    // releases plaintext into the next buffer before the tag is checked).  AES only: plaintext lands in d_orig
+    // (chunk_cap per chunk); AES+zstd: in a d_frames slot; zstd only: the frame is read in place from d_xf.
+    const uint32_t room = (flags & TSGPU_FLAG_ZSTD) ? (uint32_t)(c->frame_stride - 16) : c->chunk_cap;
     uint64_t ip = 0, op = 0;
     uint32_t max_t = 0;
     for (uint32_t i = 0; i < nb; i++) {
         const uint32_t t = tsizes[c0 + i];
-        // Sizes come from a manifest, i.e. from outside: bound them per mode BEFORE any kernel writes (the GCM kernel
-        // releases plaintext into the next buffer before the tag is checked).  AES only: plaintext lands in d_orig
-        // (chunk_cap per chunk); AES+zstd: in a d_frames slot; zstd only: the frame is read in place from d_xf.
         const uint64_t payload = (flags & TSGPU_FLAG_AES) ? (t >= 28 ? t - 28 : 0) : t;
-        const uint64_t room = (flags & TSGPU_FLAG_ZSTD) ? c->frame_stride - 16 : c->chunk_cap;
         if (payload > room || t > c->slot_stride - TSGPU_SLOT_HEAD - 16)
             return fail(TSGPU_E_ARG, "transformed chunk of %u bytes exceeds the context's capacity", t);
         w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
@@ -580,40 +629,18 @@ static int detransform_issue(tsgpu_ctx* c, Work& w, uint32_t flags, const uint8_
         w.hd.a_off[i] = op;                              // used when there is no zstd stage (sizes are known)
         if (t) RT(rt::h2d(w.d_xf + w.hd.c_off[i], src + ip, t, st));
         ip += t;
-        op += (flags & TSGPU_FLAG_AES) ? (t >= 28 ? t - 28 : 0) : t;
+        op += payload;
         max_t = std::max(max_t, t);
     }
     if ((flags & TSGPU_FLAG_AES) && aad_len) memcpy(w.hd.aad, aad, aad_len);
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
     RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
-
-    const uint8_t* cur_base = w.d_xf; const uint64_t* cur_off = w.dd.c_off; const uint32_t* cur_len = w.dd.c_len;
-    if (flags & TSGPU_FLAG_AES) {
-        const bool z = flags & TSGPU_FLAG_ZSTD;
-        uint8_t* ob = z ? w.d_frames : w.d_orig;
-        const uint64_t* oo = z ? w.dd.b_off : w.dd.a_off;
-        uint32_t* ol = z ? w.dd.b_len : w.dd.a_len;
-        const bool key_ready = w.key_valid && memcmp(&w.key_rk, &rk, sizeof rk) == 0;
-        w.key_rk = rk; w.key_valid = false;                  // valid again once the stage has been enqueued
-        if (!z) { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }                          // d_orig is the final buffer
-        int rc = gcm_stage<false>(c, w, st, rk, key_ready, cur_base, cur_off, cur_len, ob, oo, ol, nullptr, w.dd.aad, aad_len,
-                                  w.dd.status, nb, max_t, w.d_partials, w.max_ranges,
-                                  z ? (uint32_t)(c->frame_stride - 16) : c->chunk_cap);
-        if (rc) return rc;
-        w.key_valid = true;
-        cur_base = ob; cur_off = oo; cur_len = ol;
-    }
-    if (flags & TSGPU_FLAG_ZSTD) {
-        { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
-        int rc = zstd_decompress_batch(w.zdec, st, cur_base, cur_off, cur_len, nb, c->chunk_cap,
-                                       w.d_orig, w.dd.a_off, w.dd.a_len, w.dd.status, /*compute_offsets=*/true, c->prof);
-        if (rc) return fail(rc, "zstd decompress: %s", zstd_last_error());
-    }
+    const DxBounds lim{max_t, room, 0xffffffffu, c->chunk_cap};
+    { int rc = detransform_enqueue(c, w, st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
+                                   ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len}, w.dd.status, lim, /*packed=*/true); if (rc) return rc; }
     RT(rt::d2h(w.h_sizes, w.dd.a_len, 4ull * nb, st));
     RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
-    db.w = &w; db.c0 = c0; db.nb = nb; db.in_bytes = ip;
-    w.busy = true;
     return TSGPU_OK;
 }
 
@@ -626,7 +653,7 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
     if (!src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
     if (!transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
-    if (flags & ~(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
+    if (flags & ~KNOWN_FLAGS) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
     if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
     flags &= ~TSGPU_FLAG_ZSTD_DENSE;                         // how a frame was compressed does not matter to the reader
@@ -643,59 +670,27 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
     Aes256RoundKeys rk{};
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
 
-    const uint32_t nbatches = (n_chunks + c->max_batch - 1) / c->max_batch;
-    SlotClaim claim;
-    { int rcc = claim_slots(c, nbatches, claim); if (rcc) return rcc; }
-    const uint32_t nwork = (uint32_t)claim.slots.size();
-    std::vector<DxBatch> inflight(nbatches);
-    std::vector<uint64_t> in_pos(nbatches + 1, 0);
-    for (uint32_t b = 0; b < nbatches; b++) {
-        uint64_t s = 0;
-        for (uint32_t i = b * c->max_batch; i < std::min(n_chunks, (b + 1) * c->max_batch); i++) s += transformed_sizes[i];
-        in_pos[b + 1] = in_pos[b] + s;
-    }
-    uint64_t dst_off = 0;
-    int rc = TSGPU_OK, soft = TSGPU_OK;
-    auto work_of = [&](uint32_t b) -> Work& { return *claim.slots[b % nwork]; };
-    auto drain = [&](uint32_t b) -> int {
-        DxBatch& db = inflight[b];
-        Work& w = *db.w;
-        RT(rt::set_device(w.device));
-        RT(rt::event_sync(w.ev_sizes));
-        uint64_t total = 0;
-        for (uint32_t i = 0; i < db.nb; i++) {
-            uint32_t stt = w.h_sizes[db.nb + i];
-            if (stt == 1 && soft == TSGPU_OK) soft = fail(TSGPU_E_AUTH, "Tag mismatch in chunk %u", db.c0 + i);
-            else if (stt > 1 && soft == TSGPU_OK) soft = fail(TSGPU_E_CORRUPT, "Invalid zstd frame in chunk %u (code %u)", db.c0 + i, stt);
-            if (original_sizes) original_sizes[db.c0 + i] = w.h_sizes[i];
-            total += w.h_sizes[i];
-        }
-        if (soft != TSGPU_OK) return soft;
-        if (dst_off + total > dst_cap) return fail(TSGPU_E_SHORT, "dst too small");
-        rt::stream_t os = c->split_out ? w.out_stream : w.stream;
-        if (total) RT(rt::d2h(dst + dst_off, w.d_orig, total, os));
-        dst_off += total;
-        RT(rt::event_record(w.ev_done, os));
-        w.out_pending = c->split_out;
-        return TSGPU_OK;
-    };
-    uint32_t drained = 0;
-    for (uint32_t b = 0; b < nbatches && rc == TSGPU_OK; b++) {
-        if (b >= nwork) {
-            if (drained <= b - nwork) { rc = drain(drained++); if (rc) break; }
-        }
-        uint32_t c0 = b * c->max_batch, nb = std::min(c->max_batch, n_chunks - c0);
-        rc = detransform_issue(c, work_of(b), flags, src + in_pos[b], transformed_sizes, c0, nb, rk, aad, aad_len, inflight[b]);
-    }
-    while (rc == TSGPU_OK && drained < nbatches) rc = drain(drained++);
-    for (Work* wp : claim.slots) if (wp->busy) {
-        Work& w = *wp;
-        rt::set_device(w.device);
-        const char* e = rt::stream_sync(w.stream);
-        if (!e) e = rt::stream_sync(w.out_stream);
-        if (e && rc == TSGPU_OK) rc = fail(TSGPU_E_CUDA, "stream_sync: %s", e);
-        w.busy = false; w.out_pending = false;
-    }
+    uint64_t in_off = 0, dst_off = 0;                        // batches are issued in order: in_off walks src with them
+    int soft = TSGPU_OK;
+    const int rc = run_batches(c, n_chunks,
+        [&](const Batch& bt) {
+            const int r = detransform_issue(c, bt, flags, src + in_off, transformed_sizes, rk, aad, aad_len);
+            for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
+            return r;
+        },
+        [&](const Batch& bt) {
+            Work& w = *bt.w;
+            uint64_t total = 0;
+            for (uint32_t i = 0; i < bt.nb; i++) {
+                uint32_t stt = w.h_sizes[bt.nb + i];
+                if (stt == 1 && soft == TSGPU_OK) soft = fail(TSGPU_E_AUTH, "Tag mismatch in chunk %u", bt.c0 + i);
+                else if (stt > 1 && soft == TSGPU_OK) soft = fail(TSGPU_E_CORRUPT, "Invalid zstd frame in chunk %u (code %u)", bt.c0 + i, stt);
+                if (original_sizes) original_sizes[bt.c0 + i] = w.h_sizes[i];
+                total += w.h_sizes[i];
+            }
+            if (soft != TSGPU_OK) return soft;
+            return copy_out(w, w.d_orig, total, dst, dst_cap, dst_off);
+        });
     if (rc == TSGPU_E_AUTH || rc == TSGPU_E_CORRUPT) {
         // JCE releases no plaintext when the tag check fails: do not leave partial output behind
         memset(dst, 0, (size_t)dst_off);
@@ -707,22 +702,32 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
 // The device API reuses slot 0's pinned descriptor block and scratch arenas.  Two events make back-to-back calls safe on
 // any streams: the host waits until the previous call's descriptor upload has left the pinned block before rewriting it,
 // and the new call's stream waits for the previous call's kernels before touching the shared scratch.
-static int dev_call_begin(Work& w, rt::stream_t st) {
-    // (claim_slots has already waited for the previous device call's END when one was pending; the waits below matter when
-    // this begins to be relaxed, and cost nothing on completed events)
-    if (w.dev_pending) { RT(rt::event_sync(w.ev_dev_desc)); RT(rt::stream_wait_event(st, w.ev_dev_done)); }
-    return TSGPU_OK;
-}
-static int dev_call_end(Work& w, rt::stream_t st) {
-    RT(rt::event_record(w.ev_dev_done, st));
-    w.dev_pending = true;
+
+// Argument checks of both device calls; n (the number of chunks) == 0 passes, and the call then has nothing to do.
+static int dev_args_ok(tsgpu_ctx* c, int device_index, uint32_t flags, uint32_t chunk_size, uint64_t n, uint64_t slot_stride) {
+    if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
+    if (device_index < 0 || device_index >= (int)c->lanes.size()) return fail(TSGPU_E_ARG, "device_index %d out of range", device_index);
+    if ((flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)) == 0 || (flags & ~KNOWN_FLAGS)) return fail(TSGPU_E_ARG, "flags must name zstd and/or aes");
+    if (chunk_size == 0 || chunk_size > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk_size out of range for this context");
+    if (n == 0) return TSGPU_OK;
+    if (n > c->max_batch) return fail(TSGPU_E_ARG, "%llu chunks exceed the context's max_batch %u", (unsigned long long)n, c->max_batch);
+    if (slot_stride < tsgpu_slot_stride(flags, chunk_size) || (slot_stride & 15)) return fail(TSGPU_E_ARG, "slot_stride too small or not a multiple of 16");
     return TSGPU_OK;
 }
 
-static int pick_work(tsgpu_ctx* c, int device_index, Work** w) {
-    if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
-    if (device_index < 0 || device_index >= (int)c->lanes.size()) return fail(TSGPU_E_ARG, "device_index %d out of range", device_index);
-    *w = &c->lanes[device_index].w[0];
+// Claims slot 0 of the device for the duration of the enqueue, orders this call behind the previous device call, lets
+// fill(w) write the descriptor block and uploads it.  The slot is claim.slots[0].
+template <class Fill>
+static int dev_call_begin(tsgpu_ctx* c, int device_index, rt::stream_t st, SlotClaim& claim, Fill fill) {
+    { int rcc = claim_slots(c, 1, claim, device_index, 0, /*wait_dev=*/false); if (rcc) return rcc; }
+    Work& w = *claim.slots[0];
+    RT(rt::set_device(w.device));
+    if (w.dev_pending) { RT(rt::event_sync(w.ev_dev_desc)); RT(rt::stream_wait_event(st, w.ev_dev_done)); }
+    fill(w);
+    RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
+    RT(rt::event_record(w.ev_dev_desc, st));
+    w.dev_pending = true;                                    // from here on the next call must order itself behind this one
+    RT(rt::event_record(w.ev_dev_done, st));
     return TSGPU_OK;
 }
 
@@ -730,116 +735,71 @@ extern "C" int tsgpu_transform_device(tsgpu_ctx* c, int device_index, uint32_t f
                                       uint32_t chunk_size, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                                       const uint8_t* ivs, uint8_t* d_slots, uint64_t slot_stride,
                                       uint32_t* d_transformed_sizes, void* stream) {
-    Work* wp = nullptr; int rc = pick_work(c, device_index, &wp); if (rc) return rc;
-    Work& w = *wp;
-    if ((flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)) == 0 || (flags & ~(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE))) return fail(TSGPU_E_ARG, "flags must name zstd and/or aes");
-    if (chunk_size == 0 || chunk_size > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk_size out of range for this context");
-    if (src_len == 0) return TSGPU_OK;
-    const uint64_t n64 = (src_len + chunk_size - 1) / chunk_size;
-    if (n64 > c->max_batch) return fail(TSGPU_E_ARG, "%llu chunks exceed the context's max_batch %u", (unsigned long long)n64, c->max_batch);
-    if (slot_stride < tsgpu_slot_stride(flags, chunk_size) || (slot_stride & 15)) return fail(TSGPU_E_ARG, "slot_stride too small or not a multiple of 16");
+    const uint64_t n64 = chunk_size ? (src_len + chunk_size - 1) / chunk_size : 0;
+    int rc = dev_args_ok(c, device_index, flags, chunk_size, n64, slot_stride);
+    if (rc || n64 == 0) return rc;
     if ((flags & TSGPU_FLAG_AES) && (!key || !ivs || aad_len > MAX_AAD)) return fail(TSGPU_E_ARG, "key/ivs/aad invalid");
     const uint32_t nb = (uint32_t)n64, cs = chunk_size;
-    SlotClaim claim;                                         // slot 0 of the device, for the duration of the enqueue
-    { int rcc = claim_slots(c, 1, claim, device_index, 0, /*wait_dev=*/false); if (rcc) return rcc; }
-    RT(rt::set_device(w.device));
-    rt::stream_t st = (rt::stream_t)stream;
-    { int rb = dev_call_begin(w, st); if (rb) return rb; }
-    for (uint32_t i = 0; i < nb; i++) {
-        w.hd.a_off[i] = (uint64_t)i * cs;
-        w.hd.a_len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - (uint64_t)i * cs);
-        w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
-        w.hd.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD;
-    }
     Aes256RoundKeys rk{};
-    if (flags & TSGPU_FLAG_AES) {
-        rk = aes256_expand_key(key);
-        memcpy(w.hd.ivs, ivs, (size_t)nb * TSGPU_IV_SIZE);
-        if (aad_len) memcpy(w.hd.aad, aad, aad_len);
-    }
-    RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
-    RT(rt::event_record(w.ev_dev_desc, st));
-    w.dev_pending = true;                                    // from here on the next call must order itself behind this one
+    if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
+    rt::stream_t st = (rt::stream_t)stream;
+    SlotClaim claim;
+    rc = dev_call_begin(c, device_index, st, claim, [&](Work& w) {
+        for (uint32_t i = 0; i < nb; i++) {
+            w.hd.a_off[i] = (uint64_t)i * cs;
+            w.hd.a_len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - (uint64_t)i * cs);
+            w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
+            w.hd.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD;
+        }
+        if (flags & TSGPU_FLAG_AES) {
+            memcpy(w.hd.ivs, ivs, (size_t)nb * TSGPU_IV_SIZE);
+            if (aad_len) memcpy(w.hd.aad, aad, aad_len);
+        }
+    });
+    if (rc) return rc;
+    Work& w = *claim.slots[0];
+    rc = transform_enqueue(c, w, st, flags, nb, cs, rk, aad_len, ChunksIn{d_src, w.dd.a_off, w.dd.a_len},
+                           ChunksOut{d_slots, w.dd.c_off, d_transformed_sizes});
+    if (rc) return rc;
     RT(rt::event_record(w.ev_dev_done, st));
-    const uint8_t* cur_base = d_src; const uint64_t* cur_off = w.dd.a_off; const uint32_t* cur_len = w.dd.a_len;
-    uint32_t cur_max = cs;
-    if (flags & TSGPU_FLAG_ZSTD) {
-        const bool to_slots = !(flags & TSGPU_FLAG_AES);
-        uint8_t* fb = to_slots ? d_slots : w.d_frames;
-        const uint64_t* fo = to_slots ? w.dd.c_off : w.dd.b_off;
-        uint32_t* fl = to_slots ? d_transformed_sizes : w.dd.b_len;
-        int zr = zstd_stage(c, w, st, flags, cur_base, cur_off, cur_len, nb, cs, fb, fo, fl);
-        if (zr) return zr;
-        cur_base = fb; cur_off = fo; cur_len = fl; cur_max = (uint32_t)frame_bound(cs);
-    }
-    if (flags & TSGPU_FLAG_AES) {
-        // the slot's key tables are reused while the key stays the same: device calls are ordered behind each other by
-        // events (dev_call_begin) and host calls only take the slot once device work on it has completed
-        const bool key_ready = w.key_valid && memcmp(&w.key_rk, &rk, sizeof rk) == 0;
-        w.key_rk = rk; w.key_valid = false;
-        rc = gcm_stage<true>(c, w, st, rk, key_ready, cur_base, cur_off, cur_len, d_slots, w.dd.c_off, d_transformed_sizes,
-                             w.dd.ivs, w.dd.aad, aad_len, w.dd.status, nb, cur_max, w.d_partials, w.max_ranges);
-        if (rc) return rc;
-        w.key_valid = true;
-    }
-    return dev_call_end(w, st);
+    return TSGPU_OK;
 }
 
 extern "C" int tsgpu_detransform_device(tsgpu_ctx* c, int device_index, uint32_t flags, const uint8_t* d_slots,
                                         uint64_t slot_stride, const uint32_t* d_transformed_sizes, uint32_t n_chunks,
                                         uint32_t chunk_size, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                                         uint8_t* d_dst, uint32_t* d_original_sizes, uint32_t* d_status, void* stream) {
-    Work* wp = nullptr; int rc = pick_work(c, device_index, &wp); if (rc) return rc;
-    Work& w = *wp;
-    if ((flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)) == 0 || (flags & ~(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE))) return fail(TSGPU_E_ARG, "flags must name zstd and/or aes");
-    if (chunk_size == 0 || chunk_size > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk_size out of range for this context");
-    if (n_chunks == 0) return TSGPU_OK;
-    if (n_chunks > c->max_batch) return fail(TSGPU_E_ARG, "%u chunks exceed the context's max_batch %u", n_chunks, c->max_batch);
+    int rc = dev_args_ok(c, device_index, flags, chunk_size, n_chunks, slot_stride);
+    if (rc || n_chunks == 0) return rc;
     if ((flags & TSGPU_FLAG_AES) && (!key || aad_len > MAX_AAD)) return fail(TSGPU_E_ARG, "key/aad invalid");
-    if (slot_stride < tsgpu_slot_stride(flags, chunk_size) || (slot_stride & 15)) return fail(TSGPU_E_ARG, "slot_stride too small or not a multiple of 16");
     if (!d_slots || !d_transformed_sizes || !d_dst || !d_original_sizes || !d_status) return fail(TSGPU_E_ARG, "null device pointer");
-    SlotClaim claim;                                         // slot 0 of the device, for the duration of the enqueue
-    { int rcc = claim_slots(c, 1, claim, device_index, 0, /*wait_dev=*/false); if (rcc) return rcc; }
-    RT(rt::set_device(w.device));
-    rt::stream_t st = (rt::stream_t)stream;
-    { int rb = dev_call_begin(w, st); if (rb) return rb; }
-    for (uint32_t i = 0; i < n_chunks; i++) {
-        w.hd.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD;
-        w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
-        w.hd.a_off[i] = (uint64_t)i * chunk_size;            // original side: chunk i at i * chunk_size
-    }
     Aes256RoundKeys rk{};
-    if (flags & TSGPU_FLAG_AES) { rk = aes256_expand_key(key); if (aad_len) memcpy(w.hd.aad, aad, aad_len); }
-    RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
-    RT(rt::event_record(w.ev_dev_desc, st));
-    w.dev_pending = true;
-    RT(rt::event_record(w.ev_dev_done, st));
+    if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
+    rt::stream_t st = (rt::stream_t)stream;
+    SlotClaim claim;
+    rc = dev_call_begin(c, device_index, st, claim, [&](Work& w) {
+        for (uint32_t i = 0; i < n_chunks; i++) {
+            w.hd.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD;
+            w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
+            w.hd.a_off[i] = (uint64_t)i * chunk_size;        // original side: chunk i at i * chunk_size
+        }
+        if ((flags & TSGPU_FLAG_AES) && aad_len) memcpy(w.hd.aad, aad, aad_len);
+    });
+    if (rc) return rc;
+    Work& w = *claim.slots[0];
     RT(rt::memset_async(d_status, 0, 4ull * n_chunks, st));
     // sizes are device-resident (possibly from a manifest): the kernels bound them against these capacities
     const uint32_t in_room = (uint32_t)std::min<uint64_t>(slot_stride - TSGPU_SLOT_HEAD, 0xffffffffu);
-    const uint8_t* cur_base = d_slots; const uint64_t* cur_off = w.dd.c_off; const uint32_t* cur_len = d_transformed_sizes;
-    if (flags & TSGPU_FLAG_AES) {
-        const bool z = flags & TSGPU_FLAG_ZSTD;
-        uint8_t* ob = z ? w.d_frames : d_dst;
-        const uint64_t* oo = z ? w.dd.b_off : w.dd.a_off;
-        uint32_t* ol = z ? w.dd.b_len : d_original_sizes;
-        uint32_t max_t = (uint32_t)(slot_stride - TSGPU_SLOT_HEAD);
-        const bool key_ready = w.key_valid && memcmp(&w.key_rk, &rk, sizeof rk) == 0;
-        w.key_rk = rk; w.key_valid = false;
-        const uint32_t out_room = z ? (uint32_t)std::min<uint64_t>(c->frame_stride - 16, in_room - 28) : chunk_size;
-        rc = gcm_stage<false>(c, w, st, rk, key_ready, cur_base, cur_off, cur_len, ob, oo, ol, nullptr, w.dd.aad, aad_len,
-                              d_status, n_chunks, max_t, w.d_partials, w.max_ranges, out_room);
-        if (rc) return rc;
-        w.key_valid = true;
-        cur_base = ob; cur_off = oo; cur_len = ol;
-    }
-    if (flags & TSGPU_FLAG_ZSTD) {
-        const uint32_t zin_room = (flags & TSGPU_FLAG_AES) ? (uint32_t)(c->frame_stride - 16) : in_room;
-        int zr = zstd_decompress_batch(w.zdec, st, cur_base, cur_off, cur_len, n_chunks, chunk_size,
-                                       d_dst, w.dd.a_off, d_original_sizes, d_status, /*compute_offsets=*/false, c->prof, zin_room);
-        if (zr) return fail(zr, "zstd decompress: %s", zstd_last_error());
-    }
-    return dev_call_end(w, st);
+    DxBounds lim;
+    lim.max_in = (uint32_t)(slot_stride - TSGPU_SLOT_HEAD);
+    lim.aes_room = (flags & TSGPU_FLAG_ZSTD) ? (uint32_t)std::min<uint64_t>(c->frame_stride - 16, in_room - 28) : chunk_size;
+    lim.zstd_in = (flags & TSGPU_FLAG_AES) ? (uint32_t)(c->frame_stride - 16) : in_room;
+    lim.zstd_out = chunk_size;
+    rc = detransform_enqueue(c, w, st, flags, n_chunks, rk, aad_len, ChunksIn{d_slots, w.dd.c_off, d_transformed_sizes},
+                             ChunksOut{d_dst, w.dd.a_off, d_original_sizes}, d_status, lim, /*packed=*/false);
+    if (rc) return rc;
+    RT(rt::event_record(w.ev_dev_done, st));
+    return TSGPU_OK;
 }
 
 // ------------------------------------------------------------------------------------------ profiling
