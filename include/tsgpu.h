@@ -32,6 +32,16 @@ extern "C" {
  * byte-identical frames on every run.  Both are plain zstd frames with Frame_Content_Size; libzstd and this library read both.
  * TSGPU_ZSTD_MODE=dense in the environment makes dense the default of a context. */
 #define TSGPU_FLAG_ZSTD_DENSE 4u
+/* Read-back check of the host-buffer transform calls (tsgpu_transform, tsgpu_transform_chunks; any mix of ZSTD / ZSTD_DENSE /
+ * AES): each batch is detransformed on the device and compared byte for byte with its input before any of its bytes are
+ * copied to dst.  A chunk that does not read back fails the call with TSGPU_E_VERIFY.  Opt-in, like RocksDB's
+ * verify_compression: with 4 MiB chunks it adds the device decrypt / decode of every batch (cost: DESIGN.md §8).
+ * The check decodes with this library's own decoder.  It catches runtime faults of the writer -- races, memory errors,
+ * silent data corruption -- but not a misreading of the format that the writer and the reader share; the libzstd and
+ * OpenSSL cross-tests of the test suite remain the guard for that.  Its decodes count in tsgpu_decode_path_stats.
+ * TSGPU_VERIFY=1 in the environment makes the flag the default of a context's host-buffer transform calls.  The
+ * device-resident calls refuse the bit (TSGPU_E_ARG): they have no status output on the transform side. */
+#define TSGPU_FLAG_VERIFY 8u
 
 #define TSGPU_IV_SIZE   12     /* SegmentEncryptionMetadataV1.java:30 */
 #define TSGPU_TAG_SIZE  16     /* AesEncryptionProvider.java:38 (128-bit tag) */
@@ -45,6 +55,10 @@ extern "C" {
 #define TSGPU_E_NODEVICE   -6  /* no usable CUDA device: the product path does not fall back to the CPU */
 #define TSGPU_E_CUDA       -7  /* a CUDA call or kernel failed; message in tsgpu_last_error() */
 #define TSGPU_E_NOMEM      -8
+/* TSGPU_FLAG_VERIFY: a transformed chunk did not read back.  The message names the chunk and the check that failed: tag,
+ * frame, size, or the first byte offset that differs.  No byte of the failing batch reaches dst; earlier batches may
+ * already be there, and the caller discards the whole result as with any error. */
+#define TSGPU_E_VERIFY     -9
 
 typedef struct tsgpu_ctx tsgpu_ctx;
 
@@ -59,8 +73,9 @@ const char* tsgpu_version(void);
  * A host-buffer call (tsgpu_transform / tsgpu_detransform) cuts its chunks into batches of `max_batch` and keeps up to
  * 8 of them in flight per device (work slots, allocated on first use; each has a compute stream and a copy-out stream).
  * With 4 MiB chunks `max_batch = 4` measured best through PCIe; device-resident callers pass whole segments.
- * Environment (read once by tsgpu_create; tuning only): TSGPU_SLOTS=1..16 slots per device, TSGPU_ZSTD_MODE=dense makes
- * TSGPU_FLAG_ZSTD_DENSE the context's default.
+ * Environment (read once by tsgpu_create): TSGPU_SLOTS=1..16 slots per device, TSGPU_ZSTD_MODE=dense makes
+ * TSGPU_FLAG_ZSTD_DENSE the context's default (both tuning only), TSGPU_VERIFY=1 turns TSGPU_FLAG_VERIFY on for the
+ * context's host-buffer transform calls (not for the device-resident calls).
  * --------------------------------------------------------------------------------------------------------- */
 int  tsgpu_create(const int* device_ids, int n_devices, uint32_t max_chunk_bytes, uint32_t max_batch,
                   tsgpu_ctx** out);
@@ -155,6 +170,7 @@ uint64_t tsgpu_launch_count(const tsgpu_ctx* ctx);
  * of this library's writer), out[1] frames handed from a region / block to the frame executor, out[2] frames executed whole
  * (frames written by libzstd, i.e. by the reference), out[3] frames on the serial fallback kernel, out[4] self-contained 8 KiB
  * blocks executed by a warp each (speed-mode frames of this library's writer), out[5..7] reserved (0).
+ * The read-back decodes of TSGPU_FLAG_VERIFY count here like any other decode.
  * Synchronises the context's devices. */
 int tsgpu_decode_path_stats(tsgpu_ctx* ctx, uint64_t out[8]);
 /* Optional per-kernel timing with CUDA events recorded on the launching stream (bench.py's roofline numbers).

@@ -14,10 +14,12 @@ DEFAULT_LIB = os.path.join(_HERE, "libtsgpu.so")
 FLAG_ZSTD = 1
 FLAG_AES = 2
 FLAG_ZSTD_DENSE = 4
+FLAG_VERIFY = 8          # host-buffer transforms: read each batch back on the device before releasing it
 IV_SIZE = 12
 TAG_SIZE = 16
 SLOT_HEAD = 4
 OK, E_ARG, E_STATE, E_AUTH, E_CORRUPT, E_SHORT, E_NODEVICE, E_CUDA, E_NOMEM = 0, -1, -2, -3, -4, -5, -6, -7, -8
+E_VERIFY = -9
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",

@@ -6,7 +6,8 @@
 //   own stream, device arenas and pinned descriptor block -> per batch: H2D original bytes, [zstd kernels],
 //   [AES-GCM kernels], D2H of the chunk sizes, then per-chunk D2H of exactly transformed_size bytes to the
 //   running offset in dst (the packed .log object layout, SURVEY.md appendix A.1).  Batches complete in order;
-//   up to (devices x slots) batches are in flight so copies overlap kernels.
+//   up to (devices x slots) batches are in flight so copies overlap kernels.  With TSGPU_FLAG_VERIFY each batch is
+//   detransformed on the device and compared with its input before any of its bytes are copied out.
 #include <condition_variable>
 #include <mutex>
 #include <new>
@@ -20,6 +21,7 @@
 #include "aesgcm.cuh"
 #include "index_scan.cuh"
 #include "pack.cuh"
+#include "verify.cuh"
 #include "rt.h"
 #include "launch_prof.h"
 #include "zstd_enc.cuh"
@@ -53,6 +55,7 @@ constexpr uint32_t KNOWN_FLAGS = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_Z
 struct Desc {            // device-side descriptor block of one work slot (all arrays sized for max_batch)
     uint64_t* a_off; uint64_t* b_off; uint64_t* c_off;
     uint32_t* a_len; uint32_t* b_len; uint32_t* c_len; uint32_t* status;
+    uint32_t* v_len; uint32_t* v_diff;     // TSGPU_FLAG_VERIFY: read-back sizes, first differing byte per chunk
     uint8_t* ivs; uint8_t* aad;
 };
 
@@ -78,7 +81,7 @@ struct Work {
     ZstdEncScratch zenc{};         // region kernel (TSGPU_FLAG_ZSTD_DENSE), allocated on first use
     ZstdBlkScratch zblk{};         // block kernel (default), allocated on first use
     ZstdDecScratch zdec{};
-    uint32_t* h_sizes = nullptr;   // pinned: sizes/status coming back
+    uint32_t* h_sizes = nullptr;   // pinned: sizes/status (and the verify stage's first differing bytes) coming back
 };
 
 struct Lane { int device = 0; Work w[NSLOT_MAX]; };
@@ -87,6 +90,7 @@ struct Lane { int device = 0; Work w[NSLOT_MAX]; };
 
 struct tsgpu_ctx {
     bool dense_default = false;    // TSGPU_ZSTD_MODE=dense: TSGPU_FLAG_ZSTD alone already means the region kernel
+    bool verify_default = false;   // TSGPU_VERIFY=1: host-buffer transforms verify as if TSGPU_FLAG_VERIFY were set
     std::mutex mu;                 // guards slot ownership (Work::claimed, active_calls) and lazy slot allocation — NOT held while a call runs
     std::condition_variable cv;
     uint32_t active_calls = 0;
@@ -103,6 +107,7 @@ static void carve_desc(uint8_t* base, uint32_t nb, Desc& d, size_t* total) {
     d.a_off = (uint64_t*)take(8ull * nb); d.b_off = (uint64_t*)take(8ull * nb); d.c_off = (uint64_t*)take(8ull * (nb + 1));
     d.a_len = (uint32_t*)take(4ull * nb); d.b_len = (uint32_t*)take(4ull * nb); d.c_len = (uint32_t*)take(4ull * nb);
     d.status = (uint32_t*)take(4ull * nb);
+    d.v_len = (uint32_t*)take(4ull * nb); d.v_diff = (uint32_t*)take(4ull * nb);
     d.ivs = take(12ull * nb); d.aad = take(MAX_AAD);
     if (total) *total = p;
 }
@@ -139,7 +144,7 @@ static int work_init_impl(tsgpu_ctx* c, Work& w, int device) {
     w.max_ranges = (uint32_t)((frame_bound(c->chunk_cap) / 16 + GH_RANGE_BLOCKS) / GH_RANGE_BLOCKS) + 1;
     RT(rt::malloc_device((void**)&w.d_partials, sizeof(uint4) * (size_t)w.max_ranges * nb));
     RT(rt::malloc_device((void**)&w.d_keyctx, sizeof(GcmKeyCtx)));
-    RT(rt::malloc_host((void**)&w.h_sizes, 4ull * nb * 2 + 64));
+    RT(rt::malloc_host((void**)&w.h_sizes, 4ull * nb * 3 + 64));
     const char* e = zstd_dec_scratch_alloc(w.zdec, c->chunk_cap, c->max_batch);
     if (e) return fail(TSGPU_E_CUDA, "zstd dec scratch: %s", e);
     return TSGPU_OK;
@@ -194,6 +199,7 @@ extern "C" int tsgpu_create(const int* device_ids, int n_devices, uint32_t max_c
     c->chunk_cap = max_chunk_bytes; c->max_batch = max_batch;
     if (const char* e = getenv("TSGPU_SLOTS")) { int v = atoi(e); if (v >= 1 && v <= NSLOT_MAX) c->nslot = (uint32_t)v; }       // tuning knobs
     if (const char* e = getenv("TSGPU_ZSTD_MODE")) c->dense_default = strcmp(e, "dense") == 0;
+    if (const char* e = getenv("TSGPU_VERIFY")) c->verify_default = strcmp(e, "1") == 0;
     c->frame_stride = align_up(frame_bound(max_chunk_bytes), 16) + 16;
     c->slot_stride = tsgpu_slot_stride(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES, max_chunk_bytes);
     c->lanes.resize(ids.size());
@@ -472,9 +478,52 @@ static int copy_out(Work& w, const uint8_t* from, uint64_t total, uint8_t* dst, 
 }
 
 // ------------------------------------------------------------------------------------------ transform (host)
-// One batch: copy in, fill the descriptors, enqueue the stages, pack the transformed chunks, D2H of their sizes.
+// TSGPU_FLAG_VERIFY: the batch's transformed chunks (`fin`, still in their slots once pack_chunks has run) go through the
+// detransform stages and are compared with the input in d_orig.  No buffer beyond the slot's own: Z|A decrypts d_xf into
+// d_frames and decodes that into d_xf; A decrypts d_xf into d_frames; Z decodes d_frames into d_xf.  The read-back chunk i
+// lands at b_off[i] (a 16-byte aligned frame slot; d_xf's slots are larger) with its size in v_len, so a_len survives.
+// Leaves per chunk: status 0 / 1 tag / 2 frame / VERIFY_ST_SIZE, and v_diff = first differing byte or VERIFY_NO_DIFF.
+static int verify_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, uint32_t nb, uint32_t cs,
+                        const Aes256RoundKeys& rk, uint32_t aad_len, ChunksOut fin) {
+    const bool zstd = flags & TSGPU_FLAG_ZSTD;
+    RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
+    RT(rt::memset_async(w.dd.v_diff, 0xff, 4ull * nb, st));
+    DxBounds lim;
+    lim.max_in = (uint32_t)((zstd ? frame_bound(cs) : cs) + TSGPU_IV_SIZE + TSGPU_TAG_SIZE);
+    lim.aes_room = zstd ? (uint32_t)(c->frame_stride - 16) : c->chunk_cap;
+    lim.zstd_in = (uint32_t)(c->frame_stride - 16);
+    lim.zstd_out = cs;                                        // a frame claiming more than the batch's largest chunk is wrong
+    const ChunksOut back{zstd ? w.d_xf : w.d_frames, w.dd.b_off, w.dd.v_len};
+    { int rc = detransform_enqueue(c, w, st, flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES), nb, rk, aad_len, fin, back, w.dd.status,
+                                   lim, /*packed=*/false); if (rc) return rc; }
+    VerifyArgs V;
+    V.orig = w.d_orig; V.orig_off = w.dd.a_off; V.orig_len = w.dd.a_len;
+    V.back = back.base; V.back_off = back.off; V.back_len = back.len;
+    V.status = w.dd.status; V.diff = w.dd.v_diff;
+    TS_LAUNCH_P(c->prof, "verify_compare", verify_compare_kernel, dim3((cs + VERIFY_PIECE - 1) / VERIFY_PIECE, nb), dim3(VERIFY_T), 0, st, V);
+    CHECK_LAUNCH("verify_compare_kernel");
+    return TSGPU_OK;
+}
+
+#ifdef TSGPU_SIMT
+// TEST-ONLY fault injection, compiled into the emulator build alone (device memory is host memory there and every kernel
+// has finished when its launch returns).  TSGPU_SIMT_FLIP=<chunk>:<offset> flips the low bit of one byte of that chunk's
+// transformed bytes -- frame, or IV || ciphertext || tag -- before they are packed and verified.  A negative offset counts
+// from the chunk's end (-1: last tag byte).  tests/test_simt_verify.py drives it.
+static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
+    const char* e = getenv("TSGPU_SIMT_FLIP");
+    long k = 0, at = 0;
+    if (!e || sscanf(e, "%ld:%ld", &k, &at) != 2 || k < (long)c0 || k >= (long)c0 + (long)nb) return;
+    const uint32_t i = (uint32_t)(k - c0), n = fin.len[i];
+    if (at < 0) at += n;
+    if (at >= 0 && at < (long)n) fin.base[fin.off[i] + at] ^= 1;
+}
+#endif
+
+// One batch: copy in, fill the descriptors, enqueue the stages, pack the transformed chunks, [verify them,] D2H of their
+// sizes (and of the verify stage's verdicts).
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
-static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const uint8_t* src, const uint64_t* off,
+static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, const uint8_t* src, const uint64_t* off,
                            const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
                            const uint8_t* ivs) {
     Work& w = *bt.w;
@@ -500,6 +549,9 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const 
     // encrypted chunks land in the transformed slots; zstd alone leaves its frames in the frame slots
     const ChunksOut fin = aes ? ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len} : ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len};
     { int rc = transform_enqueue(c, w, st, flags, nb, cs, rk, aad_len, ChunksIn{w.d_orig, w.dd.a_off, w.dd.a_len}, fin); if (rc) return rc; }
+#ifdef TSGPU_SIMT
+    simt_inject_fault(fin, c0, nb);
+#endif
     // the transformed chunks, back to back, so the batch leaves in one copy (the previous batch's copy-out may still be
     // reading d_pack: this is the first kernel of the batch that has to wait for it)
     { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
@@ -511,8 +563,31 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const 
         TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
         CHECK_LAUNCH("pack_chunks_kernel");
     }
+    if (verify) {
+        int rc = verify_stage(c, w, st, flags, nb, cs, rk, aad_len, fin);
+        if (rc) return rc;
+        RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.h_sizes + 2 * nb, w.dd.v_diff, 4ull * nb, st));
+    }
     RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
+    return TSGPU_OK;
+}
+
+// The verify stage's verdict on a drained batch (h_sizes: sizes, status, first differing bytes); TSGPU_OK if every chunk
+// read back.  `len`: the original chunk sizes of the call.
+static int verify_verdict(const Batch& bt, const uint32_t* len) {
+    const uint32_t* status = bt.w->h_sizes + bt.nb;
+    const uint32_t* diff = bt.w->h_sizes + 2 * bt.nb;
+    for (uint32_t i = 0; i < bt.nb; i++) {
+        const uint32_t k = bt.c0 + i;
+        if (status[i] == 1) return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: tag check failed", k);
+        if (status[i] == VERIFY_ST_SIZE)
+            return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: size check failed (original %u bytes)", k, len[k]);
+        if (status[i] != 0) return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: frame check failed (code %u)", k, status[i]);
+        if (diff[i] != VERIFY_NO_DIFF)
+            return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: bytes differ from offset %u", k, diff[i]);
+    }
     return TSGPU_OK;
 }
 
@@ -525,7 +600,7 @@ static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
     if (!n_chunks || !transformed_sizes) return fail(TSGPU_E_ARG, "transformed_sizes/n_chunks cannot be null");
     if (src_len && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
-    if (flags & ~KNOWN_FLAGS) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
+    if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if ((flags & TSGPU_FLAG_AES) && (!key || !ivs)) return fail(TSGPU_E_ARG, "key and ivs are required for encryption");
     if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
     if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
@@ -578,8 +653,10 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
     const uint32_t n = (uint32_t)len.size();
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
     if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~TSGPU_FLAG_ZSTD_DENSE;   // a modifier of ZSTD: meaningless (and harmless) without it
+    const bool verify = (flags & TSGPU_FLAG_VERIFY) || c->verify_default;
+    flags &= ~TSGPU_FLAG_VERIFY;
 
-    if (flags == 0) {       // TransformFinisher no-transform fast path (TransformFinisher.java:135-140): bytes unchanged
+    if (flags == 0) {       // TransformFinisher no-transform fast path (TransformFinisher.java:135-140): bytes unchanged, nothing to verify
         if (dst_cap < src_len) return fail(TSGPU_E_SHORT, "dst too small");
         memcpy(dst, src, src_len);
         for (uint32_t i = 0; i < n; i++) transformed_sizes[i] = len[i];
@@ -591,9 +668,10 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
 
     uint64_t dst_off = 0;
     const int rc = run_batches(c, n,
-        [&](const Batch& bt) { return transform_issue(c, bt, flags, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
+        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
         [&](const Batch& bt) {
             Work& w = *bt.w;
+            if (verify) { int rcv = verify_verdict(bt, len.data()); if (rcv) return rcv; }   // none of the batch's bytes leave
             uint64_t total = 0;
             for (uint32_t i = 0; i < bt.nb; i++) { transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
             return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);     // one copy per batch: packed on the device
@@ -707,6 +785,8 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
 static int dev_args_ok(tsgpu_ctx* c, int device_index, uint32_t flags, uint32_t chunk_size, uint64_t n, uint64_t slot_stride) {
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
     if (device_index < 0 || device_index >= (int)c->lanes.size()) return fail(TSGPU_E_ARG, "device_index %d out of range", device_index);
+    if (flags & TSGPU_FLAG_VERIFY)
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_VERIFY (%u) applies to the host-buffer transform calls only", TSGPU_FLAG_VERIFY);
     if ((flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)) == 0 || (flags & ~KNOWN_FLAGS)) return fail(TSGPU_E_ARG, "flags must name zstd and/or aes");
     if (chunk_size == 0 || chunk_size > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk_size out of range for this context");
     if (n == 0) return TSGPU_OK;
