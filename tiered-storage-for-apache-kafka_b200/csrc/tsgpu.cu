@@ -900,6 +900,17 @@ extern "C" int tsgpu_profile_report(tsgpu_ctx* c, char* out, uint32_t* out_len) 
     return TSGPU_OK;
 }
 
+#if ZB_TUNE_PHASES && !defined(TSGPU_SIMT)
+// Measurement builds only (-DZB_TUNE_PHASES=1): the speed-mode compressor's per-block phase records of the last launch
+// (ts::ZbPhases, indexed chunk * blocks_per_chunk + block), `bytes` of them from the start, into host memory.
+extern "C" int tsgpu_zb_phases(void* out, uint64_t bytes) {
+    if (!out || bytes > sizeof(ts::g_zb_phases)) return fail(TSGPU_E_ARG, "bad phase-record request");
+    RT(rt::device_sync());
+    RT(rt::err(cudaMemcpyFromSymbol(out, ts::g_zb_phases, bytes)));
+    return TSGPU_OK;
+}
+#endif
+
 // Which decode path the zstd frames of this context's calls took so far (summed over devices and work slots):
 // out[0] regions executed in shared memory, out[1] frames a region / block handed to the frame executor, out[2] frames executed
 // whole (libzstd-shaped), out[3] frames on the serial kernel, out[4] independent blocks executed by a warp each, out[5..7] 0.

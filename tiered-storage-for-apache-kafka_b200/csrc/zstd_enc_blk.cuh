@@ -4,7 +4,7 @@
 // different trade: every 8 KiB block is self-contained (own Huffman tree, own FSE tables, no match leaves the block), so a
 // 1 GiB segment is 131,072 independent warps with no barrier between them, 20 warps per SM.  That is the round-1 kernel with
 // the streamlined FSE chains and the backwards growth of taken matches ("catch up"); it compresses the K corpus ~3.1 : 1 at
-// ~16.7 ms per GiB on an H100, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
+// ~15.7 ms per GiB on an H100, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
 // window and one set of tables per 8 blocks).  TSGPU_FLAG_ZSTD picks this kernel, TSGPU_FLAG_ZSTD | TSGPU_FLAG_ZSTD_DENSE the region kernel;
 // the decoder reads both through the same region path (zstd_dec.cuh).
 //   zstd_enc_blocks_kernel    one WARP per block: block staged in shared memory; 32 positions hashed and verified per step
@@ -37,6 +37,9 @@ constexpr uint32_t ZB_HSIZE = 1u << ZB_HLOG;
 #ifndef ZB_TUNE_EXTLDS    // 1: the warp-wide extension of long matches reads shared memory with LDS word pairs instead of generic loads
 #define ZB_TUNE_EXTLDS 0  //    (H100: within 1 % of the generic loads, 16.5 vs 16.6 ms per GiB — off)
 #endif
+#ifndef ZB_TUNE_PHASES    // 1: every warp stamps clock64() at its block's phase boundaries into g_zb_phases, read back through
+#define ZB_TUNE_PHASES 0  //    tsgpu_zb_phases (scripts/enc_phases.py); measurement builds only, never the product
+#endif
 constexpr int ZB_WPB = ZB_TUNE_WPB;            // warps (= blocks in flight) per CTA
 constexpr uint32_t ZB_LANE_EXT = ZB_TUNE_LANE_EXT;   // bytes a lane extends its own match beyond the first 4
 constexpr uint32_t ZB_BUF_PAD = 416;           // zero pad for over-reads; its tail also holds the FSE tile scratch
@@ -51,12 +54,28 @@ struct ZbCTab {                                // per-warp FSE encoding tables (
     uint16_t st_ll[128], st_ml[128], st_of[128];
     zf::FseCSym sy_ll[ZE_NSYM_LL], sy_ml[ZE_NSYM_ML], sy_of[ZE_NSYM_OF];
 };
-static_assert(sizeof(ZbCTab) <= ZB_HSIZE * 2 && 2048 <= ZB_HSIZE * 2, "FSE tables and the 2 KiB Huffman scratch alias the hash-table area");
+static_assert(sizeof(ZbCTab) + sizeof(ZeCodeTabs) <= ZB_HSIZE * 2 && 2048 <= ZB_HSIZE * 2,
+              "FSE tables + sequence code tables, and the 2 KiB Huffman scratch, alias the hash-table area");
 struct ZbFsePre { zf::PredefinedCTables t; };
 
+#if ZB_TUNE_PHASES
+// t[0] start, then the end of: 1 staging, 2 parse, 3 Huffman code table, 4 literals section, 5 FSE tables, 6 sequence
+// bit stream, 7 look-back, 8 copy into the frame.  A phase the block skips (raw literals, no sequences) keeps t = 0.
+struct ZbPhases { unsigned long long t[9]; uint32_t nseq, nlit, nsym, pad; };
+constexpr uint32_t ZB_PHASES_MAX = 1u << 17;   // blocks of one launch recorded (chunk * blocks_per_chunk + block): 1 GiB
+__device__ ZbPhases g_zb_phases[ZB_PHASES_MAX];
+#define ZB_PH_PARAM , ZbPhases* ph
+#define ZB_PH_ARG , ph
+#define ZB_MARK(k) do { if (lane == 0 && ph) ph->t[k] = clock64(); } while (0)
+#define ZB_NOTE(f, v) do { if (lane == 0 && ph) ph->f = (v); } while (0)
+#else
+#define ZB_PH_PARAM
+#define ZB_PH_ARG
+#define ZB_MARK(k) do {} while (0)
+#define ZB_NOTE(f, v) do {} while (0)
+#endif
+
 __device__ __forceinline__ uint32_t zb_hash(uint32_t v) { return (v * 2654435761u) >> (32 - ZB_HLOG); }
-__device__ __forceinline__ uint32_t zb_ll_code(uint32_t ll) { return ll < 64 ? g_seq_tables.ll_code[ll] : (uint32_t)zf::highbit32(ll) + 19; }
-__device__ __forceinline__ uint32_t zb_ml_code(uint32_t mlbase) { return mlbase < 128 ? g_seq_tables.ml_code[mlbase] : (uint32_t)zf::highbit32(mlbase) + 36; }
 
 struct ZstdBlkScratch {
     uint8_t* blk_out = nullptr;      // blocks * ZB_SLOT
@@ -97,21 +116,26 @@ __device__ __forceinline__ uint32_t zb_rle_literals(uint8_t v, uint32_t n, uint8
 // Returns the bytes written at `body`.  `work`: >= ZB + 160 bytes of shared memory (tree scratch, then the
 // stream staging area); `aux16`: 2 KiB of shared memory (histogram + code table).
 __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict__ lits, uint32_t n, uint8_t* body,
-                                                       uint32_t* work, uint16_t* aux16, uint32_t lane) {
+                                                       uint32_t* work, uint16_t* aux16, uint32_t lane ZB_PH_PARAM) {
     if (n < ZE_HUF_MIN) return zb_raw_literals(lits, n, body, lane);
     uint32_t* hist = (uint32_t*)aux16;         // [256]
     uint32_t* ctab = hist + 256;               // [256] code | len << 16
     uint32_t* keys = work + 1280;              // [256] used symbols: count << 8 | symbol
-    uint32_t* sorted = work;                   // [256]
-    uint32_t* nodew = work + 256;              // [512]
-    uint16_t* parent = (uint16_t*)(work + 768);   // [512]
-    uint8_t* depth = (uint8_t*)(work + 1024);  // [512]
     uint32_t* meta = work + 1200;              // small scalars shared by the warp
 
     for (uint32_t i = lane; i < 256; i += 32) { hist[i] = 0; ctab[i] = 0; }
     __syncwarp();
-    _Pragma("unroll 2")
-    for (uint32_t i = lane; i < n; i += 32) atomicAdd(&hist[lits[i]], 1u);
+    {   // 16 literals per load: the block's literal slot is 16-byte aligned and ZB bytes long
+        const uint4* l16 = (const uint4*)lits;
+        _Pragma("unroll 2")
+        for (uint32_t i = lane; i * 16 < n; i += 32) {
+            const uint4 q = l16[i];
+            const uint32_t w4[4] = {q.x, q.y, q.z, q.w};
+            _Pragma("unroll")
+            for (uint32_t k = 0; k < 16; k++)
+                if (i * 16 + k < n) atomicAdd(&hist[(w4[k >> 2] >> (8 * (k & 3))) & 0xff], 1u);
+        }
+    }
     __syncwarp();
 
     // compact the used symbols (8 per lane, ascending symbol order)
@@ -119,6 +143,7 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
     for (uint32_t k = 0; k < 8; k++) mine += hist[lane * 8 + k] ? 1u : 0u;
     const uint32_t inc = warp_inclusive_scan_u32(mine, lane);
     const uint32_t m = __shfl_sync(TS_FULL, inc, 31);
+    ZB_NOTE(nsym, m);
     {
         uint32_t at = inc - mine;
         for (uint32_t k = 0; k < 8; k++) { const uint32_t s = lane * 8 + k; if (hist[s]) keys[at++] = (hist[s] << 8) | s; }
@@ -139,77 +164,11 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
         if ((bits16 >> 7) + m / 2 + 16 >= n) return zb_raw_literals(lits, n, body, lane);   // >= n bytes even before rounding losses
     }
     const uint32_t last_sym = keys[m - 1] & 0xff;
-
-    // ---- code lengths: rebuild with halved counts until the tree is at most 11 deep
-    uint32_t max_len = 0;
-    for (uint32_t round = 0; round < 16; round++) {
-        for (uint32_t e = lane; e < m; e += 32) {                         // rank sort (keys are distinct)
-            const uint32_t key = keys[e];
-            uint32_t r = 0;
-            _Pragma("unroll 2")
-            for (uint32_t j = 0; j < m; j++) r += keys[j] < key ? 1u : 0u;
-            sorted[r] = key;
-        }
-        __syncwarp();
-        if (lane == 0) {
-            _Pragma("unroll 1")
-            for (uint32_t i = 0; i < m; i++) nodew[i] = sorted[i] >> 8;
-            uint32_t li = 0, ii = m, ni = m;
-            _Pragma("unroll 1")
-            for (uint32_t k = 0; k + 1 < m; k++) {
-                uint32_t a, b;
-                if (li < m && (ii >= ni || nodew[li] <= nodew[ii])) a = li++; else a = ii++;
-                if (li < m && (ii >= ni || nodew[li] <= nodew[ii])) b = li++; else b = ii++;
-                nodew[ni] = nodew[a] + nodew[b];
-                parent[a] = (uint16_t)ni; parent[b] = (uint16_t)ni;
-                ni++;
-            }
-            const uint32_t root = 2 * m - 2;
-            depth[root] = 0;
-            uint32_t mx = 0;
-            _Pragma("unroll 1")
-            for (int32_t i = (int32_t)root - 1; i >= 0; i--) {
-                depth[i] = (uint8_t)(depth[parent[i]] + 1);
-                if ((uint32_t)i < m && depth[i] > mx) mx = depth[i];
-            }
-            meta[0] = mx;
-        }
-        __syncwarp();
-        max_len = meta[0];
-        if (max_len <= (uint32_t)zf::HUF_MAX_LOG) break;
-        for (uint32_t e = lane; e < m; e += 32) {                         // flatten the distribution and retry
-            const uint32_t key = keys[e];
-            keys[e] = ((((key >> 8) + 1) >> 1) << 8) | (key & 0xff);
-        }
-        __syncwarp();
-    }
+    uint32_t total_bits;
+    const uint32_t max_len = ze_huf_codes(hist, m, last_sym, 16, ctab, work, &total_bits, lane);
     if (max_len > (uint32_t)zf::HUF_MAX_LOG) return zb_raw_literals(lits, n, body, lane);
-
-    // ---- canonical codes: weight w = max_len + 1 - len; cells are dealt weight-ascending, symbol-ascending
-    if (lane == 0) {
-        uint32_t cnt[16];
-        for (int w = 0; w < 16; w++) cnt[w] = 0;
-        _Pragma("unroll 1")
-        for (uint32_t i = 0; i < m; i++) cnt[max_len + 1 - depth[i]]++;
-        uint32_t start[16], pos = 0;
-        for (uint32_t w = 1; w <= max_len; w++) { start[w] = pos; pos += cnt[w] << (w - 1); }
-        // sorted[] is ordered by count; symbol order inside a weight class comes from walking symbols ascending
-        _Pragma("unroll 1")
-        for (uint32_t i = 0; i < m; i++) ctab[sorted[i] & 0xff] = (uint32_t)depth[i] << 16;      // park the length
-        uint64_t total_bits = 0;
-        _Pragma("unroll 1")
-        for (uint32_t s = 0; s <= last_sym; s++) {
-            const uint32_t len = ctab[s] >> 16;
-            if (!len) continue;
-            const uint32_t w = max_len + 1 - len;
-            ctab[s] = (start[w] >> (w - 1)) | (len << 16);
-            start[w] += 1u << (w - 1);
-            total_bits += (uint64_t)len * hist[s];
-        }
-        meta[1] = (uint32_t)total_bits;
-    }
-    __syncwarp();
-    const uint32_t nweights = last_sym;                                   // symbols 0 .. last_sym-1 are listed
+    ZB_MARK(3);
+    const uint32_t nweights = last_sym;                                 // symbols 0 .. last_sym-1 are listed
     // Tree description: direct 4-bit weights (at most 128 of them) or FSE-compressed weights (RFC 8878 §4.2.1.1);
     // the shorter wins.  The FSE form is what lets alphabets above byte value 128 (binary payloads) be Huffman-coded.
     uint32_t tree_bytes = nweights <= 128 ? 1 + (nweights + 1) / 2 : 0xffffffffu;
@@ -237,24 +196,26 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
                 if (lane == 0) {                                          // two interleaved states, last weight first
                     uint8_t* o = wdesc + 1 + dsz;
                     uint64_t acc = 0; uint32_t nb = 0, ob = 0;
-                    uint32_t st[2];
+                    uint32_t st_even = 0, st_odd = 0;                     // the chains of the even and the odd weights
                     for (uint32_t q = 0; q < 2; q++) {                    // FSE_initCState2 for the two last weights
                         const uint32_t i = nweights - 1 - q;
                         const zf::FseCSym c = wsy[wts[i]];
                         const uint32_t nbo = (uint32_t)(c.delta_nb_bits + (1 << 15)) >> 16;
                         const uint32_t v = (nbo << 16) - (uint32_t)c.delta_nb_bits;
-                        st[i & 1] = wst[(int32_t)(v >> nbo) + c.delta_find_state];
+                        const uint32_t s0 = wst[(int32_t)(v >> nbo) + c.delta_find_state];
+                        if (i & 1) st_odd = s0; else st_even = s0;
                     }
                     for (int32_t i = (int32_t)nweights - 3; i >= 0; i--) {
                         const zf::FseCSym c = wsy[wts[i]];
-                        const uint32_t sv = st[i & 1];
+                        const uint32_t sv = (i & 1) ? st_odd : st_even;
                         const uint32_t nbo = (sv + (uint32_t)c.delta_nb_bits) >> 16;
                         acc |= (uint64_t)(sv & ((1u << nbo) - 1)) << nb; nb += nbo;
-                        st[i & 1] = wst[(int32_t)(sv >> nbo) + c.delta_find_state];
+                        const uint32_t s1 = wst[(int32_t)(sv >> nbo) + c.delta_find_state];
+                        if (i & 1) st_odd = s1; else st_even = s1;
                         while (nb >= 8) { o[ob++] = (uint8_t)acc; acc >>= 8; nb -= 8; }
                     }
-                    acc |= (uint64_t)(st[1] & ((1u << wk.log) - 1)) << nb; nb += wk.log;      // flush odd chain, then even chain
-                    acc |= (uint64_t)(st[0] & ((1u << wk.log) - 1)) << nb; nb += wk.log;
+                    acc |= (uint64_t)(st_odd & ((1u << wk.log) - 1)) << nb; nb += wk.log;     // flush odd chain, then even chain
+                    acc |= (uint64_t)(st_even & ((1u << wk.log) - 1)) << nb; nb += wk.log;
                     acc |= 1ull << nb; nb += 1;                                                // end mark
                     while (nb > 0) { o[ob++] = (uint8_t)acc; acc >>= 8; nb = nb >= 8 ? nb - 8 : 0; }
                     meta[2] = dsz + ob;
@@ -271,7 +232,7 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
     }
     if (tree_bytes == 0xffffffffu) return zb_raw_literals(lits, n, body, lane);   // neither form can describe this tree
     const bool fse_weights = wdesc[0] != 0xff;
-    const uint32_t est = tree_bytes + 6 + (meta[1] >> 3) + 8;
+    const uint32_t est = tree_bytes + 6 + (total_bits >> 3) + 8;
     if (est + 5 >= n) return zb_raw_literals(lits, n, body, lane);        // Huffman would not pay
 
     // ---- the four streams, staged in `work` (cleared first; tree scratch is dead from here on)
@@ -279,29 +240,30 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
     __syncwarp();
     for (uint32_t i = lane; i < (ZB + 128) / 4; i += 32) work[i] = 0;
     __syncwarp();
-    uint32_t byte_pos = 0;
-    uint64_t ssz_all = 0;                                                 // four 16-bit stream sizes
-    _Pragma("unroll 1")
+    // this lane's run [ra, rb) of each stream (32 runs per stream, symbols written last-to-first: the offset of a run is the
+    // number of bits of all LATER runs); the loads of the four runs go out together, once to size them and once to encode
+    uint32_t ra[4], rb[4], rbits[4];
+    _Pragma("unroll")
     for (uint32_t st = 0; st < 4; st++) {
         const uint32_t s0 = st * seg, s1 = st < 3 ? min(n, s0 + seg) : n;
         const uint32_t cnt = s1 > s0 ? s1 - s0 : 0;
         const uint32_t per = (cnt + 31) / 32;
-        const uint32_t a = min(cnt, lane * per), b = min(cnt, a + per);   // this lane's run [a, b) of the stream
-        uint32_t mybits = 0;
-        _Pragma("unroll 2")
-        for (uint32_t i = a; i < b; i++) mybits += ctab[lits[s0 + i]] >> 16;
-        // symbols are written last-to-first: the offset of a run is the number of bits of all LATER runs
-        const uint32_t incb = warp_inclusive_scan_u32(mybits, lane);
+        ra[st] = s0 + min(cnt, lane * per); rb[st] = s0 + min(cnt, lane * per + per); rbits[st] = 0;
+    }
+    const uint32_t per0 = (seg + 31) / 32;                                // the longest run (stream 0 is full)
+    _Pragma("unroll 2")
+    for (uint32_t k = 0; k < per0; k++) {
+        _Pragma("unroll")
+        for (uint32_t st = 0; st < 4; st++) if (ra[st] + k < rb[st]) rbits[st] += ctab[lits[ra[st] + k]] >> 16;
+    }
+    uint32_t off[4];
+    uint32_t byte_pos = 0;
+    uint64_t ssz_all = 0;                                                 // four 16-bit stream sizes
+    _Pragma("unroll")
+    for (uint32_t st = 0; st < 4; st++) {
+        const uint32_t incb = warp_inclusive_scan_u32(rbits[st], lane);
         const uint32_t total = __shfl_sync(TS_FULL, incb, 31);
-        uint32_t off = byte_pos * 8 + (total - incb);
-        for (uint32_t i = b; i > a; i--) {
-            const uint32_t c = ctab[lits[s0 + i - 1]];
-            const uint32_t len = c >> 16, code = c & 0xffff;
-            const uint32_t w = off >> 5, sh = off & 31;
-            atomicOr(&work[w], code << sh);
-            if (sh + len > 32) atomicOr(&work[w + 1], code >> (32 - sh));
-            off += len;
-        }
+        off[st] = byte_pos * 8 + (total - incb);
         if (lane == 0) {                                                  // end mark
             const uint32_t o = byte_pos * 8 + total;
             atomicOr(&work[o >> 5], 1u << (o & 31));
@@ -309,8 +271,22 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
         const uint32_t sz = (total + 1 + 7) >> 3;
         ssz_all |= (uint64_t)sz << (16 * st);
         byte_pos += sz;
-        __syncwarp();
     }
+    _Pragma("unroll 2")
+    for (uint32_t k = 0; k < per0; k++) {
+        _Pragma("unroll")
+        for (uint32_t st = 0; st < 4; st++) {
+            if (ra[st] + k < rb[st]) {
+                const uint32_t c = ctab[lits[rb[st] - 1 - k]];
+                const uint32_t len = c >> 16, code = c & 0xffff;
+                const uint32_t w = off[st] >> 5, sh = off[st] & 31;
+                atomicOr(&work[w], code << sh);
+                if (sh + len > 32) atomicOr(&work[w + 1], code >> (32 - sh));
+                off[st] += len;
+            }
+        }
+    }
+    __syncwarp();
     const uint32_t comp = tree_bytes + 6 + byte_pos;
     const uint32_t hsz = (n < 1024 && comp < 1024) ? 3u : (n < 16384 && comp < 16384) ? 4u : 5u;
     if (hsz + comp >= 3 + n) return zb_raw_literals(lits, n, body, lane);
@@ -348,8 +324,9 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
 // descriptions go straight to `hdr_out` (global), the bit stream is staged in the word buffer `bits` (shared).
 // Returns the bit-stream bytes; *desc_bytes = 1 (modes byte) + table descriptions.  Warp-uniform, N >= 1.
 __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict__ seqs, uint32_t N, uint32_t* bits, ZbCTab* ct,
+                                                        const ZeCodeTabs* tabs,
                                                         uint2* pk /*[3][32]*/, uint32_t* sb /*[3][32]*/,
-                                                        const ZbFsePre* fs, uint8_t* hdr_out, uint32_t* desc_bytes, uint32_t lane) {
+                                                        const ZbFsePre* fs, uint8_t* hdr_out, uint32_t* desc_bytes, uint32_t lane ZB_PH_PARAM) {
     // ---- pass 1: code histograms (then normalised counts), in the word buffer beyond ze_build_kind's own scratch
     uint32_t* cnt = bits + 256;
     for (uint32_t i = lane; i < ZE_NSYM_LL + ZE_NSYM_ML + ZE_NSYM_OF; i += 32) cnt[i] = 0;
@@ -360,8 +337,8 @@ __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict_
         const uint2 s = pre;
         if (j + 32 < N) pre = seqs[j + 32];                  // next tile in flight while this one is counted
         if (j < N) {
-            atomicAdd(&cnt[zb_ll_code(s.x & 0xffff)], 1u);
-            atomicAdd(&cnt[ZE_NSYM_LL + zb_ml_code(s.x >> 16)], 1u);
+            atomicAdd(&cnt[ze_ll_code_s(tabs, s.x & 0xffff)], 1u);
+            atomicAdd(&cnt[ZE_NSYM_LL + ze_ml_code_s(tabs, s.x >> 16)], 1u);
             atomicAdd(&cnt[ZE_NSYM_LL + ZE_NSYM_ML + (uint32_t)zf::highbit32(s.y + 3)], 1u);
         }
     }
@@ -380,6 +357,7 @@ __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict_
     __syncwarp();
     for (uint32_t i = lane; i < (ZB + ZB_BUF_PAD) / 4; i += 32) bits[i] = 0;
     __syncwarp();
+    ZB_MARK(5);
 
     // ---- pass 2: encode.  Per tile of 32 sequences every lane looks up the transforms of its sequence's three codes;
     // lanes 0-2 then walk the three state chains (one 8-byte load, the bit count, one store, one table load per symbol).
@@ -398,7 +376,7 @@ __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict_
         if (j + 32 < N) pre = seqs[N - 1 - (j + 32)];
         if (have) {
             ll = s.x & 0xffff; mlb = s.x >> 16; offb = s.y + 3;       // mlb = matchLength - 3, offb = offset + 3 (no repcodes)
-            llc = zb_ll_code(ll); mlc = zb_ml_code(mlb); ofc = (uint32_t)zf::highbit32(offb);
+            llc = ze_ll_code_s(tabs, ll); mlc = ze_ml_code_s(tabs, mlb); ofc = (uint32_t)zf::highbit32(offb);
             const zf::FseCSym a = ct->sy_of[ofc], b = ct->sy_ml[mlc], c = ct->sy_ll[llc];
             pk[lane] = make_uint2((uint32_t)a.delta_nb_bits, (uint32_t)a.delta_find_state);
             pk[32 + lane] = make_uint2((uint32_t)b.delta_nb_bits, (uint32_t)b.delta_find_state);
@@ -431,7 +409,7 @@ __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict_
         __syncwarp();
         uint64_t field = 0; uint32_t nb = 0;
         if (have) {
-            const uint32_t llb = g_seq_tables.ll_bits[llc], mlbits = g_seq_tables.ml_bits[mlc];
+            const uint32_t llb = tabs->ll_bits[llc], mlbits = tabs->ml_bits[mlc];
             // order inside a field (first written = lowest bits): OF state, ML state, LL state, LL extra, ML extra, OF extra
             const uint32_t b0 = sb[lane], b1 = sb[32 + lane], b2 = sb[64 + lane];
             field = b0 & 0xffff; nb = b0 >> 16;
@@ -463,7 +441,7 @@ __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict_
 }
 
 
-__global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __grid_constant__ ZstdBlkArgs A) {
+__global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const __grid_constant__ ZstdBlkArgs A) {
 // Common prologue of the block kernels (included inside a __global__ function body; see zstd_enc.cuh): which block this
 // warp owns, its scratch slots and its shared-memory window.
     TS_DYN_SMEM(smem);
@@ -496,6 +474,10 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
     uint16_t* ht = (uint16_t*)(wbase + ZB + ZB_BUF_PAD);
     uint2* pk = (uint2*)(buf + ZB_SEQ_AUX_OFF);
     uint32_t* sb = (uint32_t*)(pk + 96);
+#if ZB_TUNE_PHASES
+    ZbPhases* ph = gblk < ZB_PHASES_MAX ? &g_zb_phases[gblk] : nullptr;
+    if (lane == 0 && ph) { *ph = ZbPhases{}; ph->t[0] = clock64(); }
+#endif
 // Stage + LZ parse of one 8 KiB block (included inside a __global__ function body after
 // zstd_enc_prologue.inc).  Leaves nseq sequences in `seqs`, nlit literals in `lits`.
     // ---- stage the block in shared memory (128-bit loads when the source is aligned), zero the pad, reset the table
@@ -512,6 +494,7 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
     for (uint32_t i = bn + lane; i < ZB + ZB_BUF_PAD; i += 32) buf[i] = 0;
     for (uint32_t i = lane; i < ZB_HSIZE / 2; i += 32) ((uint32_t*)ht)[i] = 0;
     __syncwarp();
+    ZB_MARK(1);
 
     // ---- phase A: greedy LZ parse, 32 positions per step
     // Selection (which of the 32 candidate matches survive, left to right) is the only serial part and costs a
@@ -652,6 +635,9 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
     }
     __syncwarp();
     __threadfence_block();
+    ZB_MARK(2);
+    ZB_NOTE(nseq, nseq);
+    ZB_NOTE(nlit, nlit);
 // Entropy stage + emission of one block (included inside a __global__ function body after zstd_enc_prologue.inc; needs
 // nseq / nlit).  `buf` and `ht` are scratch here: the block's bytes are no longer needed in shared memory.
     // ---- phase B: entropy stage into the (now free) shared block buffer, then emit
@@ -659,8 +645,9 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
     {
         // literals section first (into `out` directly), then the sequences bit stream staged in `buf`
         uint8_t* body = out + 3;
-        const uint32_t lit_bytes = zb_encode_literals(lits, nlit, body, (uint32_t*)buf, ht, lane);   // header + payload
+        const uint32_t lit_bytes = zb_encode_literals(lits, nlit, body, (uint32_t*)buf, ht, lane ZB_PH_ARG);   // header + payload
         __syncwarp();
+        ZB_MARK(4);
         if (nseq == 0) {
             // no match at all: the block may still be worth a compressed block with entropy-coded literals and zero sequences
             if (lit_bytes + 1 < bn) {
@@ -671,7 +658,17 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
             const uint32_t shdr = nseq < 128 ? 1u : (nseq < 0x7f00 ? 2u : 3u);
             uint8_t* sp = body + lit_bytes;
             uint32_t desc_bytes = 0;
-            const uint32_t sbytes = zb_encode_sequences(seqs, nseq, (uint32_t*)buf, (ZbCTab*)ht, pk, sb, &fs, sp + shdr, &desc_bytes, lane);
+            // the code tables of the sequence fields go next to the FSE tables, over the (now dead) Huffman scratch
+            ZeCodeTabs* tabs = (ZeCodeTabs*)((uint8_t*)ht + sizeof(ZbCTab));
+            for (uint32_t i = lane; i < 128; i += 32) {
+                if (i < 64) tabs->ll_code[i] = g_seq_tables.ll_code[i];
+                tabs->ml_code[i] = g_seq_tables.ml_code[i];
+                if (i < 36) tabs->ll_bits[i] = g_seq_tables.ll_bits[i];
+                if (i < 53) tabs->ml_bits[i] = g_seq_tables.ml_bits[i];
+            }
+            __syncwarp();
+            const uint32_t sbytes = zb_encode_sequences(seqs, nseq, (uint32_t*)buf, (ZbCTab*)ht, tabs, pk, sb, &fs, sp + shdr, &desc_bytes, lane ZB_PH_ARG);
+            ZB_MARK(6);
             const uint32_t total = lit_bytes + shdr + desc_bytes + sbytes;
             if (total < bn) {
                 if (lane == 0) {
@@ -707,7 +704,9 @@ __global__ void __launch_bounds__(ZB_WPB * 32) zstd_enc_blocks_kernel(const __gr
         const uint32_t base = ze_lookback(st, blk, bsize_all, ze_frame_header_size(clen), last_block, lane);
         if (last_block && lane == 0) A.out_len[chunk] = base + bsize_all;
         __syncwarp();
+        ZB_MARK(7);
         ze_warp_copy(frame + base, out, bsize_all, lane);
+        ZB_MARK(8);
     }
 }
 

@@ -29,14 +29,118 @@ struct ZeHuf {                                 // region-wide result of ze_huf_b
     uint8_t desc[132];                         // header byte + weights (direct: <= 1 + 64; FSE-compressed: <= 1 + 127)
 };
 
+// Code lengths and canonical codes of a Huffman tree over the m >= 2 used symbols, one warp.  keys[] (at work + 1280: count << 8 |
+// symbol for each used symbol, distinct) is rewritten with halved counts while the tree is deeper than 11 levels, at most
+// `max_rounds` times.  On success ctab[s] = code | len << 16 for every used symbol (ctab must be zero on entry), *total_bits =
+// sum of len * hist[s], and the result is max_len <= HUF_MAX_LOG; otherwise the result is larger and ctab is untouched.
+//   rank sort of the keys (lane-parallel) -> two-queue merge on lane 0 (queue heads in registers; ties take the leaf, which
+//   the format of the frames depends on) -> depths by pointer jumping over parent[] (ceil(log2(m - 1)) warp rounds) ->
+//   canonical codes, weight ascending then symbol ascending: the first code of each weight class from a scan of the class
+//   sizes, then 32 symbols per step, each taking its class's next code plus its rank among the step's symbols of its class.
+// work: >= 1296 words of shared memory.
+__device__ __forceinline__ uint32_t ze_huf_codes(const uint32_t* hist, uint32_t m, uint32_t last_sym, uint32_t max_rounds,
+                                                 uint32_t* ctab, uint32_t* work, uint32_t* total_bits, uint32_t lane) {
+    uint32_t* keys = work + 1280;              // [256]
+    uint32_t* sorted = work;                   // [256]
+    uint32_t* nodew = work + 256;              // [512] node weights while merging
+    uint16_t* anc1 = (uint16_t*)(work + 256);  // [512] then (dead weights) the second buffer of the pointer jumping
+    uint8_t* dep1 = (uint8_t*)(work + 512);    // [512]
+    uint16_t* anc0 = (uint16_t*)(work + 768);  // [512] parent[], then the first buffer
+    uint8_t* dep0 = (uint8_t*)(work + 1024);   // [512]
+    uint32_t* wcnt = work + 1200;              // [16] symbols per weight class
+    const uint32_t root = 2 * m - 2;
+    const uint32_t jumps = m <= 2 ? 0u : 32u - (uint32_t)__clz((int)(m - 2));   // 2^jumps >= m - 1 >= any depth
+    uint32_t max_len = 0xffu;
+    const uint8_t* depth = dep0;
+    for (uint32_t round = 0; round < max_rounds; round++) {
+        for (uint32_t e = lane; e < m; e += 32) {                         // rank sort (keys are distinct)
+            const uint32_t key = keys[e];
+            uint32_t r = 0;
+            _Pragma("unroll 2")
+            for (uint32_t j = 0; j < m; j++) r += keys[j] < key ? 1u : 0u;
+            sorted[r] = key;
+            nodew[r] = key >> 8;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            uint32_t li = 0, ii = m, ni = m;
+            uint32_t wl = nodew[0], wi = 0;                               // heads of the leaf and internal-node queues
+            _Pragma("unroll 1")
+            for (uint32_t k = 0; k + 1 < m; k++) {
+                uint32_t a, b, wa, wb;
+                if (li < m && (ii >= ni || wl <= wi)) { a = li++; wa = wl; wl = nodew[li]; } else { a = ii++; wa = wi; wi = nodew[ii]; }
+                if (li < m && (ii >= ni || wl <= wi)) { b = li++; wb = wl; wl = nodew[li]; } else { b = ii++; wb = wi; wi = nodew[ii]; }
+                nodew[ni] = wa + wb;
+                anc0[a] = (uint16_t)ni; anc0[b] = (uint16_t)ni;
+                if (ii == ni) wi = wa + wb;                               // the new node heads an empty queue
+                ni++;
+            }
+            anc0[root] = (uint16_t)root;
+        }
+        __syncwarp();
+        // depth = edges to the root: dep holds the distance to anc, both double each round until every anc is the root
+        for (uint32_t e = lane; e <= root; e += 32) dep0[e] = e == root ? 0 : 1;
+        __syncwarp();
+        const uint16_t* ai = anc0; const uint8_t* di = dep0;
+        uint16_t* ao = anc1; uint8_t* dn = dep1;
+        for (uint32_t j = 0; j < jumps; j++) {
+            for (uint32_t e = lane; e <= root; e += 32) { const uint32_t a = ai[e]; dn[e] = (uint8_t)(di[e] + di[a]); ao[e] = ai[a]; }
+            __syncwarp();
+            const uint16_t* ta = ai; const uint8_t* td = di;
+            ai = ao; di = dn; ao = (uint16_t*)ta; dn = (uint8_t*)td;
+        }
+        depth = di;
+        uint32_t mx = 0;
+        for (uint32_t e = lane; e < m; e += 32) mx = max(mx, (uint32_t)di[e]);
+        max_len = __reduce_max_sync(TS_FULL, mx);
+        if (max_len <= (uint32_t)zf::HUF_MAX_LOG) break;
+        for (uint32_t e = lane; e < m; e += 32) {                         // flatten the distribution and retry
+            const uint32_t key = keys[e];
+            keys[e] = ((((key >> 8) + 1) >> 1) << 8) | (key & 0xff);
+        }
+        __syncwarp();
+    }
+    if (max_len > (uint32_t)zf::HUF_MAX_LOG) return max_len;
+
+    // ---- canonical codes: weight w = max_len + 1 - len; cells are dealt weight-ascending, symbol-ascending
+    if (lane < 16) wcnt[lane] = 0;
+    __syncwarp();
+    uint32_t tb = 0;
+    for (uint32_t i = lane; i < m; i += 32) {
+        const uint32_t s = sorted[i] & 0xff, len = depth[i];
+        ctab[s] = len << 16;                                              // park the length
+        atomicAdd(&wcnt[max_len + 1 - len], 1u);
+        tb += len * hist[s];
+    }
+    *total_bits = __reduce_add_sync(TS_FULL, tb);
+    __syncwarp();
+    // lane w (1 .. max_len) keeps the next code of weight class w
+    const bool cls = lane >= 1 && lane <= max_len;
+    const uint32_t cells = cls ? wcnt[lane] << (lane - 1) : 0u;
+    const uint32_t inc = warp_inclusive_scan_u32(cells, lane);
+    uint32_t next = cls ? (inc - cells) >> (lane - 1) : 0u;
+    const uint32_t lt = (1u << lane) - 1;
+    for (uint32_t s0 = 0; s0 <= last_sym; s0 += 32) {
+        const uint32_t s = s0 + lane;
+        const uint32_t len = ctab[s] >> 16;
+        const uint32_t w = len ? max_len + 1 - len : 0u;
+        const uint32_t first = __shfl_sync(TS_FULL, next, w);
+        uint32_t rank = 0;
+        for (uint32_t c = 1; c <= max_len; c++) {
+            const uint32_t bm = __ballot_sync(TS_FULL, w == c);
+            if (w == c) rank = (uint32_t)__popc(bm & lt);
+            if (lane == c) next += (uint32_t)__popc(bm);
+        }
+        if (len) ctab[s] = (first + rank) | (len << 16);
+    }
+    __syncwarp();
+    return max_len;
+}
+
 // Region-wide tree.  hist[256] (counts, destroyed), ctab[256] out (code | len << 16, 0 = unused symbol), work: >= 7.5 KiB of
 // shared-memory scratch, n = literals in the region.  One warp.
 __device__ TS_NOINLINE void ze_huf_build(uint32_t* hist, uint32_t* ctab, uint32_t* work, uint32_t n, ZeHuf* hf, uint32_t lane) {
     uint32_t* keys = work + 1280;              // [256] used symbols: count << 8 | symbol
-    uint32_t* sorted = work;                   // [256]
-    uint32_t* nodew = work + 256;              // [512]
-    uint16_t* parent = (uint16_t*)(work + 768);   // [512]
-    uint8_t* depth = (uint8_t*)(work + 1024);  // [512]
     uint32_t* meta = work + 1200;              // small scalars shared by the warp
     if (lane == 0) { hf->ok = 0; hf->tree_bytes = 0; hf->max_len = 0; }
     for (uint32_t i = lane; i < 256; i += 32) ctab[i] = 0;
@@ -70,73 +174,9 @@ __device__ TS_NOINLINE void ze_huf_build(uint32_t* hist, uint32_t* ctab, uint32_
         if ((bits16 >> 7) + m / 2 + 16 >= n) return;                      // >= n bytes even before rounding losses
     }
     const uint32_t last_sym = keys[m - 1] & 0xff;
-
-    // ---- code lengths: rebuild with halved counts until the tree is at most 11 deep
-    uint32_t max_len = 0;
-    for (uint32_t round = 0; round < 20; round++) {
-        for (uint32_t e = lane; e < m; e += 32) {                         // rank sort (keys are distinct)
-            const uint32_t key = keys[e];
-            uint32_t r = 0;
-            _Pragma("unroll 2")
-            for (uint32_t j = 0; j < m; j++) r += keys[j] < key ? 1u : 0u;
-            sorted[r] = key;
-        }
-        __syncwarp();
-        if (lane == 0) {
-            _Pragma("unroll 1")
-            for (uint32_t i = 0; i < m; i++) nodew[i] = sorted[i] >> 8;
-            uint32_t li = 0, ii = m, ni = m;
-            _Pragma("unroll 1")
-            for (uint32_t k = 0; k + 1 < m; k++) {
-                uint32_t a, b;
-                if (li < m && (ii >= ni || nodew[li] <= nodew[ii])) a = li++; else a = ii++;
-                if (li < m && (ii >= ni || nodew[li] <= nodew[ii])) b = li++; else b = ii++;
-                nodew[ni] = nodew[a] + nodew[b];
-                parent[a] = (uint16_t)ni; parent[b] = (uint16_t)ni;
-                ni++;
-            }
-            const uint32_t root = 2 * m - 2;
-            depth[root] = 0;
-            uint32_t mx = 0;
-            _Pragma("unroll 1")
-            for (int32_t i = (int32_t)root - 1; i >= 0; i--) {
-                depth[i] = (uint8_t)(depth[parent[i]] + 1);
-                if ((uint32_t)i < m && depth[i] > mx) mx = depth[i];
-            }
-            meta[0] = mx;
-        }
-        __syncwarp();
-        max_len = meta[0];
-        if (max_len <= (uint32_t)zf::HUF_MAX_LOG) break;
-        for (uint32_t e = lane; e < m; e += 32) {                         // flatten the distribution and retry
-            const uint32_t key = keys[e];
-            keys[e] = ((((key >> 8) + 1) >> 1) << 8) | (key & 0xff);
-        }
-        __syncwarp();
-    }
+    uint32_t total_bits;
+    const uint32_t max_len = ze_huf_codes(hist, m, last_sym, 20, ctab, work, &total_bits, lane);
     if (max_len > (uint32_t)zf::HUF_MAX_LOG) return;
-
-    // ---- canonical codes: weight w = max_len + 1 - len; cells are dealt weight-ascending, symbol-ascending
-    if (lane == 0) {
-        uint32_t cnt[16];
-        for (int w = 0; w < 16; w++) cnt[w] = 0;
-        _Pragma("unroll 1")
-        for (uint32_t i = 0; i < m; i++) cnt[max_len + 1 - depth[i]]++;
-        uint32_t start[16], pos = 0;
-        for (uint32_t w = 1; w <= max_len; w++) { start[w] = pos; pos += cnt[w] << (w - 1); }
-        // sorted[] is ordered by count; symbol order inside a weight class comes from walking symbols ascending
-        _Pragma("unroll 1")
-        for (uint32_t i = 0; i < m; i++) ctab[sorted[i] & 0xff] = (uint32_t)depth[i] << 16;      // park the length
-        _Pragma("unroll 1")
-        for (uint32_t s = 0; s <= last_sym; s++) {
-            const uint32_t len = ctab[s] >> 16;
-            if (!len) continue;
-            const uint32_t w = max_len + 1 - len;
-            ctab[s] = (start[w] >> (w - 1)) | (len << 16);
-            start[w] += 1u << (w - 1);
-        }
-    }
-    __syncwarp();
     const uint32_t nweights = last_sym;                                   // symbols 0 .. last_sym-1 are listed
     // Tree description: direct 4-bit weights (at most 128 of them) or FSE-compressed weights (RFC 8878 §4.2.1.1);
     // the shorter wins.  The FSE form is what lets alphabets above byte value 128 (binary payloads) be Huffman-coded.
