@@ -148,7 +148,6 @@ __device__ __forceinline__ void ze_insert_max(uint16_t* ht, uint32_t h, uint32_t
 namespace ts {
 
 // ------------------------------------------------------------------------------------------ region-wide state (shared memory)
-struct ZeFsePre { zf::PredefinedCTables t; };   // view of the predefined encoding tables in constant memory
 struct ZeRegion {                    // lives in the ctl area
     uint32_t nseq[ZR_SLICES], nlit[ZR_SLICES];
     ZeLitBlock lit[ZR_SLICES];
@@ -179,31 +178,55 @@ constexpr uint32_t ZE_KIND_SCRATCH = 1024;     // per FSE kind in the ht_fin are
 static_assert(8192 + 3 * ZE_KIND_SCRATCH <= ZE_HTH_BYTES, "tree scratch (7.5 KiB) + three table scratches must fit the history-table area");
 
 // ------------------------------------------------------------------------------------------ sequences of one block
-// Code histograms of one block's sequences, added to the region's counters (shared-memory atomics).
-__device__ __forceinline__ void ze_seq_hist(const uint2* __restrict__ seqs, uint32_t N, uint32_t* cnt, const uint8_t* ll_code, const uint8_t* ml_code, uint32_t lane) {
+// Code histograms of one block's sequences, added to cnt (LL, ML, OF back to back; shared-memory atomics).
+__device__ __forceinline__ void ze_seq_hist(const uint2* __restrict__ seqs, uint32_t N, uint32_t* cnt, const ZeCodeTabs* tabs, uint32_t lane) {
     uint2 pre = lane < N ? seqs[lane] : make_uint2(0, 0);
     for (uint32_t t0 = 0; t0 < N; t0 += 32) {
         const uint32_t j = t0 + lane;
         const uint2 s = pre;
         if (j + 32 < N) pre = seqs[j + 32];                  // next tile in flight while this one is counted
         if (j < N) {
-            const uint32_t ll = s.x & 0xffff, mlb = s.x >> 16;
-            atomicAdd(&cnt[ll < 64 ? ll_code[ll] : (uint32_t)zf::highbit32(ll) + 19], 1u);
-            atomicAdd(&cnt[ZE_NSYM_LL + (mlb < 128 ? ml_code[mlb] : (uint32_t)zf::highbit32(mlb) + 36)], 1u);
+            atomicAdd(&cnt[ze_ll_code_s(tabs, s.x & 0xffff)], 1u);
+            atomicAdd(&cnt[ZE_NSYM_LL + ze_ml_code_s(tabs, s.x >> 16)], 1u);
             atomicAdd(&cnt[ZE_NSYM_LL + ZE_NSYM_ML + (uint32_t)zf::highbit32(s.y + 3)], 1u);
         }
     }
 }
 
-// Bit stream of one block's sequences with the region's tables, staged in the word buffer `bits` (shared, zeroed here).
-// Returns its size in bytes.  Warp-uniform, N >= 1.  Per tile of 32 sequences every lane looks up the transforms of its
-// sequence's three codes; lanes 0-2 then walk the three state chains (the only serial part: one 8-byte load, the bit
-// count, one store, one table load per symbol) and every lane packs its own field.
-__device__ __forceinline__ uint32_t ze_encode_seq_bits(const uint2* __restrict__ seqs, uint32_t N, uint32_t* bits, const ZeCTab* ct,
+// ze_build_kind for one sequence code, k = 0 LL, 1 OF, 2 ML (the order of the descriptions in the stream), from the histograms
+// in cnt (LL, ML, OF back to back) with the predefined tables as the Predefined_Mode choice.  CT: ZeCTab or a smaller table
+// set with the same members.
+template <class CT>
+__device__ __forceinline__ uint32_t ze_build_seq_kind(uint32_t k, uint32_t* cnt, uint32_t N, CT* ct, uint8_t* scratch, uint8_t* desc,
+                                                      ZeKind* kind, uint32_t lane) {
+    const zf::PredefinedCTables& pre = g_pre_ctables;
+    if (k == 0) return ze_build_kind(cnt, ZE_NSYM_LL, N, zf::LL_MAX_LOG, zf::LL_DEFAULT_LOG, pre.ll.state, pre.ll.sym,
+                                     ct->st_ll, ct->sy_ll, scratch, desc, kind, true, lane);
+    if (k == 1) return ze_build_kind(cnt + ZE_NSYM_LL + ZE_NSYM_ML, ZE_NSYM_OF, N, zf::OF_MAX_LOG, zf::OF_DEFAULT_LOG, pre.of.state,
+                                     pre.of.sym, ct->st_of, ct->sy_of, scratch, desc, kind, true, lane);
+    return ze_build_kind(cnt + ZE_NSYM_LL, ZE_NSYM_ML, N, zf::ML_MAX_LOG, zf::ML_DEFAULT_LOG, pre.ml.state, pre.ml.sym,
+                         ct->st_ml, ct->sy_ml, scratch, desc, kind, true, lane);
+}
+
+// Number_of_Sequences field: its size, and the field itself (one lane; returns the size)
+__device__ __forceinline__ uint32_t ze_nseq_size(uint32_t n) { return n < 128 ? 1u : n < 0x7f00 ? 2u : 3u; }
+__device__ __forceinline__ uint32_t ze_write_nseq(uint8_t* p, uint32_t n) {
+    if (n < 128) p[0] = (uint8_t)n;
+    else if (n < 0x7f00) { p[0] = (uint8_t)((n >> 8) + 0x80); p[1] = (uint8_t)n; }
+    else { p[0] = 0xff; p[1] = (uint8_t)(n - 0x7f00); p[2] = (uint8_t)((n - 0x7f00) >> 8); }
+    return ze_nseq_size(n);
+}
+
+// Bit stream of one block's sequences, staged in the word buffer `bits` (shared, zeroed by the caller), with the per-tile
+// scratch at ZE_SEQ_AUX_OFF.  Returns its size in bytes.  Warp-uniform, N >= 1.  Per tile of 32 sequences every lane looks
+// up the transforms of its sequence's three codes; lanes 0-2 then walk the three state chains (the only serial part: one
+// 8-byte load, the bit count, one store, one table load per symbol) and every lane packs its own field.  CT: as above.
+template <class CT>
+__device__ __forceinline__ uint32_t ze_encode_seq_bits(const uint2* __restrict__ seqs, uint32_t N, uint32_t* bits, const CT* ct,
                                                        const ZeCodeTabs* tabs, const ZeKind kll, const ZeKind kof, const ZeKind kml,
-                                                       uint2* pk /*[3][32]*/, uint32_t* sb /*[3][32]*/, uint32_t lane) {
-    for (uint32_t i = lane; i < ZE_STAGE / 4; i += 32) bits[i] = 0;
-    __syncwarp();
+                                                       uint32_t lane) {
+    uint2* pk = (uint2*)((uint8_t*)bits + ZE_SEQ_AUX_OFF);   // [3][32] transforms going in (OF, ML, LL)
+    uint32_t* sb = (uint32_t*)(pk + 96);                     // [3][32] state bits coming out: value | count << 16
     uint32_t bitpos = 0;
     uint32_t state = 0;                              // lanes 0..2: OF, ML, LL chains
     const uint16_t* st_tab = lane == 0 ? ct->st_of : lane == 1 ? ct->st_ml : ct->st_ll;
@@ -568,7 +591,7 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
     if (have_slice) {
         _Pragma("unroll 2")
         for (uint32_t i = lane; i < nlit; i += 32) atomicAdd(&S->hist[lits[i]], 1u);
-        ze_seq_hist(seqs, nseq, S->cnt, S->tabs.ll_code, S->tabs.ml_code, lane);
+        ze_seq_hist(seqs, nseq, S->cnt, &S->tabs, lane);
     }
     __syncthreads();
     uint32_t nseq_total = 0, nlit_total = 0;
@@ -580,16 +603,9 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
         if (w == 0) {
             ze_huf_build(S->hist, S->ctab, (uint32_t*)fin_area, nlit_total, &S->huf, lane);
         } else if (w <= 3 && nseq_total) {
-            const ZeFsePre& pre = *(const ZeFsePre*)&g_pre_ctables;
-            uint8_t* scratch = fin_area + 8192 + (w - 1) * ZE_KIND_SCRATCH;
             ZeKind k;
-            uint32_t dn;
-            if (w == 1) dn = ze_build_kind(S->cnt, ZE_NSYM_LL, nseq_total, zf::LL_MAX_LOG, zf::LL_DEFAULT_LOG, pre.t.ll.state, pre.t.ll.sym,
-                                           S->ct.st_ll, S->ct.sy_ll, scratch, S->desc[0], &k, true, lane);
-            else if (w == 2) dn = ze_build_kind(S->cnt + ZE_NSYM_LL + ZE_NSYM_ML, ZE_NSYM_OF, nseq_total, zf::OF_MAX_LOG, zf::OF_DEFAULT_LOG,
-                                                pre.t.of.state, pre.t.of.sym, S->ct.st_of, S->ct.sy_of, scratch, S->desc[1], &k, true, lane);
-            else dn = ze_build_kind(S->cnt + ZE_NSYM_LL, ZE_NSYM_ML, nseq_total, zf::ML_MAX_LOG, zf::ML_DEFAULT_LOG, pre.t.ml.state, pre.t.ml.sym,
-                                    S->ct.st_ml, S->ct.sy_ml, scratch, S->desc[2], &k, true, lane);
+            const uint32_t dn = ze_build_seq_kind(w - 1, S->cnt, nseq_total, &S->ct, fin_area + 8192 + (w - 1) * ZE_KIND_SCRATCH,
+                                                  S->desc[w - 1], &k, lane);
             if (lane == 0) {
                 S->desc_len[w - 1] = dn;
                 if (w == 1) R->kll = k; else if (w == 2) R->kof = k; else R->kml = k;
@@ -612,9 +628,9 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
         __syncwarp();
         uint32_t sbytes = 0;
         if (nseq) {
-            uint2* pk = (uint2*)(stage + ZE_SEQ_AUX_OFF);
-            uint32_t* sb = (uint32_t*)(pk + 96);
-            sbytes = ze_encode_seq_bits(seqs, nseq, (uint32_t*)stage, &S->ct, &S->tabs, R->kll, R->kof, R->kml, pk, sb, lane);
+            for (uint32_t i = lane; i < ZE_STAGE / 4; i += 32) ((uint32_t*)stage)[i] = 0;
+            __syncwarp();
+            sbytes = ze_encode_seq_bits(seqs, nseq, (uint32_t*)stage, &S->ct, &S->tabs, R->kll, R->kof, R->kml, lane);
             ze_warp_copy(slot_b, stage, sbytes, lane);
         }
         if (lane == 0) R->seq_bytes[w] = sbytes;
@@ -642,7 +658,7 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
                 const uint32_t comp = (tree_here ? S->huf.tree_bytes : 0) + 6 + lb.stream_bytes;
                 lit_sz = ze_lit_header_huf_size(lb.n, comp) + comp;
             }
-            const uint32_t shdr = nsq == 0 ? 1u : (nsq < 128 ? 1u : 2u) + 1u;      // Number_of_Sequences (+ modes byte)
+            const uint32_t shdr = ze_nseq_size(nsq) + (nsq ? 1u : 0u);            // Number_of_Sequences (+ modes byte)
             const uint32_t payload = lit_sz + shdr + (desc_here ? desc_total : 0) + R->seq_bytes[k];
             const bool raw = payload >= bn;                                  // would not shrink (with its duties): Raw_Block, state untouched
             const uint32_t bsize = 3 + (raw ? bn : payload);
@@ -691,23 +707,18 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
                 const uint32_t hsz = ze_lit_header_huf_size(lb.n, comp);
                 if (lane == 0) {
                     ze_lit_header_huf(body, my_lit_type, lb.n, comp);
-                    uint8_t* j = body + hsz + tb;
-                    j[0] = (uint8_t)lb.ssz[0]; j[1] = (uint8_t)(lb.ssz[0] >> 8); j[2] = (uint8_t)lb.ssz[1]; j[3] = (uint8_t)(lb.ssz[1] >> 8);
-                    j[4] = (uint8_t)lb.ssz[2]; j[5] = (uint8_t)(lb.ssz[2] >> 8);
+                    ze_lit_jump_table(body + hsz + tb, lb.ssz[0] | (lb.ssz[1] << 16) | ((uint64_t)lb.ssz[2] << 32));
                 }
                 for (uint32_t i = lane; i < tb; i += 32) body[hsz + i] = S->huf.desc[i];
                 ze_warp_copy(body + hsz + tb + 6, slot_a, lb.stream_bytes, lane);
                 at = hsz + comp;
             }
             uint8_t* sp = body + at;
-            if (nseq == 0) {
-                if (lane == 0) sp[0] = 0;                              // Number_of_Sequences = 0: the sequences section ends here
-            } else {
-                const uint32_t shdr = nseq < 128 ? 1u : 2u;
+            const uint32_t shdr = ze_nseq_size(nseq);
+            if (lane == 0) ze_write_nseq(sp, nseq);                    // 0: the sequences section ends here
+            if (nseq) {
                 uint32_t dn = 0;
                 if (lane == 0) {
-                    if (shdr == 1) sp[0] = (uint8_t)nseq;
-                    else { sp[0] = (uint8_t)((nseq >> 8) + 0x80); sp[1] = (uint8_t)nseq; }
                     // owner: the real modes + descriptions; the others repeat them (Predefined_Mode costs nothing to restate)
                     const uint32_t mll = R->kll.mode, mof = R->kof.mode, mml = R->kml.mode;
                     const uint32_t rll = mll == 0 ? 0u : 3u, rof = mof == 0 ? 0u : 3u, rml = mml == 0 ? 0u : 3u;

@@ -46,17 +46,14 @@ constexpr uint32_t ZB_BUF_PAD = 416;           // zero pad for over-reads; its t
 constexpr uint32_t ZB_SLOT = ZB + 512;         // per-block output slot: 3-byte header + payload
 constexpr uint32_t ZB_SMEM_WARP = ZB + ZB_BUF_PAD + ZB_HSIZE * 2;   // buf, ht
 constexpr uint32_t ZB_SMEM_WARP_AL = (ZB_SMEM_WARP + 15) & ~15u;
-// per-tile FSE scratch lives in the tail of `buf`: the sequence bit stream staged there is at most ZE_MAXSEQ * 58 bits
-constexpr uint32_t ZB_SEQ_AUX_OFF = 7456;
-static_assert(ZB_SEQ_AUX_OFF + 3 * 32 * 8 + 3 * 32 * 4 <= ZB + ZB_BUF_PAD && ZB_SEQ_AUX_OFF % 8 == 0, "FSE tile scratch must fit the block buffer");
-static_assert(ZE_MAXSEQ * 58 / 8 + 16 <= 7456, "sequence bit stream bound");
+// the sequence bit stream is staged in `buf`, its per-tile FSE scratch at ZE_SEQ_AUX_OFF in the tail
+static_assert(ZE_SEQ_AUX_OFF + 3 * 32 * 8 + 3 * 32 * 4 <= ZB + ZB_BUF_PAD, "FSE tile scratch must fit the block buffer");
 struct ZbCTab {                                // per-warp FSE encoding tables (logs <= 7 for <= 1024 sequences); aliases the hash-table area
     uint16_t st_ll[128], st_ml[128], st_of[128];
     zf::FseCSym sy_ll[ZE_NSYM_LL], sy_ml[ZE_NSYM_ML], sy_of[ZE_NSYM_OF];
 };
 static_assert(sizeof(ZbCTab) + sizeof(ZeCodeTabs) <= ZB_HSIZE * 2 && 2048 <= ZB_HSIZE * 2,
               "FSE tables + sequence code tables, and the 2 KiB Huffman scratch, alias the hash-table area");
-struct ZbFsePre { zf::PredefinedCTables t; };
 
 #if ZB_TUNE_PHASES
 // t[0] start, then the end of: 1 staging, 2 parse, 3 Huffman code table, 4 literals section, 5 FSE tables, 6 sequence
@@ -94,22 +91,9 @@ struct ZstdBlkArgs {
 
 // Raw_Literals_Block with the 3-byte header (Size_Format 11: 20-bit Regenerated_Size).
 __device__ TS_NOINLINE uint32_t zb_raw_literals(const uint8_t* __restrict__ lits, uint32_t n, uint8_t* body, uint32_t lane) {
-    if (lane == 0) {
-        body[0] = (uint8_t)((3u << 2) | ((n & 0xf) << 4));
-        body[1] = (uint8_t)(n >> 4);
-        body[2] = (uint8_t)(n >> 12);
-    }
+    if (lane == 0) ze_lit_header_raw(body, 0, n);
     for (uint32_t i = lane; i < n; i += 32) body[3 + i] = lits[i];
     return 3 + n;
-}
-__device__ __forceinline__ uint32_t zb_rle_literals(uint8_t v, uint32_t n, uint8_t* body, uint32_t lane) {
-    if (lane == 0) {
-        body[0] = (uint8_t)(1u | (3u << 2) | ((n & 0xf) << 4));
-        body[1] = (uint8_t)(n >> 4);
-        body[2] = (uint8_t)(n >> 12);
-        body[3] = v;
-    }
-    return 4;
 }
 
 
@@ -120,8 +104,6 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
     if (n < ZE_HUF_MIN) return zb_raw_literals(lits, n, body, lane);
     uint32_t* hist = (uint32_t*)aux16;         // [256]
     uint32_t* ctab = hist + 256;               // [256] code | len << 16
-    uint32_t* keys = work + 1280;              // [256] used symbols: count << 8 | symbol
-    uint32_t* meta = work + 1200;              // small scalars shared by the warp
 
     for (uint32_t i = lane; i < 256; i += 32) { hist[i] = 0; ctab[i] = 0; }
     __syncwarp();
@@ -138,100 +120,22 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
     }
     __syncwarp();
 
-    // compact the used symbols (8 per lane, ascending symbol order)
-    uint32_t mine = 0;
-    for (uint32_t k = 0; k < 8; k++) mine += hist[lane * 8 + k] ? 1u : 0u;
-    const uint32_t inc = warp_inclusive_scan_u32(mine, lane);
-    const uint32_t m = __shfl_sync(TS_FULL, inc, 31);
+    bool pays;
+    const uint32_t m = ze_huf_symbols(hist, n, work, &pays, lane);
     ZB_NOTE(nsym, m);
-    {
-        uint32_t at = inc - mine;
-        for (uint32_t k = 0; k < 8; k++) { const uint32_t s = lane * 8 + k; if (hist[s]) keys[at++] = (hist[s] << 8) | s; }
+    if (m == 1) {                                                         // RLE literals
+        if (lane == 0) { ze_lit_header_raw(body, 1, n); body[3] = (uint8_t)work[1280]; }
+        return 4;
     }
-    __syncwarp();
-    if (m == 1) return zb_rle_literals((uint8_t)(keys[0] & 0xff), n, body, lane);
-    {   // Shannon estimate in 1/16 bit units: sum c * (log2(n) - log2(c)), log2 by leading zeros + a linear fraction
-        uint32_t cost = 0;
-        for (uint32_t k = 0; k < 8; k++) {
-            const uint32_t c = hist[lane * 8 + k];
-            if (c) {
-                const uint32_t hb = (uint32_t)zf::highbit32(c);
-                const uint32_t lg16 = (hb << 4) + (((c << (31 - hb)) >> 27) & 15);       // ~ 16 * log2(c)
-                cost += c * (((uint32_t)zf::highbit32(n) << 4) + (((n << (31 - zf::highbit32(n))) >> 27) & 15) + 1 - lg16);
-            }
-        }
-        const uint32_t bits16 = __reduce_add_sync(TS_FULL, cost);
-        if ((bits16 >> 7) + m / 2 + 16 >= n) return zb_raw_literals(lits, n, body, lane);   // >= n bytes even before rounding losses
-    }
-    const uint32_t last_sym = keys[m - 1] & 0xff;
+    if (!pays) return zb_raw_literals(lits, n, body, lane);
+    const uint32_t last_sym = work[1280 + m - 1] & 0xff;
     uint32_t total_bits;
     const uint32_t max_len = ze_huf_codes(hist, m, last_sym, 16, ctab, work, &total_bits, lane);
     if (max_len > (uint32_t)zf::HUF_MAX_LOG) return zb_raw_literals(lits, n, body, lane);
     ZB_MARK(3);
-    const uint32_t nweights = last_sym;                                 // symbols 0 .. last_sym-1 are listed
-    // Tree description: direct 4-bit weights (at most 128 of them) or FSE-compressed weights (RFC 8878 §4.2.1.1);
-    // the shorter wins.  The FSE form is what lets alphabets above byte value 128 (binary payloads) be Huffman-coded.
-    uint32_t tree_bytes = nweights <= 128 ? 1 + (nweights + 1) / 2 : 0xffffffffu;
-    uint8_t* wdesc = (uint8_t*)hist;                                      // the histogram is dead: header byte + FSE description
-    {
-        uint8_t* wts = (uint8_t*)(work + 1536);                           // weights, then FSE tables, in dead tree scratch
-        uint32_t* wcnt = (uint32_t*)(wts + 256);                          // [16]
-        uint16_t* wst = (uint16_t*)(wcnt + 16);                           // [64]
-        zf::FseCSym* wsy = (zf::FseCSym*)(wst + 64);                      // [16]
-        uint8_t* wscratch = (uint8_t*)(wsy + 16);                         // >= 772 bytes
-        if (lane < 16) wcnt[lane] = 0;
-        __syncwarp();
-        for (uint32_t s2 = lane; s2 < nweights; s2 += 32) {
-            const uint32_t l = ctab[s2] >> 16;
-            const uint32_t w = l ? max_len + 1 - l : 0;
-            wts[s2] = (uint8_t)w;
-            atomicAdd(&wcnt[w], 1u);
-        }
-        __syncwarp();
-        if (nweights >= 2 && (ZE_FSE_WEIGHTS_ALWAYS || nweights > 128)) {
-            ZeKind wk;
-            const uint32_t dsz = ze_build_kind(wcnt, 13, nweights, zf::HUFW_MAX_LOG, zf::HUFW_MAX_LOG, nullptr, nullptr, wst, wsy,
-                                               wscratch, wdesc + 1, &wk, false, lane);
-            if (wk.mode == 2) {
-                if (lane == 0) {                                          // two interleaved states, last weight first
-                    uint8_t* o = wdesc + 1 + dsz;
-                    uint64_t acc = 0; uint32_t nb = 0, ob = 0;
-                    uint32_t st_even = 0, st_odd = 0;                     // the chains of the even and the odd weights
-                    for (uint32_t q = 0; q < 2; q++) {                    // FSE_initCState2 for the two last weights
-                        const uint32_t i = nweights - 1 - q;
-                        const zf::FseCSym c = wsy[wts[i]];
-                        const uint32_t nbo = (uint32_t)(c.delta_nb_bits + (1 << 15)) >> 16;
-                        const uint32_t v = (nbo << 16) - (uint32_t)c.delta_nb_bits;
-                        const uint32_t s0 = wst[(int32_t)(v >> nbo) + c.delta_find_state];
-                        if (i & 1) st_odd = s0; else st_even = s0;
-                    }
-                    for (int32_t i = (int32_t)nweights - 3; i >= 0; i--) {
-                        const zf::FseCSym c = wsy[wts[i]];
-                        const uint32_t sv = (i & 1) ? st_odd : st_even;
-                        const uint32_t nbo = (sv + (uint32_t)c.delta_nb_bits) >> 16;
-                        acc |= (uint64_t)(sv & ((1u << nbo) - 1)) << nb; nb += nbo;
-                        const uint32_t s1 = wst[(int32_t)(sv >> nbo) + c.delta_find_state];
-                        if (i & 1) st_odd = s1; else st_even = s1;
-                        while (nb >= 8) { o[ob++] = (uint8_t)acc; acc >>= 8; nb -= 8; }
-                    }
-                    acc |= (uint64_t)(st_odd & ((1u << wk.log) - 1)) << nb; nb += wk.log;     // flush odd chain, then even chain
-                    acc |= (uint64_t)(st_even & ((1u << wk.log) - 1)) << nb; nb += wk.log;
-                    acc |= 1ull << nb; nb += 1;                                                // end mark
-                    while (nb > 0) { o[ob++] = (uint8_t)acc; acc >>= 8; nb = nb >= 8 ? nb - 8 : 0; }
-                    meta[2] = dsz + ob;
-                }
-                __syncwarp();
-                const uint32_t fsz = meta[2];
-                if (fsz < 128 && 1 + fsz < tree_bytes) {
-                    if (lane == 0) wdesc[0] = (uint8_t)fsz;
-                    tree_bytes = 1 + fsz;
-                } else if (lane == 0) wdesc[0] = 0xff;
-            } else if (lane == 0) wdesc[0] = 0xff;
-        } else if (lane == 0) wdesc[0] = 0xff;
-        __syncwarp();
-    }
-    if (tree_bytes == 0xffffffffu) return zb_raw_literals(lits, n, body, lane);   // neither form can describe this tree
-    const bool fse_weights = wdesc[0] != 0xff;
+    uint8_t* desc = (uint8_t*)hist;                                       // the histogram is dead
+    const uint32_t tree_bytes = ze_huf_tree_desc(ctab, last_sym, max_len, desc, work, lane);   // symbols 0 .. last_sym-1 are listed
+    if (tree_bytes == ZE_NO_TREE) return zb_raw_literals(lits, n, body, lane);
     const uint32_t est = tree_bytes + 6 + (total_bits >> 3) + 8;
     if (est + 5 >= n) return zb_raw_literals(lits, n, body, lane);        // Huffman would not pay
 
@@ -288,29 +192,13 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
     }
     __syncwarp();
     const uint32_t comp = tree_bytes + 6 + byte_pos;
-    const uint32_t hsz = (n < 1024 && comp < 1024) ? 3u : (n < 16384 && comp < 16384) ? 4u : 5u;
+    const uint32_t hsz = ze_lit_header_huf_size(n, comp);
     if (hsz + comp >= 3 + n) return zb_raw_literals(lits, n, body, lane);
     if (lane == 0) {
-        const uint32_t sf = hsz - 2;                                      // 1, 2, 3: all with four streams
-        uint64_t h;
-        if (hsz == 3) h = 2u | (sf << 2) | ((uint64_t)n << 4) | ((uint64_t)comp << 14);
-        else if (hsz == 4) h = 2u | (sf << 2) | ((uint64_t)n << 4) | ((uint64_t)comp << 18);
-        else h = 2u | (sf << 2) | ((uint64_t)n << 4) | ((uint64_t)comp << 22);
-        for (uint32_t k = 0; k < hsz; k++) body[k] = (uint8_t)(h >> (8 * k));
-        uint8_t* t = body + hsz;
-        if (fse_weights) {
-            for (uint32_t i = 0; i < tree_bytes; i++) t[i] = wdesc[i];
-        } else {
-            t[0] = (uint8_t)(127 + nweights);
-            for (uint32_t i = 0; i < nweights; i += 2) {
-                const uint32_t l0 = ctab[i] >> 16, l1 = i + 1 < nweights ? ctab[i + 1] >> 16 : 0;
-                const uint32_t w0 = l0 ? max_len + 1 - l0 : 0, w1 = l1 ? max_len + 1 - l1 : 0;
-                t[1 + i / 2] = (uint8_t)((w0 << 4) | w1);
-            }
-        }
-        uint8_t* j = t + tree_bytes;
-        for (uint32_t k = 0; k < 6; k++) j[k] = (uint8_t)(ssz_all >> (8 * k));            // jump table: sizes of streams 1-3
+        ze_lit_header_huf(body, 2, n, comp);
+        ze_lit_jump_table(body + hsz + tree_bytes, ssz_all);
     }
+    for (uint32_t i = lane; i < tree_bytes; i += 32) body[hsz + i] = desc[i];
     uint8_t* sp = body + hsz + tree_bytes + 6;
     const uint8_t* wb = (const uint8_t*)work;
     _Pragma("unroll 2")
@@ -324,129 +212,33 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
 // descriptions go straight to `hdr_out` (global), the bit stream is staged in the word buffer `bits` (shared).
 // Returns the bit-stream bytes; *desc_bytes = 1 (modes byte) + table descriptions.  Warp-uniform, N >= 1.
 __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict__ seqs, uint32_t N, uint32_t* bits, ZbCTab* ct,
-                                                        const ZeCodeTabs* tabs,
-                                                        uint2* pk /*[3][32]*/, uint32_t* sb /*[3][32]*/,
-                                                        const ZbFsePre* fs, uint8_t* hdr_out, uint32_t* desc_bytes, uint32_t lane ZB_PH_PARAM) {
-    // ---- pass 1: code histograms (then normalised counts), in the word buffer beyond ze_build_kind's own scratch
+                                                        const ZeCodeTabs* tabs, uint8_t* hdr_out, uint32_t* desc_bytes,
+                                                        uint32_t lane ZB_PH_PARAM) {
+    // code histograms (then normalised counts), in the word buffer beyond ze_build_kind's own scratch
     uint32_t* cnt = bits + 256;
     for (uint32_t i = lane; i < ZE_NSYM_LL + ZE_NSYM_ML + ZE_NSYM_OF; i += 32) cnt[i] = 0;
     __syncwarp();
-    uint2 pre = lane < N ? seqs[lane] : make_uint2(0, 0);
-    for (uint32_t t0 = 0; t0 < N; t0 += 32) {
-        const uint32_t j = t0 + lane;
-        const uint2 s = pre;
-        if (j + 32 < N) pre = seqs[j + 32];                  // next tile in flight while this one is counted
-        if (j < N) {
-            atomicAdd(&cnt[ze_ll_code_s(tabs, s.x & 0xffff)], 1u);
-            atomicAdd(&cnt[ZE_NSYM_LL + ze_ml_code_s(tabs, s.x >> 16)], 1u);
-            atomicAdd(&cnt[ZE_NSYM_LL + ZE_NSYM_ML + (uint32_t)zf::highbit32(s.y + 3)], 1u);
-        }
-    }
+    ze_seq_hist(seqs, N, cnt, tabs, lane);
     __syncwarp();
-    // ---- tables (descriptions in stream order LL, OF, ML); `bits` doubles as scratch until it is cleared
+    // tables (descriptions in stream order LL, OF, ML); `bits` doubles as scratch until it is cleared
     ZeKind kll, kof, kml;
     uint8_t* desc = hdr_out + 1;
-    uint32_t dn = ze_build_kind(cnt, ZE_NSYM_LL, N, zf::LL_MAX_LOG, zf::LL_DEFAULT_LOG, fs->t.ll.state, fs->t.ll.sym,
-                                ct->st_ll, ct->sy_ll, (uint8_t*)bits, desc, &kll, true, lane);
-    dn += ze_build_kind(cnt + ZE_NSYM_LL + ZE_NSYM_ML, ZE_NSYM_OF, N, zf::OF_MAX_LOG, zf::OF_DEFAULT_LOG, fs->t.of.state, fs->t.of.sym,
-                        ct->st_of, ct->sy_of, (uint8_t*)bits, desc + dn, &kof, true, lane);
-    dn += ze_build_kind(cnt + ZE_NSYM_LL, ZE_NSYM_ML, N, zf::ML_MAX_LOG, zf::ML_DEFAULT_LOG, fs->t.ml.state, fs->t.ml.sym,
-                        ct->st_ml, ct->sy_ml, (uint8_t*)bits, desc + dn, &kml, true, lane);
+    uint32_t dn = ze_build_seq_kind(0, cnt, N, ct, (uint8_t*)bits, desc, &kll, lane);
+    dn += ze_build_seq_kind(1, cnt, N, ct, (uint8_t*)bits, desc + dn, &kof, lane);
+    dn += ze_build_seq_kind(2, cnt, N, ct, (uint8_t*)bits, desc + dn, &kml, lane);
     if (lane == 0) hdr_out[0] = (uint8_t)((kll.mode << 6) | (kof.mode << 4) | (kml.mode << 2));
     *desc_bytes = 1 + dn;
     __syncwarp();
     for (uint32_t i = lane; i < (ZB + ZB_BUF_PAD) / 4; i += 32) bits[i] = 0;
     __syncwarp();
     ZB_MARK(5);
-
-    // ---- pass 2: encode.  Per tile of 32 sequences every lane looks up the transforms of its sequence's three codes;
-    // lanes 0-2 then walk the three state chains (one 8-byte load, the bit count, one store, one table load per symbol).
-    uint32_t bitpos = 0;
-    uint32_t state = 0;                              // lanes 0..2: OF, ML, LL chains
-    const uint16_t* st_tab = lane == 0 ? ct->st_of : lane == 1 ? ct->st_ml : ct->st_ll;
-    const bool rle = (lane == 0 ? kof.mode : lane == 1 ? kml.mode : kll.mode) == 1;
-    const uint2* mypk = pk + (lane < 3 ? lane : 0) * 32;
-    uint32_t* mysb = sb + (lane < 3 ? lane : 0) * 32;
-    pre = lane < N ? seqs[N - 1 - lane] : make_uint2(0, 0);
-    for (uint32_t t0 = 0; t0 < N; t0 += 32) {
-        const uint32_t j = t0 + lane;                // stream order: j = 0 is the LAST sequence
-        const bool have = j < N;
-        uint32_t ll = 0, mlb = 0, offb = 0, llc = 0, mlc = 0, ofc = 0;
-        const uint2 s = pre;
-        if (j + 32 < N) pre = seqs[N - 1 - (j + 32)];
-        if (have) {
-            ll = s.x & 0xffff; mlb = s.x >> 16; offb = s.y + 3;       // mlb = matchLength - 3, offb = offset + 3 (no repcodes)
-            llc = ze_ll_code_s(tabs, ll); mlc = ze_ml_code_s(tabs, mlb); ofc = (uint32_t)zf::highbit32(offb);
-            const zf::FseCSym a = ct->sy_of[ofc], b = ct->sy_ml[mlc], c = ct->sy_ll[llc];
-            pk[lane] = make_uint2((uint32_t)a.delta_nb_bits, (uint32_t)a.delta_find_state);
-            pk[32 + lane] = make_uint2((uint32_t)b.delta_nb_bits, (uint32_t)b.delta_find_state);
-            pk[64 + lane] = make_uint2((uint32_t)c.delta_nb_bits, (uint32_t)c.delta_find_state);
-        }
-        __syncwarp();
-        if (lane < 3) {
-            const uint32_t cnt = min(32u, N - t0);
-            if (rle) {
-                for (uint32_t i = 0; i < cnt; i++) mysb[i] = 0;
-            } else {
-                uint32_t i = 0;
-                if (t0 == 0) {                       // FSE_initCState2 with the last sequence's symbol
-                    const uint2 c = mypk[0];
-                    const uint32_t nb = (uint32_t)((int32_t)c.x + (1 << 15)) >> 16;
-                    const uint32_t v = (nb << 16) - c.x;
-                    state = st_tab[(int32_t)(v >> nb) + (int32_t)c.y];
-                    mysb[0] = 0;
-                    i = 1;
-                }
-                _Pragma("unroll 4")
-                for (; i < cnt; i++) {               // FSE_encodeSymbol
-                    const uint2 c = mypk[i];
-                    const uint32_t nb = (state + c.x) >> 16;
-                    mysb[i] = (state & ((1u << nb) - 1)) | (nb << 16);
-                    state = st_tab[(int32_t)(state >> nb) + (int32_t)c.y];
-                }
-            }
-        }
-        __syncwarp();
-        uint64_t field = 0; uint32_t nb = 0;
-        if (have) {
-            const uint32_t llb = tabs->ll_bits[llc], mlbits = tabs->ml_bits[mlc];
-            // order inside a field (first written = lowest bits): OF state, ML state, LL state, LL extra, ML extra, OF extra
-            const uint32_t b0 = sb[lane], b1 = sb[32 + lane], b2 = sb[64 + lane];
-            field = b0 & 0xffff; nb = b0 >> 16;
-            field |= (uint64_t)(b1 & 0xffff) << nb; nb += b1 >> 16;
-            field |= (uint64_t)(b2 & 0xffff) << nb; nb += b2 >> 16;
-            field |= (uint64_t)(ll & ((1u << llb) - 1)) << nb; nb += llb;
-            field |= (uint64_t)(mlb & ((1u << mlbits) - 1)) << nb; nb += mlbits;
-            field |= (uint64_t)(offb & ((1u << ofc) - 1)) << nb; nb += ofc;
-        }
-        const uint32_t inc = warp_inclusive_scan_u32(nb, lane);
-        ze_put_bits(bits, bitpos + inc - nb, field, nb);
-        bitpos += __shfl_sync(TS_FULL, inc, 31);
-        __syncwarp();
-    }
-    // FSE_flushCState x3 (ML, OF, LL) then the closing 1 bit
-    const uint32_t st_of = __shfl_sync(TS_FULL, state, 0), st_ml = __shfl_sync(TS_FULL, state, 1),
-                   st_ll = __shfl_sync(TS_FULL, state, 2);
-    if (lane == 0) {
-        uint64_t f = st_ml & ((1u << kml.log) - 1);
-        uint32_t nb = kml.log;
-        f |= (uint64_t)(st_of & ((1u << kof.log) - 1)) << nb; nb += kof.log;
-        f |= (uint64_t)(st_ll & ((1u << kll.log) - 1)) << nb; nb += kll.log;
-        f |= 1ull << nb; nb += 1;
-        ze_put_bits(bits, bitpos, f, nb);
-    }
-    bitpos += kml.log + kof.log + kll.log + 1;
-    __syncwarp();
-    return (bitpos + 7) >> 3;
+    return ze_encode_seq_bits(seqs, N, bits, ct, tabs, kll, kof, kml, lane);
 }
 
-
 __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const __grid_constant__ ZstdBlkArgs A) {
-// Common prologue of the block kernels (included inside a __global__ function body; see zstd_enc.cuh): which block this
-// warp owns, its scratch slots and its shared-memory window.
+    // which block this warp owns, its scratch slots and its shared-memory window
     TS_DYN_SMEM(smem);
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const ZbFsePre& fs = *(const ZbFsePre*)&g_pre_ctables;   // predefined tables stay in constant memory
 
     const uint32_t chunk = blockIdx.y;
     const uint32_t blk = blockIdx.x * ZB_WPB + warp;
@@ -472,14 +264,10 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
     uint8_t* wbase = smem + warp * ZB_SMEM_WARP_AL;
     uint8_t* buf = wbase;
     uint16_t* ht = (uint16_t*)(wbase + ZB + ZB_BUF_PAD);
-    uint2* pk = (uint2*)(buf + ZB_SEQ_AUX_OFF);
-    uint32_t* sb = (uint32_t*)(pk + 96);
 #if ZB_TUNE_PHASES
     ZbPhases* ph = gblk < ZB_PHASES_MAX ? &g_zb_phases[gblk] : nullptr;
     if (lane == 0 && ph) { *ph = ZbPhases{}; ph->t[0] = clock64(); }
 #endif
-// Stage + LZ parse of one 8 KiB block (included inside a __global__ function body after
-// zstd_enc_prologue.inc).  Leaves nseq sequences in `seqs`, nlit literals in `lits`.
     // ---- stage the block in shared memory (128-bit loads when the source is aligned), zero the pad, reset the table
     if ((((uintptr_t)src) & 15) == 0) {
         for (uint32_t i = lane * 16; i < bn; i += 512) {
@@ -638,9 +426,8 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
     ZB_MARK(2);
     ZB_NOTE(nseq, nseq);
     ZB_NOTE(nlit, nlit);
-// Entropy stage + emission of one block (included inside a __global__ function body after zstd_enc_prologue.inc; needs
-// nseq / nlit).  `buf` and `ht` are scratch here: the block's bytes are no longer needed in shared memory.
-    // ---- phase B: entropy stage into the (now free) shared block buffer, then emit
+
+    // ---- phase B: entropy stage into the (now free) shared block buffer and hash table, then emit
     uint32_t payload = 0xffffffffu;                                // "not compressible"
     {
         // literals section first (into `out` directly), then the sequences bit stream staged in `buf`
@@ -655,7 +442,7 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
                 payload = lit_bytes + 1;
             }
         } else {
-            const uint32_t shdr = nseq < 128 ? 1u : (nseq < 0x7f00 ? 2u : 3u);
+            const uint32_t shdr = ze_nseq_size(nseq);
             uint8_t* sp = body + lit_bytes;
             uint32_t desc_bytes = 0;
             // the code tables of the sequence fields go next to the FSE tables, over the (now dead) Huffman scratch
@@ -667,15 +454,11 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
                 if (i < 53) tabs->ml_bits[i] = g_seq_tables.ml_bits[i];
             }
             __syncwarp();
-            const uint32_t sbytes = zb_encode_sequences(seqs, nseq, (uint32_t*)buf, (ZbCTab*)ht, tabs, pk, sb, &fs, sp + shdr, &desc_bytes, lane ZB_PH_ARG);
+            const uint32_t sbytes = zb_encode_sequences(seqs, nseq, (uint32_t*)buf, (ZbCTab*)ht, tabs, sp + shdr, &desc_bytes, lane ZB_PH_ARG);
             ZB_MARK(6);
             const uint32_t total = lit_bytes + shdr + desc_bytes + sbytes;
             if (total < bn) {
-                if (lane == 0) {
-                    if (shdr == 1) sp[0] = (uint8_t)nseq;
-                    else if (shdr == 2) { sp[0] = (uint8_t)((nseq >> 8) + 0x80); sp[1] = (uint8_t)nseq; }
-                    else { sp[0] = 0xff; sp[1] = (uint8_t)(nseq - 0x7f00); sp[2] = (uint8_t)((nseq - 0x7f00) >> 8); }
-                }
+                if (lane == 0) ze_write_nseq(sp, nseq);
                 _Pragma("unroll 2")
                 for (uint32_t i = lane; i < sbytes; i += 32) sp[shdr + desc_bytes + i] = buf[i];
                 payload = total;

@@ -137,117 +137,129 @@ __device__ __forceinline__ uint32_t ze_huf_codes(const uint32_t* hist, uint32_t 
     return max_len;
 }
 
-// Region-wide tree.  hist[256] (counts, destroyed), ctab[256] out (code | len << 16, 0 = unused symbol), work: >= 7.5 KiB of
+// Compacts the used symbols of hist[256] into keys at work + 1280 (count << 8 | symbol, ascending symbol order, where
+// ze_huf_codes reads them; counts must stay below 2^24) and returns their number m.  *pays: the Shannon estimate of the
+// Huffman-coded size (in 1/16 bits: sum c * (log2(n) - log2(c)), log2 by leading zeros + a linear fraction) leaves room
+// to beat the n literals stored raw.  One warp.
+__device__ __forceinline__ uint32_t ze_huf_symbols(const uint32_t* hist, uint32_t n, uint32_t* work, bool* pays, uint32_t lane) {
+    uint32_t* keys = work + 1280;
+    uint32_t mine = 0;                                                    // 8 symbols per lane
+    for (uint32_t k = 0; k < 8; k++) mine += hist[lane * 8 + k] ? 1u : 0u;
+    const uint32_t inc = warp_inclusive_scan_u32(mine, lane);
+    const uint32_t m = __shfl_sync(TS_FULL, inc, 31);
+    uint32_t at = inc - mine, cost = 0;
+    const uint32_t hn = (uint32_t)zf::highbit32(n);
+    const uint32_t lgn = (hn << 4) + (((n << (31 - hn)) >> 27) & 15) + 1;
+    for (uint32_t k = 0; k < 8; k++) {
+        const uint32_t s = lane * 8 + k, c = hist[s];
+        if (c) {
+            keys[at++] = (c << 8) | s;
+            const uint32_t hb = (uint32_t)zf::highbit32(c);
+            const uint32_t lg16 = (hb << 4) + (((c << (31 - hb)) >> 27) & 15);       // ~ 16 * log2(c)
+            cost += c * (lgn - lg16);
+        }
+    }
+    const uint32_t bits16 = __reduce_add_sync(TS_FULL, cost);
+    *pays = (bits16 >> 7) + m / 2 + 16 < n;                               // else >= n bytes even before rounding losses
+    __syncwarp();
+    return m;
+}
+
+constexpr uint32_t ZE_NO_TREE = 0xffffffffu;
+
+// Tree description of the codes in ctab (RFC 8878 §4.2.1) for the weights of symbols 0 .. nweights-1: direct 4-bit weights
+// (at most 128 of them) or FSE-compressed weights, the shorter form.  The FSE form is what lets alphabets above byte value
+// 128 (binary payloads) be Huffman-coded.  Written to desc (shared memory, never more than 128 bytes); returns its size, or
+// ZE_NO_TREE when neither form can describe the tree.  work: the scratch given to ze_huf_codes (bytes 6144 .. 7504 are
+// used here).  One warp.
+__device__ __forceinline__ uint32_t ze_huf_tree_desc(const uint32_t* ctab, uint32_t nweights, uint32_t max_len, uint8_t* desc,
+                                                     uint32_t* work, uint32_t lane) {
+    uint8_t* wts = (uint8_t*)(work + 1536);                               // weights, then FSE tables, in dead tree scratch
+    uint32_t* wcnt = (uint32_t*)(wts + 256);                              // [16]
+    uint16_t* wst = (uint16_t*)(wcnt + 16);                               // [64]
+    zf::FseCSym* wsy = (zf::FseCSym*)(wst + 64);                          // [16]
+    uint8_t* wscratch = (uint8_t*)(wsy + 16);                             // >= 784 bytes
+    if (lane < 16) wcnt[lane] = 0;
+    __syncwarp();
+    for (uint32_t s = lane; s < nweights; s += 32) {
+        const uint32_t l = ctab[s] >> 16;
+        const uint32_t w = l ? max_len + 1 - l : 0;
+        wts[s] = (uint8_t)w;
+        atomicAdd(&wcnt[w], 1u);
+    }
+    __syncwarp();
+    uint32_t tree_bytes = nweights <= 128 ? 1 + (nweights + 1) / 2 : ZE_NO_TREE;
+    if (nweights >= 2 && (ZE_FSE_WEIGHTS_ALWAYS || nweights > 128)) {
+        ZeKind wk;
+        const uint32_t dsz = ze_build_kind(wcnt, 13, nweights, zf::HUFW_MAX_LOG, zf::HUFW_MAX_LOG, nullptr, nullptr, wst, wsy,
+                                           wscratch, desc + 1, &wk, false, lane);
+        if (wk.mode == 2) {
+            uint32_t fsz = 0;
+            if (lane == 0) {                                              // two interleaved states, last weight first
+                uint8_t* o = desc + 1 + dsz;
+                const uint32_t cap = 127 - dsz;                           // bytes left for the stream in 128
+                uint64_t acc = 0; uint32_t nb = 0, ob = 0;
+                uint32_t st_even = 0, st_odd = 0;                         // the chains of the even and the odd weights
+                for (uint32_t q = 0; q < 2; q++) {                        // FSE_initCState2 for the two last weights
+                    const uint32_t i = nweights - 1 - q;
+                    const zf::FseCSym c = wsy[wts[i]];
+                    const uint32_t nbo = (uint32_t)(c.delta_nb_bits + (1 << 15)) >> 16;
+                    const uint32_t v = (nbo << 16) - (uint32_t)c.delta_nb_bits;
+                    const uint32_t s0 = wst[(int32_t)(v >> nbo) + c.delta_find_state];
+                    if (i & 1) st_odd = s0; else st_even = s0;
+                }
+                // a full buffer stops the walk: the flush below then cannot finish and the form is rejected
+                for (int32_t i = (int32_t)nweights - 3; i >= 0 && ob < cap; i--) {
+                    const zf::FseCSym c = wsy[wts[i]];
+                    const uint32_t sv = (i & 1) ? st_odd : st_even;
+                    const uint32_t nbo = (sv + (uint32_t)c.delta_nb_bits) >> 16;
+                    acc |= (uint64_t)(sv & ((1u << nbo) - 1)) << nb; nb += nbo;
+                    const uint32_t s1 = wst[(int32_t)(sv >> nbo) + c.delta_find_state];
+                    if (i & 1) st_odd = s1; else st_even = s1;
+                    while (nb >= 8) { o[ob++] = (uint8_t)acc; acc >>= 8; nb -= 8; }       // nb <= 13: one byte at most
+                }
+                acc |= (uint64_t)(st_odd & ((1u << wk.log) - 1)) << nb; nb += wk.log;     // flush odd chain, then even chain
+                acc |= (uint64_t)(st_even & ((1u << wk.log) - 1)) << nb; nb += wk.log;
+                acc |= 1ull << nb; nb += 1;                                                // end mark
+                while (nb > 0 && ob < cap) { o[ob++] = (uint8_t)acc; acc >>= 8; nb = nb >= 8 ? nb - 8 : 0; }
+                fsz = nb ? ZE_NO_TREE : dsz + ob;                         // did not fit 127 bytes: unusable
+            }
+            fsz = __shfl_sync(TS_FULL, fsz, 0);
+            if (fsz < 128 && 1 + fsz < tree_bytes) {
+                if (lane == 0) desc[0] = (uint8_t)fsz;
+                tree_bytes = 1 + fsz;
+                __syncwarp();
+                return tree_bytes;
+            }
+        }
+    }
+    if (tree_bytes != ZE_NO_TREE) {
+        if (lane == 0) {                           // (one lane: a warp-wide loop costs the speed kernel 6 registers)
+            desc[0] = (uint8_t)(127 + nweights);
+            for (uint32_t i = 0; 2 * i < nweights; i++)
+                desc[1 + i] = (uint8_t)((wts[2 * i] << 4) | (2 * i + 1 < nweights ? wts[2 * i + 1] : 0u));
+        }
+    }
+    __syncwarp();
+    return tree_bytes;
+}
+
+// Region-wide tree.  hist[256] (counts), ctab[256] out (code | len << 16, 0 = unused symbol), work: >= 7.5 KiB of
 // shared-memory scratch, n = literals in the region.  One warp.
 __device__ TS_NOINLINE void ze_huf_build(uint32_t* hist, uint32_t* ctab, uint32_t* work, uint32_t n, ZeHuf* hf, uint32_t lane) {
-    uint32_t* keys = work + 1280;              // [256] used symbols: count << 8 | symbol
-    uint32_t* meta = work + 1200;              // small scalars shared by the warp
     if (lane == 0) { hf->ok = 0; hf->tree_bytes = 0; hf->max_len = 0; }
     for (uint32_t i = lane; i < 256; i += 32) ctab[i] = 0;
     __syncwarp();
     if (n < ZE_HUF_REGION_MIN) return;
-
-    // compact the used symbols (8 per lane, ascending symbol order); counts are capped so that count << 8 cannot overflow
-    uint32_t mine = 0;
-    for (uint32_t k = 0; k < 8; k++) mine += hist[lane * 8 + k] ? 1u : 0u;
-    const uint32_t inc = warp_inclusive_scan_u32(mine, lane);
-    const uint32_t m = __shfl_sync(TS_FULL, inc, 31);
-    {
-        uint32_t at = inc - mine;
-        for (uint32_t k = 0; k < 8; k++) { const uint32_t s = lane * 8 + k; if (hist[s]) keys[at++] = (hist[s] << 8) | s; }
-    }
-    __syncwarp();
-    if (m < 2) return;                         // a single symbol: every block of the region is an RLE literals block
-    {   // Shannon estimate in 1/16 bit units: sum c * (log2(n) - log2(c)), log2 by leading zeros + a linear fraction
-        uint32_t cost = 0;
-        const uint32_t hn = (uint32_t)zf::highbit32(n);
-        const uint32_t lgn = (hn << 4) + (((n << (31 - hn)) >> 27) & 15) + 1;
-        for (uint32_t k = 0; k < 8; k++) {
-            const uint32_t c = hist[lane * 8 + k];
-            if (c) {
-                const uint32_t hb = (uint32_t)zf::highbit32(c);
-                const uint32_t lg16 = (hb << 4) + (((c << (31 - hb)) >> 27) & 15);       // ~ 16 * log2(c)
-                cost += c * (lgn - lg16);
-            }
-        }
-        const uint32_t bits16 = __reduce_add_sync(TS_FULL, cost);
-        if ((bits16 >> 7) + m / 2 + 16 >= n) return;                      // >= n bytes even before rounding losses
-    }
-    const uint32_t last_sym = keys[m - 1] & 0xff;
+    bool pays;
+    const uint32_t m = ze_huf_symbols(hist, n, work, &pays, lane);
+    if (m < 2 || !pays) return;                // a single symbol: every block of the region is an RLE literals block
+    const uint32_t last_sym = work[1280 + m - 1] & 0xff;
     uint32_t total_bits;
     const uint32_t max_len = ze_huf_codes(hist, m, last_sym, 20, ctab, work, &total_bits, lane);
     if (max_len > (uint32_t)zf::HUF_MAX_LOG) return;
-    const uint32_t nweights = last_sym;                                   // symbols 0 .. last_sym-1 are listed
-    // Tree description: direct 4-bit weights (at most 128 of them) or FSE-compressed weights (RFC 8878 §4.2.1.1);
-    // the shorter wins.  The FSE form is what lets alphabets above byte value 128 (binary payloads) be Huffman-coded.
-    uint32_t tree_bytes = nweights <= 128 ? 1 + (nweights + 1) / 2 : 0xffffffffu;
-    uint8_t* wdesc = hf->desc;
-    bool fse_weights = false;
-    {
-        uint8_t* wts = (uint8_t*)(work + 1536);                           // weights, then FSE tables, in dead tree scratch
-        uint32_t* wcnt = (uint32_t*)(wts + 256);                          // [16]
-        uint16_t* wst = (uint16_t*)(wcnt + 16);                           // [64]
-        zf::FseCSym* wsy = (zf::FseCSym*)(wst + 64);                      // [16]
-        uint8_t* wscratch = (uint8_t*)(wsy + 16);                         // >= 784 bytes
-        if (lane < 16) wcnt[lane] = 0;
-        __syncwarp();
-        for (uint32_t s2 = lane; s2 < nweights; s2 += 32) {
-            const uint32_t l = ctab[s2] >> 16;
-            const uint32_t w = l ? max_len + 1 - l : 0;
-            wts[s2] = (uint8_t)w;
-            atomicAdd(&wcnt[w], 1u);
-        }
-        __syncwarp();
-        if (nweights >= 2 && (ZE_FSE_WEIGHTS_ALWAYS || nweights > 128)) {
-            ZeKind wk;
-            const uint32_t dsz = ze_build_kind(wcnt, 13, nweights, zf::HUFW_MAX_LOG, zf::HUFW_MAX_LOG, nullptr, nullptr, wst, wsy,
-                                               wscratch, wdesc + 1, &wk, false, lane);
-            if (wk.mode == 2) {
-                if (lane == 0) {                                          // two interleaved states, last weight first
-                    uint8_t* o = wdesc + 1 + dsz;
-                    uint64_t acc = 0; uint32_t nb = 0, ob = 0;
-                    uint32_t st[2];
-                    for (uint32_t q = 0; q < 2; q++) {                    // FSE_initCState2 for the two last weights
-                        const uint32_t i = nweights - 1 - q;
-                        const zf::FseCSym c = wsy[wts[i]];
-                        const uint32_t nbo = (uint32_t)(c.delta_nb_bits + (1 << 15)) >> 16;
-                        const uint32_t v = (nbo << 16) - (uint32_t)c.delta_nb_bits;
-                        st[i & 1] = wst[(int32_t)(v >> nbo) + c.delta_find_state];
-                    }
-                    for (int32_t i = (int32_t)nweights - 3; i >= 0; i--) {
-                        const zf::FseCSym c = wsy[wts[i]];
-                        const uint32_t sv = st[i & 1];
-                        const uint32_t nbo = (sv + (uint32_t)c.delta_nb_bits) >> 16;
-                        acc |= (uint64_t)(sv & ((1u << nbo) - 1)) << nb; nb += nbo;
-                        st[i & 1] = wst[(int32_t)(sv >> nbo) + c.delta_find_state];
-                        while (nb >= 8 && ob < 120) { o[ob++] = (uint8_t)acc; acc >>= 8; nb -= 8; }
-                    }
-                    acc |= (uint64_t)(st[1] & ((1u << wk.log) - 1)) << nb; nb += wk.log;      // flush odd chain, then even chain
-                    acc |= (uint64_t)(st[0] & ((1u << wk.log) - 1)) << nb; nb += wk.log;
-                    acc |= 1ull << nb; nb += 1;                                                // end mark
-                    while (nb > 0 && ob < 126) { o[ob++] = (uint8_t)acc; acc >>= 8; nb = nb >= 8 ? nb - 8 : 0; }
-                    meta[2] = nb ? 0xffffu : dsz + ob;                    // did not fit 127 bytes: unusable
-                }
-                __syncwarp();
-                const uint32_t fsz = meta[2];
-                if (fsz < 128 && 1 + fsz < tree_bytes) {
-                    if (lane == 0) wdesc[0] = (uint8_t)fsz;
-                    tree_bytes = 1 + fsz;
-                    fse_weights = true;
-                }
-            }
-        }
-        __syncwarp();
-    }
-    if (tree_bytes == 0xffffffffu) return;                                // neither form can describe this tree
-    if (!fse_weights && lane == 0) {
-        wdesc[0] = (uint8_t)(127 + nweights);
-        for (uint32_t i = 0; i < nweights; i += 2) {
-            const uint32_t l0 = ctab[i] >> 16, l1 = i + 1 < nweights ? ctab[i + 1] >> 16 : 0;
-            const uint32_t w0 = l0 ? max_len + 1 - l0 : 0, w1 = l1 ? max_len + 1 - l1 : 0;
-            wdesc[1 + i / 2] = (uint8_t)((w0 << 4) | w1);
-        }
-    }
+    const uint32_t tree_bytes = ze_huf_tree_desc(ctab, last_sym, max_len, hf->desc, work, lane);   // symbols 0 .. last_sym-1 are listed
+    if (tree_bytes == ZE_NO_TREE) return;
     if (lane == 0) { hf->ok = 1; hf->tree_bytes = tree_bytes; hf->max_len = max_len; }
     __syncwarp();
 }
@@ -336,8 +348,11 @@ __device__ __forceinline__ uint32_t ze_lit_header_raw(uint8_t* body, uint32_t ty
     return 3;
 }
 // ... and for a Compressed (type 2) / Treeless (type 3) block with four streams; comp = tree + jump table + streams.
+__device__ __forceinline__ uint32_t ze_lit_header_huf_size(uint32_t n, uint32_t comp) {
+    return (n < 1024 && comp < 1024) ? 3u : (n < 16384 && comp < 16384) ? 4u : 5u;
+}
 __device__ __forceinline__ uint32_t ze_lit_header_huf(uint8_t* body, uint32_t type, uint32_t n, uint32_t comp) {
-    const uint32_t hsz = (n < 1024 && comp < 1024) ? 3u : (n < 16384 && comp < 16384) ? 4u : 5u;
+    const uint32_t hsz = ze_lit_header_huf_size(n, comp);
     const uint32_t sf = hsz - 2;                                          // 1, 2, 3: all with four streams
     uint64_t h;
     if (hsz == 3) h = type | (sf << 2) | ((uint64_t)n << 4) | ((uint64_t)comp << 14);
@@ -346,8 +361,9 @@ __device__ __forceinline__ uint32_t ze_lit_header_huf(uint8_t* body, uint32_t ty
     for (uint32_t k = 0; k < hsz; k++) body[k] = (uint8_t)(h >> (8 * k));
     return hsz;
 }
-__device__ __forceinline__ uint32_t ze_lit_header_huf_size(uint32_t n, uint32_t comp) {
-    return (n < 1024 && comp < 1024) ? 3u : (n < 16384 && comp < 16384) ? 4u : 5u;
+// Jump table of a four-stream literals section: the sizes of streams 1-3, packed 16 bits each in `sizes` — one lane.
+__device__ __forceinline__ void ze_lit_jump_table(uint8_t* j, uint64_t sizes) {
+    for (uint32_t k = 0; k < 6; k++) j[k] = (uint8_t)(sizes >> (8 * k));
 }
 
 }  // namespace ts
