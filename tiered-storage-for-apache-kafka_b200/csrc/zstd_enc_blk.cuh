@@ -4,7 +4,7 @@
 // different trade: every 8 KiB block is self-contained (own Huffman tree, own FSE tables, no match leaves the block), so a
 // 1 GiB segment is 131,072 independent warps with no barrier between them, 20 warps per SM.  That is the round-1 kernel with
 // the streamlined FSE chains and the backwards growth of taken matches ("catch up"); it compresses the K corpus ~3.1 : 1 at
-// ~15.7 ms per GiB on an H100, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
+// ~14.9 ms per GiB on an H100, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
 // window and one set of tables per 8 blocks).  TSGPU_FLAG_ZSTD picks this kernel, TSGPU_FLAG_ZSTD | TSGPU_FLAG_ZSTD_DENSE the region kernel;
 // the decoder reads both through the same region path (zstd_dec.cuh).
 //   zstd_enc_blocks_kernel    one WARP per block: block staged in shared memory; 32 positions hashed and verified per step
@@ -40,6 +40,9 @@ constexpr uint32_t ZB_HSIZE = 1u << ZB_HLOG;
 #ifndef ZB_TUNE_PHASES    // 1: every warp stamps clock64() at its block's phase boundaries into g_zb_phases, read back through
 #define ZB_TUNE_PHASES 0  //    tsgpu_zb_phases (scripts/enc_phases.py); measurement builds only, never the product
 #endif
+#ifndef ZB_TUNE_PAD       // N > 0: N extra FFMAs per parse step in 4 independent chains, off the step's dependent chain: if the
+#define ZB_TUNE_PAD 0     //    kernel time grows with N as issue slots predict, the parse is issue-bound (measurement builds only)
+#endif
 constexpr int ZB_WPB = ZB_TUNE_WPB;            // warps (= blocks in flight) per CTA
 constexpr uint32_t ZB_LANE_EXT = ZB_TUNE_LANE_EXT;   // bytes a lane extends its own match beyond the first 4
 constexpr uint32_t ZB_BUF_PAD = 416;           // zero pad for over-reads; its tail also holds the FSE tile scratch
@@ -73,6 +76,23 @@ __device__ ZbPhases g_zb_phases[ZB_PHASES_MAX];
 #endif
 
 __device__ __forceinline__ uint32_t zb_hash(uint32_t v) { return (v * 2654435761u) >> (32 - ZB_HLOG); }
+// the pointer unchanged, but opaque to the compiler, which would otherwise rebuild it from its parts at every use
+template <class T> __device__ __forceinline__ T* zb_opaque(T* p) {
+#if TS_DEVICE_ASM
+    asm("mov.b64 %0, %0;" : "+l"(p));
+#endif
+    return p;
+}
+// 0xffffffff << n, 0 for every n >= 32: one SHF on the GPU (PTX clamps shift counts), spelt out for the emulator
+__device__ __forceinline__ uint32_t zb_ones_from(uint32_t n) {
+#if TS_DEVICE_ASM
+    uint32_t r;
+    asm("shl.b32 %0, %1, %2;" : "=r"(r) : "r"(0xffffffffu), "r"(n));
+    return r;
+#else
+    return n >= 32 ? 0u : 0xffffffffu << n;
+#endif
+}
 
 struct ZstdBlkScratch {
     uint8_t* blk_out = nullptr;      // blocks * ZB_SLOT
@@ -258,8 +278,9 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
     const uint8_t* src = A.in_base + A.in_off[chunk] + (size_t)blk * ZB;
     const size_t gblk = (size_t)chunk * A.blocks_per_chunk + blk;
     uint8_t* out = A.blk_out + gblk * ZB_SLOT;
-    uint2* seqs = A.seqs + gblk * ZE_MAXSEQ;
-    uint8_t* lits = A.lits + gblk * ZB;
+    // per-block bases kept in registers: the parse step indexes them with 32-bit counts instead of redoing gblk's math
+    uint2* const seqs = zb_opaque(A.seqs + gblk * ZE_MAXSEQ);
+    uint8_t* const lits = zb_opaque(A.lits + gblk * ZB);
 
     uint8_t* wbase = smem + warp * ZB_SMEM_WARP_AL;
     uint8_t* buf = wbase;
@@ -287,9 +308,16 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
     // ---- phase A: greedy LZ parse, 32 positions per step
     // Selection (which of the 32 candidate matches survive, left to right) is the only serial part and costs a
     // handful of instructions per taken match; sequences are then written by their own lanes in parallel and
-    // the step's literals (the positions no taken match covers) leave in the same step.
+    // the step's literals (the positions no taken match covers) leave in the same step.  The step is bound by instruction
+    // issue (ZB_TUNE_PAD, DESIGN.md §8), so it is written for few instructions; the `step:` markers split the loop body
+    // into the parts whose static instructions scripts/parse_step_sass.py counts.
+#if ZB_TUNE_PAD
+    float pad[4] = {(float)lane, 1.f, 2.f, 3.f};
+#endif
+    const uint32_t lanes_below = (1u << lane) - 1;
     uint32_t anchor = 0, cur = 0, nseq = 0, nlit = 0;
     while (cur + 4 <= bn && nseq + 8 <= ZE_MAXSEQ) {                // a step adds at most 8 sequences (min match 4)
+        // step: probe
         const uint32_t p = cur + lane;
         const bool valid = p + 4 <= bn;
         // unaligned 4-byte reads as a rolling pair of aligned words per stream: one new LDS per stream and step
@@ -326,8 +354,8 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
             const uint32_t x1 = __funnelshift_r(a1, a2, shp) ^ __funnelshift_r(c1, c2, shc);
             const uint32_t x2 = __funnelshift_r(a2, a3, shp) ^ __funnelshift_r(c2, c3, shc);
             const uint32_t x3 = __funnelshift_r(a3, a4, shp) ^ __funnelshift_r(c3, c4, shc);
-            const uint32_t e1 = ze_common_bytes(x1), e2 = ze_common_bytes(x2), e3 = ze_common_bytes(x3);   // 0..4 each
-            const uint32_t e = e1 + (e1 >> 2) * (e2 + (e2 >> 2) * e3);         // branch-free: a word counts only if the one before it matched whole
+            // the equal bytes end in the first word that differs (all 12 are equal when none does): one count, not three
+            const uint32_t e = (x1 ? 0u : x2 ? 4u : 8u) + ze_common_bytes(x1 ? x1 : x2 ? x2 : x3);
             len = ok ? min(4 + e, min(bn - p, 4 + ZB_LANE_EXT)) : 0u;
         }
 #else
@@ -343,20 +371,31 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
             len = min(len, lim);
         }
 #endif
+#if ZB_TUNE_PAD
+        {
+            const float pv = __uint_as_float((v & 0x007fffffu) | 0x3f000000u);   // in [0.5, 1)
+            _Pragma("unroll")
+            for (int k = 0; k < ZB_TUNE_PAD; k++) asm volatile("fma.rn.f32 %0, %0, %1, %2;" : "+f"(pad[k & 3]) : "f"(pv), "f"(0.25f));
+        }
+#endif
+        // step: select
         const uint32_t mask = __ballot_sync(TS_FULL, ok && len >= ZE_MIN_MATCH);
         // Greedy selection, left to right.  Every lane precomputes where its match would end and which candidate would
         // come next, so one shuffle per taken match walks the chain (the only serial part of the parse).
         const uint32_t e = lane + len;
-        const uint32_t mnext = e < 32 ? mask & (0xffffffffu << e) : 0u;
-        const uint32_t nxt = mnext ? (uint32_t)__ffs((int)mnext) - 1 : 32u;
+        const uint32_t nxt = (uint32_t)__clz((int)__brev(mask & zb_ones_from(e)));       // 32: none
         const bool capped = ok && len == 4 + ZB_LANE_EXT && p + len < bn;
-        const uint32_t packed = e | (nxt << 8) | (capped ? 1u << 16 : 0u);
-        uint32_t taken = 0, pos = 0;
-        uint32_t f = mask ? (uint32_t)__ffs((int)mask) - 1 : 32u;
+        const uint32_t packed = e | (capped ? 1u << 8 : 0u) | (nxt << 16);
+        // The walk also hands every taken lane where the match before it ends (`my_prev`, relative to `cur`; the step's
+        // first match gets `anchor`, at or before `cur`), so the sequences need no shuffle after the walk.
+        uint32_t taken = 0, prev = anchor - cur, my_prev = 0;
+        uint32_t f = (uint32_t)__clz((int)__brev(mask));
+        // step: walk
         while (f < 32) {
             const uint32_t info = __shfl_sync(TS_FULL, packed, f);
-            uint32_t end = info & 0xffu, nf = (info >> 8) & 0xffu;
-            if (info >> 16) {                                      // warp-wide extension of a long match
+            uint32_t end = info & 0xffu, nf = info >> 16;
+            if (info & (1u << 8)) {                                // warp-wide extension of a long match
+                // step: long
                 uint32_t L = 4 + ZB_LANE_EXT;
                 const uint32_t off = __shfl_sync(TS_FULL, p - cand, f);
                 const uint32_t mpos = cur + f;
@@ -384,38 +423,43 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
                 }
                 if (lane == f) len = L;
                 end = f + L;
-                const uint32_t m2 = end < 32 ? mask & (0xffffffffu << end) : 0u;
-                nf = m2 ? (uint32_t)__ffs((int)m2) - 1 : 32u;
+                nf = (uint32_t)__clz((int)__brev(mask & zb_ones_from(end)));
+                // step: walk
             }
             taken |= 1u << f;
-            pos = end;
+            if (lane == f) my_prev = prev;
+            prev = end;
             f = nf;
         }
+        // step: tail
         uint32_t cov = 0;                                          // positions of this step covered by a taken match
         if (taken) {
-            const bool mine_taken = (taken >> lane) & 1;
-            const uint32_t my_end = p + len;                       // meaningful on taken lanes
-            const uint32_t lower = taken & ((1u << lane) - 1);
-            const uint32_t prev_lane = lower ? (uint32_t)(31 - __clz((int)lower)) : 0u;
-            uint32_t prev_end = __shfl_sync(TS_FULL, my_end, prev_lane);
-            if (!lower) prev_end = anchor;
-            const uint32_t bk = mine_taken ? min(bkr, p - max(prev_end, cur)) : 0u;   // "catch up" over this step's literals, never into the previous match
-            if (mine_taken)
-                seqs[nseq + (uint32_t)__popc(lower)] = make_uint2((p - bk - prev_end) | ((len + bk - 3) << 16), p - cand);
+            const bool mine = (taken >> lane) & 1;
+            const uint32_t pe = cur + my_prev;                     // where the match before this lane's ends
+            const uint32_t bk = mine ? min(bkr, p - max(pe, cur)) : 0u;   // "catch up" over this step's literals, never into the previous match
+            if (mine)
+                seqs[nseq + (uint32_t)__popc(taken & lanes_below)] = make_uint2((p - bk - pe) | ((len + bk - 3) << 16), p - cand);
             nseq += (uint32_t)__popc(taken);
-            anchor = cur + pos;
-            const uint32_t sl = lane - bk, tl = len + bk;
-            cov = __reduce_or_sync(TS_FULL, mine_taken ? (tl >= 32 - sl ? 0xffffffffu : (1u << tl) - 1) << sl : 0u);
+            // Two warp syncs stand where the previous end was shuffled: the test emulator runs the lanes in an order that
+            // follows the warp's rendezvous count, and its frames (tests/golden/speed_frames.json) pin that order.
+            __syncwarp();
+            __syncwarp();
+            cov = __reduce_or_sync(TS_FULL, mine ? zb_ones_from(lane - bk) & ~zb_ones_from(lane + len) : 0u);
         }
+        anchor = cur + prev;
+        // step: literals
         // the step's literals, in order: one byte per position of the block no taken match covers
         {
-            const uint32_t inside = bn - cur >= 32 ? 0xffffffffu : (1u << (bn - cur)) - 1;
-            const uint32_t lm = ~cov & inside;
-            if ((lm >> lane) & 1) lits[nlit + (uint32_t)__popc(lm & ((1u << lane) - 1))] = (uint8_t)v;
+            const uint32_t lm = ~(cov | zb_ones_from(bn - cur));       // (positions at or past bn are no literals)
+            if ((lm >> lane) & 1) lits[nlit + (uint32_t)__popc(lm & lanes_below)] = (uint8_t)v;
             nlit += (uint32_t)__popc(lm);
         }
         cur = max(cur + 32, anchor);
+        // step: end
     }
+#if ZB_TUNE_PAD
+    if (nlit == 0xffffffffu) lits[0] = (uint8_t)__float_as_uint(pad[0] + pad[1] + pad[2] + pad[3]);   // keeps the chains live
+#endif
     if (cur < bn) {                                                // the rest of the block is literals
         const uint32_t ll = bn - cur;
         for (uint32_t k = lane; k < ll; k += 32) lits[nlit + k] = buf[cur + k];
