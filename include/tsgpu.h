@@ -42,6 +42,18 @@ extern "C" {
  * TSGPU_VERIFY=1 in the environment makes the flag the default of a context's host-buffer transform calls.  The
  * device-resident calls refuse the bit (TSGPU_E_ARG): they have no status output on the transform side. */
 #define TSGPU_FLAG_VERIFY 8u
+/* Modifier of TSGPU_FLAG_ZSTD on the transform side (ignored by detransform), for tsgpu_transform, tsgpu_transform_chunks and
+ * tsgpu_transform_device; combines with ZSTD_DENSE, AES and VERIFY.  Every frame ends with its Content_Checksum (RFC 8878
+ * 3.1.1: the low 32 bits of XXH64 of the chunk, seed 0, little-endian after the last block; Frame_Header_Descriptor bit 2 set).
+ * Otherwise the frame is exactly the one written without the flag, so it is 4 bytes longer and transformed_sizes count them;
+ * tsgpu_transform_bound and tsgpu_slot_stride already leave room.  Every zstd reader -- libzstd and zstd-jni, `zstd -t`, this
+ * library's decoder -- then verifies the content, so a damaged byte in a Raw block or a Huffman literal stream, which would
+ * otherwise decode to a different byte without an error, fails the read (TSGPU_E_CORRUPT here).  The checksum is computed
+ * from the original bytes by code that shares nothing with the compressor's stages, so with TSGPU_FLAG_VERIFY it also catches a
+ * misreading of the format that the writer and this library's reader share.  The hash runs in the compressor's own launch,
+ * beside the compression (cost: DESIGN.md §8).  TSGPU_ZSTD_CHECKSUM=1 in the environment makes the flag the default of a
+ * context's transform calls. */
+#define TSGPU_FLAG_ZSTD_CHECKSUM 16u
 
 #define TSGPU_IV_SIZE   12     /* SegmentEncryptionMetadataV1.java:30 */
 #define TSGPU_TAG_SIZE  16     /* AesEncryptionProvider.java:38 (128-bit tag) */
@@ -75,7 +87,8 @@ const char* tsgpu_version(void);
  * With 4 MiB chunks `max_batch = 4` measured best through PCIe; device-resident callers pass whole segments.
  * Environment (read once by tsgpu_create): TSGPU_SLOTS=1..16 slots per device, TSGPU_ZSTD_MODE=dense makes
  * TSGPU_FLAG_ZSTD_DENSE the context's default (both tuning only), TSGPU_VERIFY=1 turns TSGPU_FLAG_VERIFY on for the
- * context's host-buffer transform calls (not for the device-resident calls).
+ * context's host-buffer transform calls (not for the device-resident calls), TSGPU_ZSTD_CHECKSUM=1 turns
+ * TSGPU_FLAG_ZSTD_CHECKSUM on for all of the context's compressing transform calls.
  * --------------------------------------------------------------------------------------------------------- */
 int  tsgpu_create(const int* device_ids, int n_devices, uint32_t max_chunk_bytes, uint32_t max_batch,
                   tsgpu_ctx** out);

@@ -6,6 +6,8 @@ import java.nio.ByteBuffer;
 public final class TsGpu {
     public static final int FLAG_ZSTD = 1;
     public static final int FLAG_AES = 2;
+    // flags pass through to the C-ABI unchanged: TSGPU_FLAG_ZSTD_CHECKSUM (16, include/tsgpu.h) ends every zstd frame with its
+    // Content_Checksum; TSGPU_ZSTD_CHECKSUM=1 in the broker's environment turns it on without a change here
     public static final int IV_SIZE = 12;
 
     static {

@@ -15,6 +15,7 @@ FLAG_ZSTD = 1
 FLAG_AES = 2
 FLAG_ZSTD_DENSE = 4
 FLAG_VERIFY = 8          # host-buffer transforms: read each batch back on the device before releasing it
+FLAG_ZSTD_CHECKSUM = 16  # with FLAG_ZSTD: every frame ends with its Content_Checksum (XXH64 of the chunk, checked by every reader)
 IV_SIZE = 12
 TAG_SIZE = 16
 SLOT_HEAD = 4

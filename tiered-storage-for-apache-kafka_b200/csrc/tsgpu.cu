@@ -43,14 +43,19 @@ extern "C" const char* tsgpu_last_error(void) { return g_err; }
 extern "C" const char* tsgpu_version(void) { return "tsgpu 0.1 (sm_90a)"; }
 
 static inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
-static inline uint64_t frame_bound(uint64_t n) { return n + (n >> 8) + 64; }   // >= header + 3 bytes per 8 KiB block
+// Largest frame of an n-byte chunk, in either mode: a header of at most 10 bytes, at most ceil(n / 8 KiB) blocks of 3 header bytes
+// + at most 8 KiB each (a block that would not shrink goes out Raw), and the 4-byte Content_Checksum with
+// TSGPU_FLAG_ZSTD_CHECKSUM: n + 3 ceil(n / 8192) + 14 <= n + 3 n / 8192 + 17.  As n >> 8 >= n / 256 - 1 = 32 n / 8192 - 1, the
+// bound below exceeds that by at least 29 n / 8192 + 46 > 0 bytes for every n, with or without the checksum.
+static inline uint64_t frame_bound(uint64_t n) { return n + (n >> 8) + 64; }
 
 // ------------------------------------------------------------------------------------------ context
 namespace {
 
 constexpr int NSLOT_MAX = 16;       // work slots per device; tsgpu_ctx::nslot of them are used
 constexpr uint32_t MAX_AAD = 4096;
-constexpr uint32_t KNOWN_FLAGS = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE;
+constexpr uint32_t KNOWN_FLAGS = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES | TSGPU_FLAG_ZSTD_DENSE | TSGPU_FLAG_ZSTD_CHECKSUM;
+constexpr uint32_t ZSTD_MODIFIERS = TSGPU_FLAG_ZSTD_DENSE | TSGPU_FLAG_ZSTD_CHECKSUM;   // how to compress: the reader ignores them
 
 struct Desc {            // device-side descriptor block of one work slot (all arrays sized for max_batch)
     uint64_t* a_off; uint64_t* b_off; uint64_t* c_off;
@@ -91,6 +96,7 @@ struct Lane { int device = 0; Work w[NSLOT_MAX]; };
 struct tsgpu_ctx {
     bool dense_default = false;    // TSGPU_ZSTD_MODE=dense: TSGPU_FLAG_ZSTD alone already means the region kernel
     bool verify_default = false;   // TSGPU_VERIFY=1: host-buffer transforms verify as if TSGPU_FLAG_VERIFY were set
+    bool checksum_default = false; // TSGPU_ZSTD_CHECKSUM=1: every frame carries its Content_Checksum, as with TSGPU_FLAG_ZSTD_CHECKSUM
     std::mutex mu;                 // guards slot ownership (Work::claimed, active_calls) and lazy slot allocation — NOT held while a call runs
     std::condition_variable cv;
     uint32_t active_calls = 0;
@@ -200,6 +206,7 @@ extern "C" int tsgpu_create(const int* device_ids, int n_devices, uint32_t max_c
     if (const char* e = getenv("TSGPU_SLOTS")) { int v = atoi(e); if (v >= 1 && v <= NSLOT_MAX) c->nslot = (uint32_t)v; }       // tuning knobs
     if (const char* e = getenv("TSGPU_ZSTD_MODE")) c->dense_default = strcmp(e, "dense") == 0;
     if (const char* e = getenv("TSGPU_VERIFY")) c->verify_default = strcmp(e, "1") == 0;
+    if (const char* e = getenv("TSGPU_ZSTD_CHECKSUM")) c->checksum_default = strcmp(e, "1") == 0;
     c->frame_stride = align_up(frame_bound(max_chunk_bytes), 16) + 16;
     c->slot_stride = tsgpu_slot_stride(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES, max_chunk_bytes);
     c->lanes.resize(ids.size());
@@ -254,21 +261,23 @@ struct DxBounds {
 
 // zstd compress.  Two kernels, one contract (zstd_enc_blk.cuh: independent 8 KiB blocks, fastest; zstd_enc.cuh: 64 KiB
 // regions with shared tables and history, densest).  Their scratch is allocated the first time a slot runs the mode.
+// With the checksum either kernel also hashes every chunk, in extra CTAs of the same launch, and ends its frame with it.
 static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, ChunksIn in, uint32_t nb, uint32_t cs, ChunksOut out) {
     const bool dense = (flags & TSGPU_FLAG_ZSTD_DENSE) || c->dense_default;
+    const bool checksum = (flags & TSGPU_FLAG_ZSTD_CHECKSUM) || c->checksum_default;
     int rc;
     if (dense) {
         if (!w.zenc.seqs) {
             const char* e = zstd_enc_scratch_alloc(w.zenc, c->chunk_cap, c->max_batch);
             if (e) { zstd_enc_scratch_free(w.zenc); return fail(TSGPU_E_CUDA, "zstd enc scratch: %s", e); }
         }
-        rc = zstd_compress_batch(w.zenc, st, in.base, in.off, in.len, nb, cs, out.base, out.off, out.len, c->prof);
+        rc = zstd_compress_batch(w.zenc, st, in.base, in.off, in.len, nb, cs, checksum, out.base, out.off, out.len, c->prof);
     } else {
         if (!w.zblk.seqs) {
             const char* e = zstd_blk_scratch_alloc(w.zblk, c->chunk_cap, c->max_batch);
             if (e) { zstd_blk_scratch_free(w.zblk); return fail(TSGPU_E_CUDA, "zstd enc scratch: %s", e); }
         }
-        rc = zstd_compress_batch_blocks(w.zblk, st, in.base, in.off, in.len, nb, cs, out.base, out.off, out.len, c->prof);
+        rc = zstd_compress_batch_blocks(w.zblk, st, in.base, in.off, in.len, nb, cs, checksum, out.base, out.off, out.len, c->prof);
     }
     if (rc) return fail(rc, "zstd compress: %s", zstd_last_error());
     return TSGPU_OK;
@@ -652,7 +661,7 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
                             const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks) {
     const uint32_t n = (uint32_t)len.size();
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
-    if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~TSGPU_FLAG_ZSTD_DENSE;   // a modifier of ZSTD: meaningless (and harmless) without it
+    if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~ZSTD_MODIFIERS;         // modifiers of ZSTD: meaningless (and harmless) without it
     const bool verify = (flags & TSGPU_FLAG_VERIFY) || c->verify_default;
     flags &= ~TSGPU_FLAG_VERIFY;
 
@@ -734,7 +743,7 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
     if (flags & ~KNOWN_FLAGS) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
     if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
-    flags &= ~TSGPU_FLAG_ZSTD_DENSE;                         // how a frame was compressed does not matter to the reader
+    flags &= ~ZSTD_MODIFIERS;                                // how a frame was compressed does not matter to the reader
     uint64_t need = 0;
     for (uint32_t i = 0; i < n_chunks; i++) need += transformed_sizes[i];
     if (need > src_len) return fail(TSGPU_E_SHORT, "Stream has fewer bytes than expected");
@@ -851,6 +860,7 @@ extern "C" int tsgpu_detransform_device(tsgpu_ctx* c, int device_index, uint32_t
                                         uint8_t* d_dst, uint32_t* d_original_sizes, uint32_t* d_status, void* stream) {
     int rc = dev_args_ok(c, device_index, flags, chunk_size, n_chunks, slot_stride);
     if (rc || n_chunks == 0) return rc;
+    flags &= ~ZSTD_MODIFIERS;                                // how a frame was compressed does not matter to the reader
     if ((flags & TSGPU_FLAG_AES) && (!key || aad_len > MAX_AAD)) return fail(TSGPU_E_ARG, "key/aad invalid");
     if (!d_slots || !d_transformed_sizes || !d_dst || !d_original_sizes || !d_status) return fail(TSGPU_E_ARG, "null device pointer");
     Aes256RoundKeys rk{};

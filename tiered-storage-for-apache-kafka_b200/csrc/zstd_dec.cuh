@@ -1115,7 +1115,7 @@ __device__ __forceinline__ uint32_t zd_frame_header(const uint8_t* p, uint32_t n
 }
 
 // What may follow the last block of the frame inside the chunk: the 4-byte Content_Checksum when the frame header announces one
-// (verified by zd_xxh64_low32 in the last kernel of the batch), then only skippable
+// (verified by xxh64_warp_low32 in the last kernel of the batch), then only skippable
 // frames (ZSTD_decompress steps over those).  Anything else — trailing bytes, a second frame — is what zstd-jni's
 // Zstd.decompress(chunk, size) rejects ("Src size is incorrect" / "Destination buffer is too small"), so it is corrupt here too.
 __device__ __forceinline__ bool zd_frame_tail_ok(const uint8_t* p, uint32_t n, uint32_t pos) {
@@ -1131,45 +1131,10 @@ __device__ __forceinline__ bool zd_frame_tail_ok(const uint8_t* p, uint32_t n, u
 }
 
 // Content_Checksum (RFC 8878 3.1.1): the low 32 bits of XXH64(content, seed 0), little-endian after the last block.  libzstd —
-// hence zstd-jni's Zstd.decompress, DecompressionChunkEnumeration.java:41-45 — verifies it when the header announces one; the
-// reference's own writer never sets the flag, so this is a rare path: one warp, lanes 0-3 carry the four accumulators.
-__device__ __forceinline__ uint64_t zd_xx_rd64(const uint8_t* p) {
-    if ((((uintptr_t)p) & 7) == 0) return *(const uint64_t*)p;
-    uint64_t v = 0;
-    for (int k = 0; k < 8; k++) v |= (uint64_t)p[k] << (8 * k);
-    return v;
-}
-__device__ __forceinline__ uint64_t zd_xx_round(uint64_t acc, uint64_t in) {
-    acc += in * 14029467366897019727ull;
-    acc = (acc << 31) | (acc >> 33);
-    return acc * 11400714785074694791ull;
-}
-__device__ TS_NOINLINE uint32_t zd_xxh64_low32(const uint8_t* d, uint32_t n, uint32_t lane) {
-    const uint64_t P1 = 11400714785074694791ull, P2 = 14029467366897019727ull, P3 = 1609587929392839161ull,
-                   P4 = 9650029242287828579ull, P5 = 2870177450012600261ull;
-    uint64_t v = lane == 0 ? P1 + P2 : lane == 1 ? P2 : lane == 2 ? 0ull : 0ull - P1;
-    const uint32_t stripes = n / 32;
-    if (lane < 4) for (uint32_t s = 0; s < stripes; s++) v = zd_xx_round(v, zd_xx_rd64(d + (size_t)s * 32 + lane * 8));
-    const uint64_t v1 = __shfl_sync(TS_FULL, v, 0), v2 = __shfl_sync(TS_FULL, v, 1), v3 = __shfl_sync(TS_FULL, v, 2), v4 = __shfl_sync(TS_FULL, v, 3);
-    uint64_t h;
-    if (n >= 32) {
-        h = ((v1 << 1) | (v1 >> 63)) + ((v2 << 7) | (v2 >> 57)) + ((v3 << 12) | (v3 >> 52)) + ((v4 << 18) | (v4 >> 46));
-        h = (h ^ zd_xx_round(0, v1)) * P1 + P4;
-        h = (h ^ zd_xx_round(0, v2)) * P1 + P4;
-        h = (h ^ zd_xx_round(0, v3)) * P1 + P4;
-        h = (h ^ zd_xx_round(0, v4)) * P1 + P4;
-    } else h = P5;
-    h += n;
-    uint32_t at = stripes * 32;                                         // the tail (< 32 bytes): every lane computes the same value
-    for (; at + 8 <= n; at += 8) { h ^= zd_xx_round(0, zd_xx_rd64(d + at)); h = ((h << 27) | (h >> 37)) * P1 + P4; }
-    if (at + 4 <= n) {
-        const uint32_t w = d[at] | (d[at + 1] << 8) | (d[at + 2] << 16) | ((uint32_t)d[at + 3] << 24);
-        h ^= (uint64_t)w * P1; h = ((h << 23) | (h >> 41)) * P2 + P3; at += 4;
-    }
-    for (; at < n; at++) { h ^= (uint64_t)d[at] * P5; h = ((h << 11) | (h >> 53)) * P1; }
-    h ^= h >> 33; h *= P2; h ^= h >> 29; h *= P3; h ^= h >> 32;
-    return (uint32_t)h;
-}
+// hence zstd-jni's Zstd.decompress, DecompressionChunkEnumeration.java:41-45 — verifies it when the header announces one, and so
+// does this decoder: frames of this library's writer carry one with TSGPU_FLAG_ZSTD_CHECKSUM.  xxh64_warp_low32 (xxh64.cuh)
+// stages the decoded bytes through the warp's shared-memory working set, which is free by then.
+static_assert(sizeof(ZdWarpCtx) % 16 == 0 && sizeof(ZdWarpCtx) >= XXH_STAGE_BYTES, "checksum staging aliases a warp's working set");
 
 // ------------------------------------------------------------------------------------------ kernel 1: index
 __global__ void __launch_bounds__(128) zstd_dec_index_kernel(const __grid_constant__ ZstdDecArgs A) {
@@ -1245,7 +1210,8 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_frames_kernel(const __gr
         if (info[9] && A.status[chunk] == 0) {           // ... so a Content_Checksum, if the frame carries one, can be verified here
             const uint8_t* f = A.in_base + A.in_off[chunk] + info[9];
             const uint32_t want = f[0] | (f[1] << 8) | (f[2] << 16) | ((uint32_t)f[3] << 24);
-            const uint32_t got = zd_xxh64_low32(A.out_base + A.out_off[chunk], info[0], lane);
+            uint64_t* stage = (uint64_t*)(smem + (size_t)warp * sizeof(ZdWarpCtx));
+            const uint32_t got = xxh64_warp_low32(A.out_base + A.out_off[chunk], info[0], stage, lane);
             if (lane == 0 && got != want) { A.status[chunk] = ZD_ST_CORRUPT; A.out_len[chunk] = 0; }
         }
         return;
@@ -1294,7 +1260,7 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_frames_kernel(const __gr
         __syncwarp();
         __threadfence_block();
         const uint32_t want = p[pos] | (p[pos + 1] << 8) | (p[pos + 2] << 16) | ((uint32_t)p[pos + 3] << 24);
-        sum_bad = zd_xxh64_low32(dst, (uint32_t)fcs, lane) != want;
+        sum_bad = xxh64_warp_low32(dst, (uint32_t)fcs, (uint64_t*)cx, lane) != want;   // (the block walk is done with cx)
     }
     if (lane == 0) {
         if (bad || op != fcs || sum_bad || !zd_frame_tail_ok(p, n, pos)) { A.status[chunk] = ZD_ST_CORRUPT; A.out_len[chunk] = 0; }

@@ -25,6 +25,7 @@
 #include "launch_prof.h"
 #include "zstd_format.h"
 #include "index_scan.cuh"
+#include "xxh64.cuh"
 
 namespace ts {
 
@@ -84,6 +85,7 @@ struct ZstdEncScratch {
     uint8_t* slot_a = nullptr;       // blocks * ZE_SLOT_A
     uint8_t* slot_b = nullptr;       // blocks * ZE_SLOT_B
     unsigned long long* reg_state = nullptr;   // chunks * regions_per_chunk: look-back words (ready bit 63 | inclusive frame bytes)
+    unsigned long long* ck_state = nullptr;    // chunks: Content_Checksum hand-over words (ze_hash_warp)
     uint32_t blocks_per_chunk = 0, regions_per_chunk = 0;
     uint32_t max_batch = 0;
 };
@@ -93,6 +95,8 @@ struct ZstdEncArgs {
     uint2* seqs; uint8_t* lits; uint8_t* slot_a; uint8_t* slot_b; unsigned long long* reg_state;
     uint32_t blocks_per_chunk, regions_per_chunk;
     uint8_t* out_base; const uint64_t* out_off; uint32_t* out_len;
+    unsigned long long* ck_state;    // null: no Content_Checksum; else one hand-over word per chunk, zeroed before the launch
+    uint32_t hash_rows, n_chunks;    // grid rows of hashing CTAs in front of the chunks' rows (0 without the checksum)
 };
 
 // ------------------------------------------------------------------------------------------ small helpers
@@ -319,21 +323,63 @@ __device__ TS_NOINLINE void ze_warp_copy(uint8_t* __restrict__ dst, const uint8_
 }
 
 // ------------------------------------------------------------------------------------------ frame header
-__device__ __forceinline__ uint32_t ze_frame_header(uint8_t* h, uint32_t n) {     // see tshost::zstdFrameHeader
+// checksum: Content_Checksum_flag (Frame_Header_Descriptor bit 2); the frame then ends with 4 more bytes (ze_hash_warp)
+__device__ __forceinline__ uint32_t ze_frame_header(uint8_t* h, uint32_t n, bool checksum) {     // see tshost::zstdFrameHeader
     uint32_t p = 0;
+    const uint8_t ck = checksum ? 0x04 : 0x00;
     h[p++] = 0x28; h[p++] = 0xB5; h[p++] = 0x2F; h[p++] = 0xFD;
     if (n <= (1u << 21)) {
-        if (n < 256) { h[p++] = 0x20; h[p++] = (uint8_t)n; }
-        else if (n < 65536 + 256) { h[p++] = 0x60; h[p++] = (uint8_t)(n - 256); h[p++] = (uint8_t)((n - 256) >> 8); }
-        else { h[p++] = 0xA0; h[p++] = (uint8_t)n; h[p++] = (uint8_t)(n >> 8); h[p++] = (uint8_t)(n >> 16); h[p++] = (uint8_t)(n >> 24); }
+        if (n < 256) { h[p++] = 0x20 | ck; h[p++] = (uint8_t)n; }
+        else if (n < 65536 + 256) { h[p++] = 0x60 | ck; h[p++] = (uint8_t)(n - 256); h[p++] = (uint8_t)((n - 256) >> 8); }
+        else { h[p++] = 0xA0 | ck; h[p++] = (uint8_t)n; h[p++] = (uint8_t)(n >> 8); h[p++] = (uint8_t)(n >> 16); h[p++] = (uint8_t)(n >> 24); }
     } else {
-        h[p++] = 0x80; h[p++] = 0x58;
+        h[p++] = 0x80 | ck; h[p++] = 0x58;
         h[p++] = (uint8_t)n; h[p++] = (uint8_t)(n >> 8); h[p++] = (uint8_t)(n >> 16); h[p++] = (uint8_t)(n >> 24);
     }
     return p;
 }
 __device__ __forceinline__ uint32_t ze_frame_header_size(uint32_t n) {
     return n <= (1u << 21) ? (n < 256 ? 6u : n < 65536 + 256 ? 7u : 9u) : 10u;
+}
+// The frame of an empty chunk: header, one empty last Raw block [, the checksum of no bytes].  Returns its size.
+__device__ __forceinline__ uint32_t ze_empty_frame(uint8_t* frame, bool checksum) {
+    uint32_t p = ze_frame_header(frame, 0, checksum);
+    frame[p++] = 1; frame[p++] = 0; frame[p++] = 0;
+    if (checksum) { for (int k = 0; k < 4; k++) frame[p++] = (uint8_t)(XXH64_EMPTY_LOW32 >> (8 * k)); }
+    return p;
+}
+
+// ------------------------------------------------------------------------------------------ Content_Checksum
+// With TSGPU_FLAG_ZSTD_CHECKSUM the compressor's grid gains `hash_rows` rows of CTAs IN FRONT of the chunks' rows: they have the
+// lowest block indices, so they are dispatched first and hash while the other CTAs compress.  Warp k of those CTAs, counted
+// across the rows, hashes chunk k (xxh64.cuh: the chunk's four XXH64 chains take ~n/32 dependent rounds, milliseconds for a
+// 4 MiB chunk, which the compression of the other chunks hides).  The 4 bytes go right after the chunk's last block and are
+// written by whichever finishes second -- the hash warp, or the unit (region / block) that placed the last block -- decided by
+// one word per chunk: both add 1 << 32 to it, the hash warp adds its hash too.  Neither ever waits for the other.
+__device__ __forceinline__ void ze_put_u32le(uint8_t* p, uint32_t v) {
+    p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24);
+}
+__device__ TS_NOINLINE void ze_hash_warp(const uint8_t* in_base, const uint64_t* in_off, const uint32_t* in_len, uint8_t* out_base,
+                                         const uint64_t* out_off, const uint32_t* out_len, unsigned long long* ck_state,
+                                         uint32_t n_chunks, uint32_t chunk, uint64_t* stage, uint32_t lane) {
+    if (chunk >= n_chunks) return;
+    const uint32_t clen = in_len[chunk];
+    if (clen == 0) return;                                   // ze_empty_frame carries the checksum of no bytes
+    const uint32_t h = xxh64_warp_low32(in_base + in_off[chunk], clen, stage, lane);
+    if (lane == 0) {
+        const unsigned long long old = atomicAdd(&ck_state[chunk], (1ull << 32) | h);
+        if (old >> 32) {                                     // the last block is placed, and out_len (its end + 4) published
+            __threadfence();
+            const uint32_t end = *(const volatile uint32_t*)&out_len[chunk];
+            ze_put_u32le(out_base + out_off[chunk] + end - 4, h);
+        }
+    }
+}
+// The unit that placed the chunk's last block, which ends at `at`, after publishing out_len (one lane).
+__device__ __forceinline__ void ze_ck_unit_done(unsigned long long* ck, uint8_t* at) {
+    __threadfence();                                         // out_len before the hand-over word
+    const unsigned long long old = atomicAdd(ck, 1ull << 32);
+    if (old >> 32) ze_put_u32le(at, (uint32_t)old);          // the hash warp was first: its hash is in the word
 }
 
 // ------------------------------------------------------------------------------------------ look-back words
@@ -405,15 +451,17 @@ __device__ __forceinline__ uint32_t ze_lookback(unsigned long long* st, uint32_t
 __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const __grid_constant__ ZstdEncArgs A) {
     TS_DYN_SMEM(smem);
     const uint32_t tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-    const uint32_t chunk = blockIdx.y, region = blockIdx.x;
+    if (blockIdx.y < A.hash_rows) {                      // a hashing CTA: one chunk per warp (Content_Checksum)
+        ze_hash_warp(A.in_base, A.in_off, A.in_len, A.out_base, A.out_off, A.out_len, A.ck_state, A.n_chunks,
+                     (blockIdx.y * gridDim.x + blockIdx.x) * ZR_SLICES + w, (uint64_t*)(smem + w * XXH_STAGE_BYTES), lane);
+        return;
+    }
+    const uint32_t chunk = blockIdx.y - A.hash_rows, region = blockIdx.x;
     const uint32_t clen = A.in_len[chunk];
     uint8_t* frame = A.out_base + A.out_off[chunk];
+    const bool checksum = A.ck_state != nullptr;
     if (clen == 0) {                                     // empty chunk: header + empty last raw block
-        if (region == 0 && tid == 0) {
-            const uint32_t hl = ze_frame_header(frame, 0);
-            frame[hl] = 1; frame[hl + 1] = 0; frame[hl + 2] = 0;
-            A.out_len[chunk] = hl + 3;
-        }
+        if (region == 0 && tid == 0) A.out_len[chunk] = ze_empty_frame(frame, checksum);
         return;
     }
     if ((uint64_t)region * ZR >= clen) return;           // whole CTA
@@ -670,11 +718,14 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
     if (w == 0) {
         unsigned long long* rs = A.reg_state + (size_t)chunk * A.regions_per_chunk;
         const uint32_t hl = ze_frame_header_size(clen);
-        if (region == 0 && lane == 0) ze_frame_header(frame, clen);
+        if (region == 0 && lane == 0) ze_frame_header(frame, clen, checksum);
         const uint32_t base = ze_lookback(rs, region, total, hl, region + 1 == nreg, lane);
         if (lane == 0) {
             R->frame_base = base;
-            if (region + 1 == nreg) A.out_len[chunk] = base + total;
+            if (region + 1 == nreg) {
+                A.out_len[chunk] = base + total + (checksum ? 4u : 0u);
+                if (checksum) ze_ck_unit_done(A.ck_state + chunk, frame + base + total);
+            }
         }
     }
     __syncthreads();
@@ -757,15 +808,18 @@ inline const char* zstd_enc_scratch_alloc(ZstdEncScratch& s, uint32_t chunk_cap,
     if ((e = rt::malloc_device((void**)&s.slot_a, nblk * ZE_SLOT_A + 256))) return e;
     if ((e = rt::malloc_device((void**)&s.slot_b, nblk * ZE_SLOT_B + 256))) return e;
     if ((e = rt::malloc_device((void**)&s.reg_state, (size_t)s.regions_per_chunk * max_batch * 8 + 256))) return e;
+    if ((e = rt::malloc_device((void**)&s.ck_state, (size_t)max_batch * 8 + 256))) return e;
     return nullptr;
 }
 inline void zstd_enc_scratch_free(ZstdEncScratch& s) {
     rt::free_device(s.seqs); rt::free_device(s.lits); rt::free_device(s.slot_a); rt::free_device(s.slot_b); rt::free_device(s.reg_state);
+    rt::free_device(s.ck_state);
     s = ZstdEncScratch{};
 }
 
+// checksum: end every frame with its Content_Checksum, hashed by extra CTAs of the same launch (ze_hash_warp)
 inline int zstd_compress_batch(ZstdEncScratch& s, rt::stream_t st, const uint8_t* in_base, const uint64_t* d_in_off,
-                               const uint32_t* d_in_len, uint32_t n_chunks, uint32_t chunk_size,
+                               const uint32_t* d_in_len, uint32_t n_chunks, uint32_t chunk_size, bool checksum,
                                uint8_t* out_base, const uint64_t* d_out_off, uint32_t* d_out_len, LaunchProf& prof) {
     if (n_chunks > s.max_batch) { g_zstd_err = "batch larger than the context"; return -1; }
     uint32_t rpc = (chunk_size + ZR - 1) / ZR;
@@ -776,9 +830,14 @@ inline int zstd_compress_batch(ZstdEncScratch& s, rt::stream_t st, const uint8_t
     A.seqs = s.seqs; A.lits = s.lits; A.slot_a = s.slot_a; A.slot_b = s.slot_b; A.reg_state = s.reg_state;
     A.blocks_per_chunk = s.blocks_per_chunk; A.regions_per_chunk = s.regions_per_chunk;
     A.out_base = out_base; A.out_off = d_out_off; A.out_len = d_out_len;
+    A.ck_state = checksum ? s.ck_state : nullptr;
+    A.n_chunks = n_chunks;
+    A.hash_rows = checksum ? ((n_chunks + ZR_SLICES - 1) / ZR_SLICES + rpc - 1) / rpc : 0;    // one warp per chunk
     const char* e = rt::memset_async(s.reg_state, 0, (size_t)s.regions_per_chunk * n_chunks * 8, st);
+    if (!e && checksum) e = rt::memset_async(s.ck_state, 0, (size_t)n_chunks * 8, st);
     if (e) { g_zstd_err = e; return -7; }
-    TS_LAUNCH_P(prof, "zstd_enc_regions", zstd_enc_regions_kernel, dim3(rpc, n_chunks), dim3(ZE_THREADS), ZE_SMEM_BYTES, st, A);
+    static_assert(ZE_SMEM_BYTES >= ZR_SLICES * XXH_STAGE_BYTES, "hashing warps stage in the region buffer");
+    TS_LAUNCH_P(prof, "zstd_enc_regions", zstd_enc_regions_kernel, dim3(rpc, n_chunks + A.hash_rows), dim3(ZE_THREADS), ZE_SMEM_BYTES, st, A);
     e = rt::last_error();
     if (e) { g_zstd_err = e; return -7; }
     return 0;

@@ -100,6 +100,7 @@ struct ZstdBlkScratch {
     uint2* seqs = nullptr;           // blocks * ZE_MAXSEQ
     uint8_t* lits = nullptr;         // blocks * ZB
     unsigned long long* blk_state = nullptr;   // blocks: look-back words (ready bit 63 | inclusive frame bytes)
+    unsigned long long* ck_state = nullptr;    // chunks: Content_Checksum hand-over words (ze_hash_warp)
     uint32_t blocks_per_chunk = 0, max_batch = 0;
 };
 struct ZstdBlkArgs {
@@ -107,6 +108,8 @@ struct ZstdBlkArgs {
     uint8_t* blk_out; uint32_t* blk_size; uint2* seqs; uint8_t* lits; unsigned long long* blk_state;
     uint32_t blocks_per_chunk;
     uint8_t* out_base; const uint64_t* out_off; uint32_t* out_len;
+    unsigned long long* ck_state;    // as in ZstdEncArgs: null without the Content_Checksum
+    uint32_t hash_rows, n_chunks;
 };
 
 // Raw_Literals_Block with the 3-byte header (Size_Format 11: 20-bit Regenerated_Size).
@@ -259,17 +262,17 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
     // which block this warp owns, its scratch slots and its shared-memory window
     TS_DYN_SMEM(smem);
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (blockIdx.y < A.hash_rows) {                               // a hashing CTA: one chunk per warp (Content_Checksum)
+        ze_hash_warp(A.in_base, A.in_off, A.in_len, A.out_base, A.out_off, A.out_len, A.ck_state, A.n_chunks,
+                     (blockIdx.y * gridDim.x + blockIdx.x) * ZB_WPB + warp, (uint64_t*)(smem + warp * XXH_STAGE_BYTES), lane);
+        return;
+    }
 
-    const uint32_t chunk = blockIdx.y;
+    const uint32_t chunk = blockIdx.y - A.hash_rows;
     const uint32_t blk = blockIdx.x * ZB_WPB + warp;
     const uint32_t clen = A.in_len[chunk];
     if (clen == 0 && blk == 0) {                                  // empty chunk: header + empty last raw block
-        if (lane == 0) {
-            uint8_t* frame = A.out_base + A.out_off[chunk];
-            const uint32_t hl = ze_frame_header(frame, 0);
-            frame[hl] = 1; frame[hl + 1] = 0; frame[hl + 2] = 0;
-            A.out_len[chunk] = hl + 3;
-        }
+        if (lane == 0) A.out_len[chunk] = ze_empty_frame(A.out_base + A.out_off[chunk], A.ck_state != nullptr);
         return;
     }
     if ((uint64_t)blk * ZB >= clen) return;                       // whole warp
@@ -526,10 +529,13 @@ __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const _
         const uint32_t bsize_all = 3 + (payload == 0xffffffffu ? bn : payload);
         unsigned long long* st = A.blk_state + (size_t)chunk * A.blocks_per_chunk;
         uint8_t* frame = A.out_base + A.out_off[chunk];
-        if (blk == 0 && lane == 0) ze_frame_header(frame, clen);
+        if (blk == 0 && lane == 0) ze_frame_header(frame, clen, A.ck_state != nullptr);
         __threadfence();                                           // (the slot's bytes are this warp's own: ordered by the warp sync below)
         const uint32_t base = ze_lookback(st, blk, bsize_all, ze_frame_header_size(clen), last_block, lane);
-        if (last_block && lane == 0) A.out_len[chunk] = base + bsize_all;
+        if (last_block && lane == 0) {
+            A.out_len[chunk] = base + bsize_all + (A.ck_state ? 4u : 0u);
+            if (A.ck_state) ze_ck_unit_done(A.ck_state + chunk, frame + base + bsize_all);
+        }
         __syncwarp();
         ZB_MARK(7);
         ze_warp_copy(frame + base, out, bsize_all, lane);
@@ -548,16 +554,19 @@ inline const char* zstd_blk_scratch_alloc(ZstdBlkScratch& s, uint32_t chunk_cap,
     if ((e = rt::malloc_device((void**)&s.seqs, nblk * ZE_MAXSEQ * sizeof(uint2) + 256))) return e;
     if ((e = rt::malloc_device((void**)&s.lits, nblk * ZB + 256))) return e;
     if ((e = rt::malloc_device((void**)&s.blk_state, nblk * 8 + 256))) return e;
+    if ((e = rt::malloc_device((void**)&s.ck_state, (size_t)max_batch * 8 + 256))) return e;
     return nullptr;
 }
 inline void zstd_blk_scratch_free(ZstdBlkScratch& s) {
     rt::free_device(s.blk_out); rt::free_device(s.blk_size); rt::free_device(s.seqs); rt::free_device(s.lits); rt::free_device(s.blk_state);
+    rt::free_device(s.ck_state);
     s = ZstdBlkScratch{};
 }
 constexpr uint32_t ZB_SMEM_BYTES = ZB_WPB * ZB_SMEM_WARP_AL;
+static_assert(ZB_SMEM_BYTES >= ZB_WPB * XXH_STAGE_BYTES && ZB_SMEM_WARP_AL % 16 == 0, "hashing warps stage in the block buffers");
 
 inline int zstd_compress_batch_blocks(ZstdBlkScratch& s, rt::stream_t st, const uint8_t* in_base, const uint64_t* d_in_off,
-                                      const uint32_t* d_in_len, uint32_t n_chunks, uint32_t chunk_size,
+                                      const uint32_t* d_in_len, uint32_t n_chunks, uint32_t chunk_size, bool checksum,
                                       uint8_t* out_base, const uint64_t* d_out_off, uint32_t* d_out_len, LaunchProf& prof) {
     if (n_chunks > s.max_batch) { g_zstd_err = "batch larger than the context"; return -1; }
     const uint32_t bpc = (chunk_size + ZB - 1) / ZB;
@@ -568,9 +577,13 @@ inline int zstd_compress_batch_blocks(ZstdBlkScratch& s, rt::stream_t st, const 
     A.blocks_per_chunk = s.blocks_per_chunk;
     A.out_base = out_base; A.out_off = d_out_off; A.out_len = d_out_len;
     const uint32_t gx = bpc ? (bpc + ZB_WPB - 1) / ZB_WPB : 1;   // (empty chunks still get their frame from block 0)
+    A.ck_state = checksum ? s.ck_state : nullptr;
+    A.n_chunks = n_chunks;
+    A.hash_rows = checksum ? ((n_chunks + ZB_WPB - 1) / ZB_WPB + gx - 1) / gx : 0;     // one warp per chunk (ze_hash_warp)
     const char* e = rt::memset_async(s.blk_state, 0, (size_t)s.blocks_per_chunk * n_chunks * 8, st);
+    if (!e && checksum) e = rt::memset_async(s.ck_state, 0, (size_t)n_chunks * 8, st);
     if (e) { g_zstd_err = e; return -7; }
-    TS_LAUNCH_P(prof, "zstd_enc_blocks", zstd_enc_blocks_kernel, dim3(gx, n_chunks), dim3(ZB_WPB * 32), ZB_SMEM_BYTES, st, A);
+    TS_LAUNCH_P(prof, "zstd_enc_blocks", zstd_enc_blocks_kernel, dim3(gx, n_chunks + A.hash_rows), dim3(ZB_WPB * 32), ZB_SMEM_BYTES, st, A);
     e = rt::last_error();
     if (e) { g_zstd_err = e; return -7; }
     return 0;
