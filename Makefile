@@ -45,3 +45,6 @@ tests/cpp/test_host_mirror_gpu: tests/cpp/test_host_mirror.cpp $(PKG)/host/chunk
 # JNI glue compiled as it stands against a test-only stand-in for <jni.h> and driven through a fake JNIEnv (no JDK here)
 tests/cpp/test_jni_shim_simt: tests/cpp/test_jni_shim.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so oracle
 	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_shim.c -Ltests/simt -ltsgpu_simt -Loracle -ltsoracle -Wl,-rpath,'$$ORIGIN/../simt' -Wl,-rpath,'$$ORIGIN/../../oracle'
+# JNI glue's record-validation path (RecordsCursor.transformCursor) in the window flow of GpuTransformChunkEnumeration, same fake JNIEnv
+tests/cpp/test_jni_records_simt: tests/cpp/test_jni_records.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so
+	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_records.c -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'

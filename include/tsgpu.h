@@ -54,6 +54,21 @@ extern "C" {
  * beside the compression (cost: DESIGN.md §8).  TSGPU_ZSTD_CHECKSUM=1 in the environment makes the flag the default of a
  * context's transform calls. */
 #define TSGPU_FLAG_ZSTD_CHECKSUM 16u
+/* Validation of the Kafka log segment given to tsgpu_transform / tsgpu_transform_cursor, on the GPU, before any of its bytes are
+ * uploaded: every entry `offset i64 | size i32 | ...` (12 + size bytes; the entries must end exactly at the end of the segment;
+ * an empty segment is valid) is checked as DefaultRecordBatch.ensureValid() checks a batch -- magic 2: size >= 49 and the
+ * CRC-32C at +17 over [+21, end); magic 0/1 (legacy message sets): size >= 14 and the CRC-32 at +12 over [+16, end); any other
+ * magic fails.  Records inside a batch are not parsed.  The first invalid entry fails the call with TSGPU_E_RECORDS.  The check
+ * reads the bytes the transform already copied to HBM and adds no copy; the transformed bytes are exactly those written without
+ * the flag.  It combines with ZSTD, ZSTD_DENSE, ZSTD_CHECKSUM, AES and VERIFY and needs ZSTD or AES (TSGPU_E_ARG without: with
+ * flags 0 the transform is a host memcpy and no byte reaches the GPU).  tsgpu_transform_chunks and the device-resident calls
+ * refuse it (TSGPU_E_ARG: index blobs are not record batches, and the device calls have no status output on the transform side);
+ * detransform ignores it.  TSGPU_VALIDATE_RECORDS=1 in the environment makes the flag the default of a context's
+ * tsgpu_transform_cursor calls that have ZSTD or AES: those callers say where their segment ends, and the JNI enumeration
+ * transforms every window of a segment that way.  It does not reach tsgpu_transform, which a caller may also use for one
+ * window of a segment (a window checked as a whole segment would fail where an entry crosses its end).  Cost and memory:
+ * DESIGN.md §3 and §8. */
+#define TSGPU_FLAG_VALIDATE_RECORDS 32u
 
 #define TSGPU_IV_SIZE   12     /* SegmentEncryptionMetadataV1.java:30 */
 #define TSGPU_TAG_SIZE  16     /* AesEncryptionProvider.java:38 (128-bit tag) */
@@ -71,6 +86,11 @@ extern "C" {
  * frame, size, or the first byte offset that differs.  No byte of the failing batch reaches dst; earlier batches may
  * already be there, and the caller discards the whole result as with any error. */
 #define TSGPU_E_VERIFY     -9
+/* TSGPU_FLAG_VALIDATE_RECORDS: a record batch failed validation.  The message names the segment byte position of the first
+ * invalid entry and the check that failed -- "Record batch is corrupt (check: length)" / "(check: magic)", or "Record is corrupt
+ * (stored crc = S, computed crc = C) (check: crc)".  No byte of the failing batch reaches dst; earlier batches may already be
+ * there, as with TSGPU_E_VERIFY. */
+#define TSGPU_E_RECORDS   -10
 
 typedef struct tsgpu_ctx tsgpu_ctx;
 
@@ -88,7 +108,8 @@ const char* tsgpu_version(void);
  * Environment (read once by tsgpu_create): TSGPU_SLOTS=1..16 slots per device, TSGPU_ZSTD_MODE=dense makes
  * TSGPU_FLAG_ZSTD_DENSE the context's default (both tuning only), TSGPU_VERIFY=1 turns TSGPU_FLAG_VERIFY on for the
  * context's host-buffer transform calls (not for the device-resident calls), TSGPU_ZSTD_CHECKSUM=1 turns
- * TSGPU_FLAG_ZSTD_CHECKSUM on for all of the context's compressing transform calls.
+ * TSGPU_FLAG_ZSTD_CHECKSUM on for all of the context's compressing transform calls, TSGPU_VALIDATE_RECORDS=1 turns
+ * TSGPU_FLAG_VALIDATE_RECORDS on for the context's tsgpu_transform_cursor calls with ZSTD or AES.
  * --------------------------------------------------------------------------------------------------------- */
 int  tsgpu_create(const int* device_ids, int n_devices, uint32_t max_chunk_bytes, uint32_t max_batch,
                   tsgpu_ctx** out);
@@ -121,6 +142,22 @@ int tsgpu_transform(tsgpu_ctx* ctx, uint32_t flags,
                     const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
                     uint8_t* dst, uint64_t dst_cap,
                     uint32_t* transformed_sizes, uint32_t* n_chunks);
+
+/* A segment transformed in several calls (windows of chunks, as a streaming caller reads it) with
+ * TSGPU_FLAG_VALIDATE_RECORDS: entries cross the calls, so the validation state goes from one call to the next in a cursor.  A
+ * zeroed cursor is the start of a segment; each call continues at the byte after the previous call's last one and updates the
+ * cursor on success (after a failure it is meaningless).  The cursor holds what an entry that straddles the end of the call
+ * needs: its start, its end, the running CRC with its kind and the stored value, and up to 21 header bytes when the call ends
+ * inside its header.  segment_ends_here != 0 marks the last call (a short or empty window): a segment that ends inside an entry
+ * then fails with check "length".  Without the flag (or its environment default) the cursor is not used and may be NULL.
+ * With the flag, tsgpu_transform is tsgpu_transform_cursor with a zeroed cursor and segment_ends_here = 1. */
+typedef struct tsgpu_records_cursor { uint64_t opaque[8]; } tsgpu_records_cursor;
+int tsgpu_transform_cursor(tsgpu_ctx* ctx, uint32_t flags,
+                           const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
+                           const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                           uint8_t* dst, uint64_t dst_cap,
+                           uint32_t* transformed_sizes, uint32_t* n_chunks,
+                           tsgpu_records_cursor* cursor, int segment_ends_here);
 
 /* Ragged variant of tsgpu_transform: chunk i is the next chunk_lens[i] bytes of src (no fixed chunk size).
  * Replaces the per-index chains of RemoteStorageManager.transformIndex (RemoteStorageManager.java:455-490; each Kafka

@@ -21,6 +21,10 @@ import io.aiven.kafka.tieredstorage.transform.TransformChunkEnumeration;
  * <p>The segment stream is read straight into a pinned direct buffer (no byte[] bounce in front of the H2D copy).
  * The two pinned staging buffers come from a per-context {@link PinnedPool} and go back to it when the stream is
  * exhausted, on {@link #close()}, or — as a last resort — when the enumeration is garbage collected.
+ *
+ * <p>One enumeration is one segment, so it keeps one {@link RecordsCursor} across its windows and marks the last (short
+ * or empty) window: with record validation on (the validateRecords argument, or TSGPU_VALIDATE_RECORDS=1 in the
+ * environment) a record batch that crosses a window is checked whole, and a segment that ends inside a batch fails.
  */
 public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, AutoCloseable {
     private final long ctx;
@@ -30,6 +34,7 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
     private final int flags;
     private final DataKeyAndAAD keyAndAad;   // null when encryption is off
     private final int batchChunks;
+    private final RecordsCursor records = new RecordsCursor();
     private final SecureRandom random = new SecureRandom();
     private final ArrayDeque<byte[]> ready = new ArrayDeque<>();
     private final PinnedPool pool;
@@ -40,6 +45,14 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
     public GpuTransformChunkEnumeration(final long ctx, final PinnedPool pool, final InputStream inputStream,
                                         final int originalChunkSize, final boolean compression,
                                         final DataKeyAndAAD keyAndAad, final int batchChunks) {
+        this(ctx, pool, inputStream, originalChunkSize, compression, keyAndAad, batchChunks, false);
+    }
+
+    /** validateRecords: check every record batch of the segment on the GPU (TsGpu.FLAG_VALIDATE_RECORDS); it applies when the
+     *  segment is compressed or encrypted, otherwise the bytes are copied on the host and never reach the GPU. */
+    public GpuTransformChunkEnumeration(final long ctx, final PinnedPool pool, final InputStream inputStream,
+                                        final int originalChunkSize, final boolean compression,
+                                        final DataKeyAndAAD keyAndAad, final int batchChunks, final boolean validateRecords) {
         if (inputStream == null) {
             throw new NullPointerException("inputStream cannot be null");
         }
@@ -52,7 +65,8 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
         this.inputStream = inputStream;
         this.channel = Channels.newChannel(inputStream);
         this.originalChunkSize = originalChunkSize;
-        this.flags = (compression ? TsGpu.FLAG_ZSTD : 0) | (keyAndAad != null ? TsGpu.FLAG_AES : 0);
+        final int transforms = (compression ? TsGpu.FLAG_ZSTD : 0) | (keyAndAad != null ? TsGpu.FLAG_AES : 0);
+        this.flags = transforms | (validateRecords && transforms != 0 ? TsGpu.FLAG_VALIDATE_RECORDS : 0);
         this.keyAndAad = keyAndAad;
         this.batchChunks = batchChunks;
         if (originalChunkSize > 0) {
@@ -110,7 +124,10 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
                 }
             }
             final long total = in.position();
-            if (total == 0) {
+            if (total == 0) {                            // the segment ended with the previous, full window
+                records.transform(ctx, flags, in, 0, originalChunkSize,
+                    keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                    new byte[TsGpu.IV_SIZE], dst.buffer(), new int[0], true);
                 release();
                 return;
             }
@@ -122,9 +139,9 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             random.nextBytes(ivs);
             final int[] sizes = new int[chunks];
             final ByteBuffer out = dst.buffer();
-            final int n = TsGpu.transform(ctx, flags, in, total, originalChunkSize,
+            final int n = records.transform(ctx, flags, in, total, originalChunkSize,
                 keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
-                ivs, out, sizes);
+                ivs, out, sizes, eof);
             out.clear();
             for (int i = 0; i < n; i++) {
                 final byte[] chunk = new byte[sizes[i]];
@@ -161,9 +178,9 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             random.nextBytes(ivs);
             final int[] sizes = new int[1];
             final ByteBuffer out = dst.buffer();
-            final int n = TsGpu.transform(ctx, flags, in, all.length, 0,
+            final int n = records.transform(ctx, flags, in, all.length, 0,
                 keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
-                ivs, out, sizes);
+                ivs, out, sizes, true);
             out.clear();
             for (int i = 0; i < n; i++) {
                 final byte[] chunk = new byte[sizes[i]];

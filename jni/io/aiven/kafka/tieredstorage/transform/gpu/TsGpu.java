@@ -8,6 +8,10 @@ public final class TsGpu {
     public static final int FLAG_AES = 2;
     // flags pass through to the C-ABI unchanged: TSGPU_FLAG_ZSTD_CHECKSUM (16, include/tsgpu.h) ends every zstd frame with its
     // Content_Checksum; TSGPU_ZSTD_CHECKSUM=1 in the broker's environment turns it on without a change here
+    /** Check every record batch of the segment (length, magic, CRC) on the GPU before it is uploaded; needs FLAG_ZSTD or
+     *  FLAG_AES.  A damaged batch fails the call with a RuntimeException, so Kafka keeps the local segment and retries the
+     *  copy.  Segments that arrive in windows carry the state from one window to the next in a {@link RecordsCursor}. */
+    public static final int FLAG_VALIDATE_RECORDS = 32;
     public static final int IV_SIZE = 12;
 
     static {

@@ -3,7 +3,7 @@
  * There is no JDK in this repository's build image: the tests compile this file against a test-only stand-in for
  * <jni.h> and drive it through a fake JNIEnv (tests/cpp/test_jni_shim.c).  Build on the broker host with
  *   gcc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude jni/tsgpu_jni.c -L<pkg> -ltsgpu -o libtsgpu_jni.so
- * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
+ * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
  * (implement TransformChunkEnumeration / DetransformChunkEnumeration of the reference, core/M/transform/TransformChunkEnumeration.java:28-42,
  * DetransformChunkEnumeration.java:28-29) and jni/io/aiven/kafka/tieredstorage/fetch/gpu/GpuChunkManager.java (ChunkManager, fetch/ChunkManager.java).
  *
@@ -60,10 +60,10 @@ JNIEXPORT jlong JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_tr
                                                                                              jlong srcLen, jint chunkSize) {
     return (jlong)tsgpu_transform_bound((uint32_t)flags, (uint64_t)srcLen, (uint32_t)chunkSize);
 }
-/* returns the number of chunks; transformedSizes (int[]) receives one entry per chunk */
-JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_transform(
-    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
-    jbyteArray ivs, jobject dst, jintArray transformedSizes) {
+/* tsgpu_transform, or tsgpu_transform_cursor when `cursor` is given; returns the number of chunks, or -1 with an exception
+ * pending.  transformedSizes (int[]) receives one entry per chunk. */
+static jint transform_call(JNIEnv* env, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
+                           jbyteArray ivs, jobject dst, jintArray transformedSizes, tsgpu_records_cursor* cursor, int segmentEndsHere) {
     jlong dcap = 0;
     uint8_t* s = direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer");
     if (!s) return -1;
@@ -85,14 +85,34 @@ JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_tra
         return -1;
     }
     jint* sizes = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
-    int rc = tsgpu_transform((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
-                             (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n);
+    int rc = cursor
+        ? tsgpu_transform_cursor((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
+                                 (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n,
+                                 cursor, segmentEndsHere)
+        : tsgpu_transform((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
+                          (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n);
     (*env)->ReleaseIntArrayElements(env, transformedSizes, sizes, 0);
     if (k) (*env)->ReleaseByteArrayElements(env, key, k, JNI_ABORT);
     if (a) (*env)->ReleaseByteArrayElements(env, aad, a, JNI_ABORT);
     if (iv) (*env)->ReleaseByteArrayElements(env, ivs, iv, JNI_ABORT);
-    if (rc) { throw_rt(env, rc); return -1; }
+    if (rc) { throw_rt(env, rc); return -1; }           /* TSGPU_E_RECORDS too: a RuntimeException, the copy is retried */
     return (jint)n;
+}
+JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_transform(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
+    jbyteArray ivs, jobject dst, jintArray transformedSizes) {
+    return transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, NULL, 0);
+}
+/* One window of a segment (RecordsCursor.transformCursor): `cursor` is a direct ByteBuffer of at least 64 bytes holding the
+ * tsgpu_records_cursor (zeros at the start of the segment), updated in place; segmentEndsHere marks the segment's last window. */
+JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RecordsCursor_transformCursor(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
+    jbyteArray ivs, jobject dst, jintArray transformedSizes, jobject cursor, jboolean segmentEndsHere) {
+    jlong ccap = 0;
+    tsgpu_records_cursor* cur = (tsgpu_records_cursor*)direct(env, cursor, 0, &ccap, "cursor must be a direct ByteBuffer of 64 bytes");
+    if (!cur) return -1;
+    if (ccap < (jlong)sizeof(tsgpu_records_cursor)) { throw_arg(env, "cursor must be a direct ByteBuffer of 64 bytes"); return -1; }
+    return transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, cur, segmentEndsHere ? 1 : 0);
 }
 JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_detransform(
     JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray transformedSizes, jbyteArray key, jbyteArray aad,

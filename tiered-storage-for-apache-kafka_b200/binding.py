@@ -16,11 +16,14 @@ FLAG_AES = 2
 FLAG_ZSTD_DENSE = 4
 FLAG_VERIFY = 8          # host-buffer transforms: read each batch back on the device before releasing it
 FLAG_ZSTD_CHECKSUM = 16  # with FLAG_ZSTD: every frame ends with its Content_Checksum (XXH64 of the chunk, checked by every reader)
+FLAG_VALIDATE_RECORDS = 32  # segment transforms with ZSTD or AES: check every Kafka record batch's length, magic and CRC first
 IV_SIZE = 12
 TAG_SIZE = 16
 SLOT_HEAD = 4
 OK, E_ARG, E_STATE, E_AUTH, E_CORRUPT, E_SHORT, E_NODEVICE, E_CUDA, E_NOMEM = 0, -1, -2, -3, -4, -5, -6, -7, -8
 E_VERIFY = -9
+E_RECORDS = -10
+CURSOR_SIZE = 64         # tsgpu_records_cursor
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",
@@ -29,6 +32,7 @@ SYMBOLS = [
     "tsgpu_chunk_sizes_encode", "tsgpu_chunk_sizes_decode", "tsgpu_transformed_chunks_serialize",
     "tsgpu_transformed_chunks_deserialize", "tsgpu_chunk_index_json", "tsgpu_profile_enable", "tsgpu_profile_report",
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
+    "tsgpu_transform_cursor",
 ]
 
 
@@ -64,6 +68,7 @@ def load(path=None):
     L.tsgpu_slot_stride.restype = u64
     L.tsgpu_slot_stride.argtypes = [u32, u32]
     L.tsgpu_transform.argtypes = [vp, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
+    L.tsgpu_transform_cursor.argtypes = [vp, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp, vp, C.c_int]
     L.tsgpu_transform_chunks.argtypes = [vp, u32, vp, vp, u32, vp, vp, u32, vp, vp, u64, vp]
     L.tsgpu_detransform.argtypes = [vp, u32, vp, u64, vp, u32, vp, vp, u32, vp, u64, vp]
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
@@ -162,6 +167,24 @@ class Context:
         k, a, iv = _u8(key), _u8(aad), _u8(ivs)
         self._check(self.lib.tsgpu_transform(self._h, flags, _p(s), s.size, chunk_size, _p(k), _p(a), a.size, _p(iv),
                                              dst.ctypes.data, dst.size, sizes.ctypes.data, C.addressof(n)))
+        sizes = sizes[:n.value]
+        return dst[:int(sizes.sum(dtype=np.uint64))], [int(x) for x in sizes]
+
+    def transform_cursor(self, flags, src, chunk_size, cursor, segment_ends_here, key=None, aad=b"", ivs=None):
+        """One window of a segment with FLAG_VALIDATE_RECORDS: `cursor` is a 64-byte np.uint8 array (zeros at the start of the
+        segment), updated in place on success.  Returns (transformed bytes, [transformed sizes])."""
+        s = _u8(src)
+        if not (isinstance(cursor, np.ndarray) and cursor.dtype == np.uint8 and cursor.size == CURSOR_SIZE and cursor.flags.c_contiguous):
+            raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % CURSOR_SIZE)
+        cs = chunk_size if chunk_size else max(s.size, 1)
+        n_max = (s.size + cs - 1) // cs + 1
+        dst = np.empty(int(self.lib.tsgpu_transform_bound(flags, s.size, chunk_size)) + 64, dtype=np.uint8)
+        sizes = np.zeros(n_max, dtype=np.uint32)
+        n = C.c_uint32(n_max)
+        k, a, iv = _u8(key), _u8(aad), _u8(ivs)
+        self._check(self.lib.tsgpu_transform_cursor(self._h, flags, _p(s), s.size, chunk_size, _p(k), _p(a), a.size, _p(iv),
+                                                    dst.ctypes.data, dst.size, sizes.ctypes.data, C.addressof(n),
+                                                    cursor.ctypes.data, 1 if segment_ends_here else 0))
         sizes = sizes[:n.value]
         return dst[:int(sizes.sum(dtype=np.uint64))], [int(x) for x in sizes]
 

@@ -7,7 +7,9 @@
 //   [AES-GCM kernels], D2H of the chunk sizes, then per-chunk D2H of exactly transformed_size bytes to the
 //   running offset in dst (the packed .log object layout, SURVEY.md appendix A.1).  Batches complete in order;
 //   up to (devices x slots) batches are in flight so copies overlap kernels.  With TSGPU_FLAG_VERIFY each batch is
-//   detransformed on the device and compared with its input before any of its bytes are copied out.
+//   detransformed on the device and compared with its input before any of its bytes are copied out.  With
+//   TSGPU_FLAG_VALIDATE_RECORDS the Kafka log entries of each batch are checked on the device (records.cuh) and the batch's
+//   verdict is resolved, in batch order, before its bytes are copied out.
 #include <condition_variable>
 #include <mutex>
 #include <new>
@@ -22,6 +24,7 @@
 #include "index_scan.cuh"
 #include "pack.cuh"
 #include "verify.cuh"
+#include "records.cuh"
 #include "rt.h"
 #include "launch_prof.h"
 #include "zstd_enc.cuh"
@@ -64,6 +67,15 @@ struct Desc {            // device-side descriptor block of one work slot (all a
     uint8_t* ivs; uint8_t* aad;
 };
 
+// Device arrays of the record validation of one slot (records.cuh), sized for batches of up to `cap` bytes.
+struct RecScratch {
+    uint8_t* d = nullptr;
+    uint64_t cap = 0;
+    RecArgs a{};                   // the batch last enqueued on the slot: rec_resolve reads the same arrays at its drain
+    RecOut* d_out = nullptr;
+    RecOut* h_out = nullptr;       // pinned
+};
+
 struct Work {
     int device = 0;
     rt::stream_t stream{}, out_stream{};   // out_stream: copies of finished chunks back to the host
@@ -87,6 +99,7 @@ struct Work {
     ZstdBlkScratch zblk{};         // block kernel (default), allocated on first use
     ZstdDecScratch zdec{};
     uint32_t* h_sizes = nullptr;   // pinned: sizes/status (and the verify stage's first differing bytes) coming back
+    RecScratch rec{};              // TSGPU_FLAG_VALIDATE_RECORDS, allocated on first use
 };
 
 struct Lane { int device = 0; Work w[NSLOT_MAX]; };
@@ -97,6 +110,7 @@ struct tsgpu_ctx {
     bool dense_default = false;    // TSGPU_ZSTD_MODE=dense: TSGPU_FLAG_ZSTD alone already means the region kernel
     bool verify_default = false;   // TSGPU_VERIFY=1: host-buffer transforms verify as if TSGPU_FLAG_VERIFY were set
     bool checksum_default = false; // TSGPU_ZSTD_CHECKSUM=1: every frame carries its Content_Checksum, as with TSGPU_FLAG_ZSTD_CHECKSUM
+    bool records_default = false;  // TSGPU_VALIDATE_RECORDS=1: tsgpu_transform_cursor calls with ZSTD or AES validate their record batches
     std::mutex mu;                 // guards slot ownership (Work::claimed, active_calls) and lazy slot allocation — NOT held while a call runs
     std::condition_variable cv;
     uint32_t active_calls = 0;
@@ -165,6 +179,7 @@ static void work_free(Work& w) {
     rt::free_device(w.d_desc); rt::free_host(w.h_desc);
     rt::free_device(w.d_partials); rt::free_device(w.d_keyctx); rt::free_host(w.h_sizes);
     zstd_enc_scratch_free(w.zenc); zstd_blk_scratch_free(w.zblk); zstd_dec_scratch_free(w.zdec);
+    rt::free_device(w.rec.d); rt::free_device(w.rec.d_out); rt::free_host(w.rec.h_out); w.rec = RecScratch{};
     memset(&w.key_rk, 0, sizeof w.key_rk); w.key_valid = false;
     rt::event_destroy(w.ev_sizes); rt::event_destroy(w.ev_done);
     rt::event_destroy(w.ev_dev_desc); rt::event_destroy(w.ev_dev_done);
@@ -207,6 +222,7 @@ extern "C" int tsgpu_create(const int* device_ids, int n_devices, uint32_t max_c
     if (const char* e = getenv("TSGPU_ZSTD_MODE")) c->dense_default = strcmp(e, "dense") == 0;
     if (const char* e = getenv("TSGPU_VERIFY")) c->verify_default = strcmp(e, "1") == 0;
     if (const char* e = getenv("TSGPU_ZSTD_CHECKSUM")) c->checksum_default = strcmp(e, "1") == 0;
+    if (const char* e = getenv("TSGPU_VALIDATE_RECORDS")) c->records_default = strcmp(e, "1") == 0;
     c->frame_stride = align_up(frame_bound(max_chunk_bytes), 16) + 16;
     c->slot_stride = tsgpu_slot_stride(TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES, max_chunk_bytes);
     c->lanes.resize(ids.size());
@@ -514,6 +530,87 @@ static int verify_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, 
     return TSGPU_OK;
 }
 
+// ------------------------------------------------------------------------------------------ record validation
+// Largest batch the validation indexes: positions are 31-bit (node indices carry a terminal bit).
+constexpr uint64_t REC_MAX_BATCH = 0x7fffff00ull;
+
+static int records_alloc(RecScratch& r, uint64_t L) {
+    if (r.cap >= L) return TSGPU_OK;
+    rt::free_device(r.d); r.d = nullptr; r.cap = 0;
+    const uint64_t np = (L + REC_PIECE - 1) / REC_PIECE, nt = (L + REC_TILE - 1) / REC_TILE;
+    const uint64_t sz[7] = {8 * np, 8 * nt, 8 * nt, 4 * nt, 4 * (nt + 1), 4 * L, 8 * L};
+    uint64_t total = 0;
+    for (uint64_t b : sz) total += align_up(b, 256);
+    RT(rt::malloc_device((void**)&r.d, total));
+    if (!r.d_out) RT(rt::malloc_device((void**)&r.d_out, sizeof(RecOut)));
+    if (!r.h_out) RT(rt::malloc_host((void**)&r.h_out, sizeof(RecOut)));
+    uint8_t* p = r.d;
+    auto take = [&](uint64_t b) { uint8_t* q = p; p += align_up(b, 256); return q; };
+    r.a.pin = (uint32_t*)take(sz[0]); r.a.ttot = (uint32_t*)take(sz[1]); r.a.tex = (uint32_t*)take(sz[2]);
+    r.a.cnt = (uint32_t*)take(sz[3]); r.a.tbase = (uint32_t*)take(sz[4]); r.a.cpos = (uint32_t*)take(sz[5]);
+    r.a.node = (unsigned long long*)take(sz[6]);
+    r.cap = L;
+    return TSGPU_OK;
+}
+
+// Enqueues the validation of the batch's L original bytes in d_orig: every kernel but the resolve, which waits for the drain.
+static int records_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint64_t L) {
+    RecArgs& a = w.rec.a;
+    a.b = w.d_orig; a.L = (uint32_t)L;
+    a.npieces = (uint32_t)((L + REC_PIECE - 1) / REC_PIECE); a.ntiles = (uint32_t)((L + REC_TILE - 1) / REC_TILE);
+    TS_LAUNCH_P(c->prof, "rec_scan", rec_scan_kernel, dim3(a.ntiles), dim3(REC_T), 0, st, a);
+    CHECK_LAUNCH("rec_scan_kernel");
+    TS_LAUNCH_P(c->prof, "rec_tiles", rec_tiles_kernel, dim3(1), dim3(REC_TILES_T), 0, st, a);
+    CHECK_LAUNCH("rec_tiles_kernel");
+    TS_LAUNCH_P(c->prof, "rec_place", rec_place_kernel, dim3(a.ntiles), dim3(REC_T), 0, st, a);
+    CHECK_LAUNCH("rec_place_kernel");
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(264, (L + 16383) / 16384);
+    TS_LAUNCH_P(c->prof, "rec_link", rec_link_kernel, dim3(grid), dim3(REC_LINK_T), 0, st, a);
+    CHECK_LAUNCH("rec_link_kernel");
+    for (uint64_t reach = 1; reach < L; reach *= REC_JUMPS + 1) {       // at most L candidates; every launch multiplies the reach
+        TS_LAUNCH_P(c->prof, "rec_jump", rec_jump_kernel, dim3(grid), dim3(REC_LINK_T), 0, st, a);
+        CHECK_LAUNCH("rec_jump_kernel");
+    }
+    return TSGPU_OK;
+}
+
+static int records_failure(const RecOut& o) {
+    const unsigned long long at = (unsigned long long)o.fail;
+    switch (o.kind) {
+    case REC_MAGIC:
+        return fail(TSGPU_E_RECORDS, "Record batch is corrupt (check: magic): the entry at segment position %llu has magic %u, not 0, 1 or 2", at, o.magic);
+    case REC_LENGTH:
+        return fail(TSGPU_E_RECORDS, "Record batch is corrupt (check: length): the entry at segment position %llu does not fit: size %d, "
+                    "below the minimum for its magic or past the end of the segment", at, o.size);
+    case REC_CRC:
+        return fail(TSGPU_E_RECORDS, "Record is corrupt (stored crc = %u, computed crc = %u) (check: crc): the entry at segment position %llu",
+                    o.stored, o.computed, at);
+    default:
+        return fail(TSGPU_E_CUDA, "record validation did not resolve the entry at segment position %llu", at);
+    }
+}
+
+// The drained batch's verdict, in batch order: the carry of the batches before it goes in, its own comes out.
+static int records_resolve(tsgpu_ctx* c, Work& w, RecCarry& carry) {
+    TS_LAUNCH_P(c->prof, "rec_resolve", rec_resolve_kernel, dim3(1), dim3(32), 0, w.stream, w.rec.a, carry, w.rec.d_out);
+    CHECK_LAUNCH("rec_resolve_kernel");
+    RT(rt::d2h(w.rec.h_out, w.rec.d_out, sizeof(RecOut), w.stream));
+    RT(rt::stream_sync(w.stream));
+    if (w.rec.h_out->kind != REC_OK) return records_failure(*w.rec.h_out);
+    carry = w.rec.h_out->carry;
+    return TSGPU_OK;
+}
+
+// A segment that ends inside an entry: the entry is too long for it (or, with its magic byte there, has a bad one).
+static int records_segment_end(const RecCarry& carry) {
+    if (!carry.open) return TSGPU_OK;
+    RecOut o{};
+    o.fail = carry.start; o.kind = REC_LENGTH;
+    o.size = carry.hlen >= 12 ? (int32_t)((uint32_t)carry.hdr[8] << 24 | (uint32_t)carry.hdr[9] << 16 | (uint32_t)carry.hdr[10] << 8 | carry.hdr[11]) : 0;
+    if (carry.hlen > 16) { o.magic = carry.hdr[16]; if (o.magic > 2) o.kind = REC_MAGIC; }
+    return records_failure(o);
+}
+
 #ifdef TSGPU_SIMT
 // TEST-ONLY fault injection, compiled into the emulator build alone (device memory is host memory there and every kernel
 // has finished when its launch returns).  TSGPU_SIMT_FLIP=<chunk>:<offset> flips the low bit of one byte of that chunk's
@@ -532,7 +629,7 @@ static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
 // One batch: copy in, fill the descriptors, enqueue the stages, pack the transformed chunks, [verify them,] D2H of their
 // sizes (and of the verify stage's verdicts).
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
-static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, const uint8_t* src, const uint64_t* off,
+static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, const uint8_t* src, const uint64_t* off,
                            const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
                            const uint8_t* ivs) {
     Work& w = *bt.w;
@@ -578,6 +675,11 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool v
         RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
         RT(rt::d2h(w.h_sizes + 2 * nb, w.dd.v_diff, 4ull * nb, st));
     }
+    if (records) {
+        int rc = records_alloc(w.rec, (uint64_t)c->max_batch * cs);
+        if (!rc) rc = records_stage(c, w, st, byte1 - byte0);
+        if (rc) return rc;
+    }
     RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
     return TSGPU_OK;
@@ -602,36 +704,84 @@ static int verify_verdict(const Batch& bt, const uint32_t* len) {
 
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
-                            const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks);
+                            const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                            RecCarry* records);
 
 static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint8_t* key, const uint8_t* aad,
                              uint32_t aad_len, const uint8_t* ivs, uint32_t* transformed_sizes, uint32_t* n_chunks) {
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
     if (!n_chunks || !transformed_sizes) return fail(TSGPU_E_ARG, "transformed_sizes/n_chunks cannot be null");
     if (src_len && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
-    if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
+    if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY | TSGPU_FLAG_VALIDATE_RECORDS)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if ((flags & TSGPU_FLAG_AES) && (!key || !ivs)) return fail(TSGPU_E_ARG, "key and ivs are required for encryption");
     if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
     if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
     return TSGPU_OK;
 }
 
+static_assert(sizeof(tsgpu_records_cursor) == sizeof(RecCarry), "the cursor holds the carry");
+static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
+                             const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
+                             uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
+                             bool env_default);
+
 extern "C" int tsgpu_transform(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
                                const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
-                               uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks) try {
+                               uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks) {
+    // One call is the whole segment.  The environment default does not reach this call: streaming callers (the JNI
+    // enumeration) pass one window of a segment per call, and a window validated as a segment would fail where an entry
+    // crosses its end.
+    tsgpu_records_cursor whole{};
+    return transform_segment(c, flags, src, src_len, chunk_size, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, n_chunks,
+                             &whole, 1, /*env_default=*/false);
+}
+
+extern "C" int tsgpu_transform_cursor(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
+                                      const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                                      uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                                      tsgpu_records_cursor* cursor, int segment_ends_here) {
+    return transform_segment(c, flags, src, src_len, chunk_size, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, n_chunks,
+                             cursor, segment_ends_here, /*env_default=*/true);
+}
+
+static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
+                             const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
+                             uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
+                             bool env_default) try {
     int rc = transform_args_ok(c, flags, src, src_len, key, aad, aad_len, ivs, transformed_sizes, n_chunks);
     if (rc) return rc;
+    const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
+    if ((flags & TSGPU_FLAG_VALIDATE_RECORDS) && !(flags & xf))
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_VALIDATE_RECORDS (%u) needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU",
+                    TSGPU_FLAG_VALIDATE_RECORDS);
+    const bool records = (flags & TSGPU_FLAG_VALIDATE_RECORDS) || (env_default && c->records_default && (flags & xf));
+    if (records && !cursor) return fail(TSGPU_E_ARG, "cursor cannot be null when record batches are validated");
+    RecCarry carry{};
+    if (records) memcpy(&carry, cursor, sizeof carry);
     // BaseTransformChunkEnumeration: originalChunkSize 0 disables chunking (one chunk = whole stream)
     uint64_t cs64 = chunk_size ? chunk_size : src_len;
-    if (src_len == 0) { *n_chunks = 0; return TSGPU_OK; }
+    if (src_len == 0) {
+        if (records && segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
+        *n_chunks = 0;
+        return TSGPU_OK;
+    }
     if (cs64 > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk size %llu exceeds the context's max_chunk_bytes %u", (unsigned long long)cs64, c->chunk_cap);
     const uint32_t cs = (uint32_t)cs64;
+    if (records && (uint64_t)c->max_batch * cs > REC_MAX_BATCH)
+        return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch, cs);
     const uint64_t n64 = (src_len + cs - 1) / cs;
     if (n64 > *n_chunks) return fail(TSGPU_E_SHORT, "transformed_sizes too small: %llu chunks", (unsigned long long)n64);
     std::vector<uint64_t> off(n64);
     std::vector<uint32_t> len(n64);
     for (uint64_t i = 0; i < n64; i++) { off[i] = i * cs; len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - i * cs); }
-    return transform_common(c, flags, src, src_len, off, len, cs, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, n_chunks);
+    rc = transform_common(c, flags & ~TSGPU_FLAG_VALIDATE_RECORDS, src, src_len, off, len, cs, key, aad, aad_len, ivs, dst, dst_cap,
+                          transformed_sizes, n_chunks, records ? &carry : nullptr);
+    if (rc) return rc;
+    if (records) {
+        if (segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
+        memcpy(cursor, &carry, sizeof carry);
+    }
+    return TSGPU_OK;
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
 // Ragged variant: chunk i is the next chunk_lens[i] bytes of src.  This is what RemoteStorageManager.transformIndex
@@ -641,6 +791,9 @@ extern "C" int tsgpu_transform_chunks(tsgpu_ctx* c, uint32_t flags, const uint8_
                                       const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
                                       uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes) try {
     uint32_t cap = n;
+    if (flags & TSGPU_FLAG_VALIDATE_RECORDS)
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_VALIDATE_RECORDS (%u) applies to segments, not to ragged chunks such as index files",
+                    TSGPU_FLAG_VALIDATE_RECORDS);
     if (n && !chunk_lens) return fail(TSGPU_E_ARG, "chunk_lens cannot be null");
     uint64_t total = 0; uint32_t mx = 0;
     std::vector<uint64_t> off(n);
@@ -653,12 +806,13 @@ extern "C" int tsgpu_transform_chunks(tsgpu_ctx* c, uint32_t flags, const uint8_
     if (rc) return rc;
     if (n == 0) return TSGPU_OK;
     if (mx > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk size %u exceeds the context's max_chunk_bytes %u", mx, c->chunk_cap);
-    return transform_common(c, flags, src, total, off, len, mx, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, &cap);
+    return transform_common(c, flags, src, total, off, len, mx, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, &cap, nullptr);
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
-                            const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks) {
+                            const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                            RecCarry* records) {
     const uint32_t n = (uint32_t)len.size();
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
     if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~ZSTD_MODIFIERS;         // modifiers of ZSTD: meaningless (and harmless) without it
@@ -677,9 +831,10 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
 
     uint64_t dst_off = 0;
     const int rc = run_batches(c, n,
-        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
+        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, records != nullptr, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
         [&](const Batch& bt) {
             Work& w = *bt.w;
+            if (records) { int rcr = records_resolve(c, w, *records); if (rcr) return rcr; }   // the input first: none of the batch's bytes leave
             if (verify) { int rcv = verify_verdict(bt, len.data()); if (rcv) return rcv; }   // none of the batch's bytes leave
             uint64_t total = 0;
             for (uint32_t i = 0; i < bt.nb; i++) { transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
@@ -736,6 +891,7 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
                                  const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                                  uint8_t* dst, uint64_t dst_cap, uint32_t* original_sizes) try {
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
+    flags &= ~TSGPU_FLAG_VALIDATE_RECORDS;                   // a property of the upload: nothing to do on the way back
     if (n_chunks == 0) return TSGPU_OK;
     if (!src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
     if (!transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
@@ -796,6 +952,8 @@ static int dev_args_ok(tsgpu_ctx* c, int device_index, uint32_t flags, uint32_t 
     if (device_index < 0 || device_index >= (int)c->lanes.size()) return fail(TSGPU_E_ARG, "device_index %d out of range", device_index);
     if (flags & TSGPU_FLAG_VERIFY)
         return fail(TSGPU_E_ARG, "TSGPU_FLAG_VERIFY (%u) applies to the host-buffer transform calls only", TSGPU_FLAG_VERIFY);
+    if (flags & TSGPU_FLAG_VALIDATE_RECORDS)
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_VALIDATE_RECORDS (%u) applies to the host-buffer segment transform only", TSGPU_FLAG_VALIDATE_RECORDS);
     if ((flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)) == 0 || (flags & ~KNOWN_FLAGS)) return fail(TSGPU_E_ARG, "flags must name zstd and/or aes");
     if (chunk_size == 0 || chunk_size > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk_size out of range for this context");
     if (n == 0) return TSGPU_OK;

@@ -13,7 +13,9 @@
 //   v2:  baseOffset i64 | batchLength i32 | partitionLeaderEpoch i32 | magic i8 (=2) | crc u32 (CRC-32C of everything
 //        after it) | attributes i16 (bits 0-2 = compression codec) | ... 61 bytes of header in all
 //   v0/v1: offset i64 | size i32 | crc u32 (CRC-32 of everything after it) | magic i8 | attributes i8 (bits 0-2) | ...
-// Everything here is plain CPU code: the GPU never sees record batches.
+// SegmentCompressionChecker below is plain CPU code and checks the first batch only, as the reference does.  With
+// SegmentLogUploader::validateRecords every entry of the segment is checked on the GPU inside the transform call
+// (TSGPU_FLAG_VALIDATE_RECORDS, csrc/records.cuh), against the same layout and checksums.
 #pragma once
 #include <chrono>
 #include <cstdint>
@@ -173,12 +175,17 @@ public:
         if (!ctx) throw NullPointerException("ctx cannot be null");
         if (chunkSize < 0) throw IllegalArgumentException("originalChunkSize must be non-negative, " + std::to_string(chunkSize) + " given");
     }
+    // Check every record batch of the segment before it is uploaded (TSGPU_FLAG_VALIDATE_RECORDS): a damaged batch fails the
+    // upload with InvalidRecordBatchException, so the copy is retried and the local segment kept.  It applies when the segment
+    // is compressed or encrypted: otherwise the transform is a plain copy on the host and no byte reaches the GPU.
+    bool validateRecords = false;
     // `log`/`n`: the segment file (ideally in memory from tsgpu_host_alloc); `ivs`: 12 bytes per chunk when encrypting.
     SegmentLogUpload upload(const uint8_t* log, uint64_t n, const DataKeyAndAAD* key, const uint8_t* ivs, const PartSink& sink) {
         if (n > 0x7fffffffull) throw IllegalArgumentException("originalFileSize must fit an int");
         SegmentLogUpload r;
         r.compressed = requiresCompression(compressionEnabled, compressionHeuristic, log, (size_t)n);
         uint32_t flags = (r.compressed ? TSGPU_FLAG_ZSTD : 0u) | (encryptionEnabled ? TSGPU_FLAG_AES : 0u);
+        const uint32_t callFlags = flags | (validateRecords && flags ? TSGPU_FLAG_VALIDATE_RECORDS : 0u);
         if (encryptionEnabled) {
             if (!key || !ivs) throw NullPointerException("cipherSupplier cannot be null");
             if (key->dataKey.size() != 32) throw IllegalArgumentException("dataKey must be 32 bytes");
@@ -192,8 +199,9 @@ public:
         uint32_t nChunks = (uint32_t)((n + per - 1) / per);
         std::vector<uint32_t> sizes(nChunks ? nChunks : 1);
         uint32_t got = (uint32_t)sizes.size();
-        const int rc = tsgpu_transform(ctx, flags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
+        const int rc = tsgpu_transform(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
                                        key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got);
+        if (rc == TSGPU_E_RECORDS) throw InvalidRecordBatchException(tsgpu_last_error());
         if (rc) throw std::runtime_error(tsgpu_last_error());            // RuntimeException in the reference
         // TransformFinisher: fixed index when every chunk has the same known transformed size, variable after compression
         const int ocs = chunkSize ? chunkSize : (int)n;
