@@ -4,7 +4,7 @@ CSRC := $(PKG)/csrc
 NVCC ?= nvcc
 NVCCFLAGS := -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC,-Wall -Xptxas -v \
              --expt-relaxed-constexpr
-HDRS := $(wildcard $(CSRC)/*.cuh $(CSRC)/*.h $(CSRC)/*.hpp $(CSRC)/*.inc) include/tsgpu.h
+HDRS := $(wildcard $(CSRC)/*.cuh $(CSRC)/*.h $(CSRC)/*.hpp) include/tsgpu.h
 
 all: $(PKG)/libtsgpu.so oracle tests/simt/libtsgpu_simt.so
 libtsgpu.so: $(PKG)/libtsgpu.so

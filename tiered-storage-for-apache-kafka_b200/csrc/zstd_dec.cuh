@@ -280,46 +280,6 @@ __device__ __forceinline__ bool zd_huf_stream(const uint16_t* __restrict__ huf, 
     return b.bits == 0;
 }
 
-// The same for a destination in global memory: symbols leave four at a time as one 32-bit store once the destination is
-// aligned, and the bit window is reloaded once per four symbols (4 * 11 bits fit behind the <= 7 already-consumed bits of a
-// byte-aligned 64-bit window).  Overruns inside a group of four only read zeros (the peek zero-extends) and are caught after it.
-__device__ __forceinline__ bool zd_huf_stream_packed(const uint16_t* __restrict__ huf, uint32_t log, const uint8_t* src, uint32_t size,
-                                                     uint8_t* dst, uint32_t count) {
-    ZdBack b;
-    if (!zd_back_init(b, src, size)) return false;
-    uint32_t i = 0;
-    const uint32_t head = min(count, (4u - (uint32_t)((uintptr_t)dst & 3)) & 3u);
-    for (; i < head; i++) {
-        const uint16_t e = huf[zd_back_peek(b, log)];
-        dst[i] = (uint8_t)e;
-        b.bits -= (int32_t)(e >> 8);
-    }
-    if (b.bits < 0) return false;
-    const uint32_t mask = (1u << log) - 1;
-    while (i + 4 <= count && b.bits >= 64) {
-        const int32_t cbase = ((b.bits + 7) & ~7) - 64;
-        const uint64_t C = zd_ld64(b.p + (cbase >> 3));
-        int32_t pos = b.bits - cbase;                    // 57..64 unread bits of C
-        uint32_t out = 0;
-        _Pragma("unroll")
-        for (int k = 0; k < 4; k++) {
-            const uint16_t e = huf[(uint32_t)(C >> (pos - (int32_t)log)) & mask];
-            out |= (uint32_t)(e & 0xff) << (8 * k);
-            pos -= (int32_t)(e >> 8);
-        }
-        *(uint32_t*)(dst + i) = out;
-        b.bits = cbase + pos;
-        i += 4;
-    }
-    for (; i < count; i++) {
-        const uint16_t e = huf[zd_back_peek(b, log)];
-        dst[i] = (uint8_t)e;
-        b.bits -= (int32_t)(e >> 8);
-        if (b.bits < 0) return false;
-    }
-    return b.bits == 0;
-}
-
 // Sequence table of one kind according to its compression mode.  Lane 0.  Returns bytes consumed, -1 on error.
 // Warp-parallel build of a sequence decoding table whose distribution has no "less than one" symbols (what this
 // library's writer emits): the spread then has the closed form pos(i) = i*step & mask, a cell's symbol is found by
@@ -400,37 +360,68 @@ template <class CX> __device__ TS_NOINLINE int32_t zd_seq_table(uint32_t mode, i
     return *validp ? 0 : -1;
 }
 
-// Literals_Section_Header of a Compressed_Block, one lane; a Huffman tree description is read into cx.  out: type, header
-// size, Regenerated_Size, Compressed_Size (incl. the tree), streams, tree-description bytes.  false: malformed.
+// 3-byte Block_Header (RFC 8878 §3.1.1.2).
+struct ZdBlkHdr { uint32_t last, type, size; };
+__device__ __forceinline__ ZdBlkHdr zd_block_header(const uint8_t* p) {
+    const uint32_t h = p[0] | (p[1] << 8) | ((uint32_t)p[2] << 16);
+    return ZdBlkHdr{h & 1, (h >> 1) & 3, h >> 3};
+}
+
+// Literals section of a Compressed_Block: type, header size, Regenerated_Size, Compressed_Size (Raw: the bytes, RLE: 1,
+// Compressed / Treeless: the streams, a Huffman tree description included), streams, tree-description bytes.
+struct ZdLitSec { uint32_t type, hs, regen, comp, streams, tree; };
+// Field decode of the Literals_Section_Header (tree = 0).  hs = 0: the block is too short to hold the header.
+__device__ __forceinline__ ZdLitSec zd_lit_section(const uint8_t* blk, uint32_t bsize) {
+    ZdLitSec L{0, 0, 0, 0, 1, 0};
+    if (bsize < 2) return L;                            // Compressed_Block needs at least literals header + seq header
+    const uint32_t b0 = blk[0], sf = (b0 >> 2) & 3;
+    L.type = b0 & 3;
+    if (L.type < 2) {
+        if ((sf & 1) == 0) { L.hs = 1; L.regen = b0 >> 3; }
+        else if (sf == 1) { L.hs = 2; L.regen = (b0 >> 4) | ((uint32_t)blk[1] << 4); }
+        else { if (bsize < 3) return L; L.hs = 3; L.regen = (b0 >> 4) | ((uint32_t)blk[1] << 4) | ((uint32_t)blk[2] << 12); }
+        L.comp = L.type == 0 ? L.regen : 1;
+    } else {
+        if (bsize < 5) return L;
+        const uint32_t h = blk[0] | ((uint32_t)blk[1] << 8) | ((uint32_t)blk[2] << 16) | ((uint32_t)blk[3] << 24);
+        if (sf <= 1) { L.hs = 3; L.regen = (h >> 4) & 0x3ff; L.comp = (h >> 14) & 0x3ff; L.streams = sf == 0 ? 1 : 4; }
+        else if (sf == 2) { L.hs = 4; L.regen = (h >> 4) & 0x3fff; L.comp = h >> 18; L.streams = 4; }
+        else { L.hs = 5; L.regen = (h >> 4) & 0x3ffff; L.comp = (h >> 22) | ((uint32_t)blk[4] << 10); L.streams = 4; }
+    }
+    return L;
+}
+
+// Literals_Section_Header of a Compressed_Block, one lane; a Huffman tree description is read into cx.  false: malformed.
 // Treeless literals with no_inherit set cx->err = 1 ("needs the general path") and still return true.
 template <class CX> __device__ __forceinline__ bool zd_parse_lit_header(const uint8_t* blk, uint32_t bsize, uint32_t limit, uint32_t litcap,
-                                                                        bool no_inherit, CX* cx, uint32_t* out) {
-    if (bsize < 2) return false;                        // Compressed_Block needs at least literals header + seq header
-    const uint32_t b0 = blk[0], type = b0 & 3, sf = (b0 >> 2) & 3;
-    uint32_t hs, regen, comp = 0, streams = 1;
-    if (type < 2) {
-        if ((sf & 1) == 0) { hs = 1; regen = b0 >> 3; }
-        else if (sf == 1) { hs = 2; regen = (b0 >> 4) | ((uint32_t)blk[1] << 4); }
-        else { if (bsize < 3) return false; hs = 3; regen = (b0 >> 4) | ((uint32_t)blk[1] << 4) | ((uint32_t)blk[2] << 12); }
-        comp = type == 0 ? regen : 1;
-    } else {
-        if (bsize < 5) return false;
-        const uint32_t h = blk[0] | ((uint32_t)blk[1] << 8) | ((uint32_t)blk[2] << 16) | ((uint32_t)blk[3] << 24);
-        if (sf <= 1) { hs = 3; regen = (h >> 4) & 0x3ff; comp = (h >> 14) & 0x3ff; streams = sf == 0 ? 1 : 4; }
-        else if (sf == 2) { hs = 4; regen = (h >> 4) & 0x3fff; comp = h >> 18; streams = 4; }
-        else { hs = 5; regen = (h >> 4) & 0x3ffff; comp = (h >> 22) | ((uint32_t)blk[4] << 10); streams = 4; }
-    }
-    if (hs + comp > bsize || regen > limit || regen > zf::BLOCK_MAX) return false;
-    if (type >= 2 && regen > litcap) return false;
-    uint32_t tree = 0;
-    if (type == 2) {
-        tree = zd_read_huf_table(blk + hs, comp, cx);
-        if (!tree) return false;
-    } else if (type == 3) {
+                                                                        bool no_inherit, CX* cx, ZdLitSec& L) {
+    L = zd_lit_section(blk, bsize);
+    if (!L.hs || L.hs + L.comp > bsize || L.regen > limit || L.regen > zf::BLOCK_MAX) return false;
+    if (L.type >= 2 && L.regen > litcap) return false;
+    if (L.type == 2) {
+        L.tree = zd_read_huf_table(blk + L.hs, L.comp, cx);
+        if (!L.tree) return false;
+    } else if (L.type == 3) {
         if (no_inherit) { cx->err = 1; }
         else if (!cx->huf_valid) return false;
     }
-    out[0] = type; out[1] = hs; out[2] = regen; out[3] = comp; out[4] = streams; out[5] = tree;
+    return true;
+}
+
+// Stream k (0..3) of a 4-stream Huffman literals section src[0..size) of `regen` symbols: where its bytes start (past the
+// 6-byte jump table), how many there are, its first symbol and its symbol count.  false: the jump table does not fit.
+struct ZdHufStream { uint32_t off, size, first, count; };
+__device__ __forceinline__ bool zd_huf4_stream(const uint8_t* src, uint32_t size, uint32_t regen, uint32_t k, ZdHufStream& s) {
+    if (size < 10) return false;
+    const uint32_t s1 = src[0] | (src[1] << 8), s2 = src[2] | (src[3] << 8), s3 = src[4] | (src[5] << 8);
+    if (6 + s1 + s2 + s3 > size) return false;
+    const uint32_t s4 = size - 6 - s1 - s2 - s3;
+    const uint32_t per = (regen + 3) / 4;
+    s.off = 6 + (k == 0 ? 0 : k == 1 ? s1 : k == 2 ? s1 + s2 : s1 + s2 + s3);
+    s.size = k == 0 ? s1 : k == 1 ? s2 : k == 2 ? s3 : s4;
+    s.first = k * per;
+    if (s.first > regen || (k == 3 && 3 * per > regen)) return false;
+    s.count = k < 3 ? min(per, regen - s.first) : regen - s.first;
     return true;
 }
 
@@ -462,23 +453,363 @@ template <class CX> __device__ __forceinline__ bool zd_parse_seq_header(const ui
     return true;
 }
 
+// ------------------------------------------------------------------------------------------ sequence words of the arenas
+// Sequence word of the arenas: bits 0..29 offset field, 30..46 literal length, 47..63 match length - 3.
+// Offset field: a concrete offset (< 2^29), or — when the sequence used a repeat offset that reaches back to the state the
+// block STARTED with, which the entropy stage cannot know — bit 29 set, bits 27..28 = which of the three initial repeat
+// offsets (1..3), bits 0..26 = how much was subtracted from it (the "rep1 - 1" form, RFC 8878 §3.1.1.5).
+constexpr uint32_t ZD_OFF_SYM = 1u << 29;
+constexpr uint32_t ZD_SYM_D = (1u << 27) - 1;
+// Does a sequence (offset value ofv as decoded: <= 3 a repeat code) fit the word?
+__device__ __forceinline__ bool zd_seq_fits(uint32_t ofv, uint32_t ll, uint32_t ml) {
+    return (ofv <= 3 || ofv - 3 < ZD_OFF_SYM) && ll < (1u << 17) && ml - 3 < (1u << 17);
+}
+__device__ __forceinline__ uint64_t zd_seq_pack(uint32_t of, uint32_t ll, uint32_t ml) {
+    return (uint64_t)of | ((uint64_t)ll << 30) | ((uint64_t)(ml - 3) << 47);
+}
+__device__ __forceinline__ void zd_seq_unpack(uint64_t v, uint32_t& of, uint32_t& ll, uint32_t& ml) {
+    of = (uint32_t)v & (2 * ZD_OFF_SYM - 1);
+    ll = (uint32_t)(v >> 30) & 0x1ffffu; ml = (uint32_t)(v >> 47) + 3;
+}
+// The repeat offset k (1..3) a block starts with, as a symbol.
+__device__ __forceinline__ uint32_t zd_sym_rep(uint32_t k) { return ZD_OFF_SYM | (k << 27); }
+// A symbolic offset field against the repeat offsets R0..R2 its block started with: returns the one it names, *d what was
+// subtracted from it.  The offset is that minus *d, which only exists when it is larger than *d.
+__device__ __forceinline__ uint32_t zd_sym_base(uint32_t of, uint32_t R0, uint32_t R1, uint32_t R2, uint32_t* d) {
+    const uint32_t k = (of >> 27) & 3;
+    *d = of & ZD_SYM_D;
+    return k == 1 ? R0 : k == 2 ? R1 : R2;
+}
+__device__ __forceinline__ uint32_t zd_rep_sub1(uint32_t v) {            // "rep1 - 1" on an offset field; 0 = invalid
+    if (v & ZD_OFF_SYM) return (v & ZD_SYM_D) == ZD_SYM_D ? 0u : v + 1;   // symbolic: one more subtracted
+    return v - 1;                                                        // concrete: 0 when the offset was 1 (corrupt)
+}
+
+// ------------------------------------------------------------------------------------------ stages of a compressed block
+// Warp-uniform.  Each stage returns false where the block cannot go on: cx->err is then set (<0 corrupt, >0 needs another
+// path), the warp agrees on it and the caller returns.
+
+// Literals section header (lane 0 parses, the warp shares it through cx->tmp); a Huffman tree description is read into cx.
+__device__ __forceinline__ bool zd_stage_lit_header(const uint8_t* blk, uint32_t bsize, uint32_t limit, ZdWarpCtx* cx, uint32_t lane,
+                                                    ZdLitSec& L) {
+    if (lane == 0) {
+        ZdLitSec h;
+        if (zd_parse_lit_header(blk, bsize, limit, zf::BLOCK_MAX, false, cx, h)) {
+            cx->tmp[1] = h.type; cx->tmp[2] = h.hs; cx->tmp[3] = h.regen; cx->tmp[4] = h.comp; cx->tmp[5] = h.streams; cx->tmp[6] = h.tree;
+            cx->tmp[0] = 1u;
+        } else cx->tmp[0] = 0u;
+    }
+    __syncwarp();
+    if (!cx->tmp[0]) { if (lane == 0 && cx->err == 0) cx->err = -1; __syncwarp(); return false; }
+    if (cx->err) return false;
+    L = ZdLitSec{cx->tmp[1], cx->tmp[2], cx->tmp[3], cx->tmp[4], cx->tmp[5], cx->tmp[6]};
+    return true;
+}
+
+// Where the literals come from: bytes (Raw in the block, Huffman decoded into litbuf by lanes 0-3) or a single RLE byte.
+struct ZdLitSrc { const uint8_t* lit; uint32_t rle_lit; };      // rle_lit 0x100: not RLE
+__device__ __forceinline__ bool zd_stage_lit_source(const uint8_t* blk, const ZdLitSec& L, ZdWarpCtx* cx, uint8_t* litbuf,
+                                                    uint32_t lane, ZdLitSrc& src) {
+    src.lit = nullptr; src.rle_lit = 0x100;
+    if (L.type == 0) src.lit = blk + L.hs;
+    else if (L.type == 1) src.rle_lit = blk[L.hs];
+    else {
+        if (L.type == 2) zd_fill_huf_warp(cx, lane);
+        const uint8_t* hsrc = blk + L.hs + L.tree;
+        const uint32_t hsize = L.comp - L.tree;
+        bool ok = true;
+        if (L.streams == 1) {
+            if (lane == 0) ok = zd_huf_stream(cx->huf, cx->huf_log, hsrc, hsize, litbuf, L.regen);
+        } else if (lane < 4) {
+            ZdHufStream s;
+            ok = zd_huf4_stream(hsrc, hsize, L.regen, lane, s) &&
+                 zd_huf_stream(cx->huf, cx->huf_log, hsrc + s.off, s.size, litbuf + s.first, s.count);
+        }
+        if (!__all_sync(TS_FULL, ok)) { if (lane == 0) cx->err = -1; __syncwarp(); return false; }
+        src.lit = litbuf;
+        __threadfence_block();
+    }
+    __syncwarp();
+    return true;
+}
+
+// Sequences section header and the three FSE tables (lane 0 reads, the warp builds).  bs: the bit stream.
+struct ZdSeqSec { uint32_t nseq; const uint8_t* bs; uint32_t bs_size; };
+__device__ __forceinline__ bool zd_stage_seq_header(const uint8_t* blk, uint32_t bsize, const ZdLitSec& L, ZdWarpCtx* cx, uint32_t lane,
+                                                    ZdSeqSec& S) {
+    const uint8_t* sp = blk + L.hs + L.comp;
+    const uint32_t ssize = bsize - L.hs - L.comp;
+    if (lane == 0) cx->tmp[0] = zd_parse_seq_header(sp, ssize, false, cx, cx->tmp + 1) ? 1u : 0u;
+    __syncwarp();
+    if (!cx->tmp[0]) { if (lane == 0 && cx->err == 0) cx->err = -1; __syncwarp(); return false; }
+    if (cx->err) return false;
+    S.nseq = cx->tmp[1];
+    {
+        const uint32_t pend = cx->tmp[3];
+        for (int k = 0; k < 3; k++) if (pend & (1u << k)) zd_build_dtable_warp(k, cx, lane);
+        __syncwarp();
+    }
+    S.bs = sp + cx->tmp[2];
+    S.bs_size = ssize - cx->tmp[2];
+    return true;
+}
+
+// Position in the sequence bit stream: the backward reader and the three FSE states (lane 0's are the real ones).
+struct ZdSeqCursor { ZdBack br; uint32_t st_ll, st_of, st_ml; };
+__device__ __forceinline__ bool zd_stage_seq_init(const ZdSeqSec& S, ZdWarpCtx* cx, uint32_t lane, ZdSeqCursor& c) {
+    c.br.p = S.bs; c.br.bits = 0; c.br.C = 0; c.br.cbase = 0x3fffffff;
+    c.st_ll = 0; c.st_of = 0; c.st_ml = 0;
+    if (S.nseq) {
+        if (lane == 0) {
+            bool ok = zd_back_init(c.br, S.bs, S.bs_size);
+            if (ok) {
+                c.st_ll = zd_back_read(c.br, cx->ll_log); c.st_of = zd_back_read(c.br, cx->of_log); c.st_ml = zd_back_read(c.br, cx->ml_log);
+                if (c.br.bits < 0) ok = false;
+            }
+            if (!ok) cx->err = -1;
+        }
+        __syncwarp();
+        if (cx->err) return false;
+    }
+    return true;
+}
+
+// One decoded sequence per lane of a batch: lane < cnt (mine), literal / match length, offset value as coded (<= 3: a repeat
+// code) and the offset (ofv - 3 until repeat codes are resolved).
+struct ZdSeq { bool mine; uint32_t ll, ml, ofv, off; };
+// Sequences s0 .. s0 + cnt - 1: (1) lane 0 walks the FSE state chain, (2) every lane cuts its own sequence's offset value /
+// match length / literal length out of the stream.
+__device__ __forceinline__ bool zd_decode_batch(const ZdSeqSec& S, uint32_t s0, uint32_t cnt, ZdWarpCtx* cx, ZdSeqCursor& c,
+                                                uint32_t lane, ZdSeq& q) {
+    // (1) lane 0 walks ONLY the state chain: per sequence three table entries, the bit count, three state updates.
+    //     It records where each sequence's bits end and which states it was decoded from.
+    if (lane == 0) {
+        const uint32_t* tof = (const uint32_t*)cx->of; const uint32_t* tml = (const uint32_t*)cx->ml; const uint32_t* tll = (const uint32_t*)cx->ll;
+        const uint32_t n_upd = min(cnt, S.nseq - 1 - s0);          // sequences of this batch that are followed by another one
+        int32_t bits = c.br.bits;
+        bool bad = false;
+        uint32_t i = 0;
+        for (; i < n_upd; i++) {
+            // Bits of one sequence, first read first: offset extra, match-length extra, literal-length extra, then the
+            // LL, ML, OF state updates (<= 27 bits: one cached window).
+            const uint32_t eo = tof[c.st_of], em = tml[c.st_ml], el = tll[c.st_ll];
+            cx->s_ll[i] = c.st_of | (c.st_ml << 10) | (c.st_ll << 20);
+            cx->s_ml[i] = (uint32_t)bits;
+            const uint32_t t = eo + em + el;                         // bits 0..5: state-update bits, bits 6..11: extra bits
+            bits -= (int32_t)((t >> 6) & 63);
+            const int32_t lo = bits - (int32_t)(t & 63);
+            if (lo < 0) { bad = true; break; }
+            if (lo < c.br.cbase || bits > c.br.cbase + 64) {
+                c.br.cbase = max(0, ((bits + 7) & ~7) - 64);
+                c.br.C = zd_ld64(c.br.p + (c.br.cbase >> 3));
+            }
+            uint32_t W = (uint32_t)(c.br.C >> (lo - c.br.cbase));
+            const uint32_t u_of = eo & 63, u_ml = em & 63, u_ll = el & 63;
+            c.st_of = (eo >> 18) + (W & ((1u << u_of) - 1)); W >>= u_of;
+            c.st_ml = (em >> 18) + (W & ((1u << u_ml) - 1)); W >>= u_ml;
+            c.st_ll = (el >> 18) + (W & ((1u << u_ll) - 1));
+            bits = lo;
+        }
+        if (!bad && i < cnt) {                                   // the block's last sequence: values only
+            const uint32_t t = tof[c.st_of] + tml[c.st_ml] + tll[c.st_ll];
+            cx->s_ll[i] = c.st_of | (c.st_ml << 10) | (c.st_ll << 20);
+            cx->s_ml[i] = (uint32_t)bits;
+            bits -= (int32_t)((t >> 6) & 63);
+            if (bits < 0) bad = true;
+        }
+        c.br.bits = bits;
+        if (bad) cx->err = -1;
+    }
+    __syncwarp();
+    if (cx->err) return false;
+    // (2) every lane cuts the three values of its own sequence out of the stream
+    q.mine = lane < cnt;
+    q.ll = 0; q.ml = 0; q.off = 1; q.ofv = 4;
+    if (q.mine) {
+        const uint32_t st = cx->s_ll[lane];
+        const int32_t end = (int32_t)cx->s_ml[lane];
+        const zf::FseDEntry eo = cx->of[st & 1023], em = cx->ml[(st >> 10) & 1023], el = cx->ll[st >> 20];
+        q.ofv = (1u << eo.sym) + zd_bits_at(S.bs, end, eo.nb_extra);
+        const uint32_t v = zd_bits_at(S.bs, end - (int32_t)eo.nb_extra, (uint32_t)em.nb_extra + el.nb_extra);
+        q.ml = g_seq_tables.ml_base[em.sym] + (v >> el.nb_extra);
+        q.ll = g_seq_tables.ll_base[el.sym] + (v & ((1u << el.nb_extra) - 1));
+        q.off = q.ofv - 3;
+    }
+    return true;
+}
+
+// Repeat offsets after a batch of cnt (1..32) sequences without a repeat code: its last three offsets, shifted in.  All lanes
+// shuffle; lanes with `upd` update r0..r2.
+__device__ __forceinline__ void zd_shift_in(uint32_t off, uint32_t cnt, bool upd, uint32_t& r0, uint32_t& r1, uint32_t& r2) {
+    const uint32_t o1 = __shfl_sync(TS_FULL, off, cnt - 1), o2 = __shfl_sync(TS_FULL, off, cnt >= 2 ? cnt - 2 : 0),
+                   o3 = __shfl_sync(TS_FULL, off, cnt >= 3 ? cnt - 3 : 0);
+    if (upd) {
+        const uint32_t q0 = r0, q1 = r1;
+        r2 = cnt >= 3 ? o3 : cnt == 2 ? q0 : q1;
+        r1 = cnt >= 2 ? o2 : q0;
+        r0 = o1;
+    }
+}
+
+// Repeat offsets of a batch (RFC 8878 §3.1.1.5), state in cx->rep: batches without a repeat code (all of this library's) only
+// shift in, others are resolved serially by lane 0 and q.off becomes the offset used.  SYM: offsets may be symbolic (see
+// ZD_OFF_SYM), "rep1 - 1" by zd_rep_sub1; otherwise they are concrete and may reach bit 29, so "rep1 - 1" is r0 - 1.
+template <bool SYM> __device__ __forceinline__ bool zd_resolve_reps(ZdSeq& q, uint32_t cnt, ZdWarpCtx* cx, uint32_t lane) {
+    const uint32_t rep_mask = __ballot_sync(TS_FULL, q.mine && q.ofv <= 3);
+    if (rep_mask == 0) {
+        zd_shift_in(q.off, cnt, lane == 0, cx->rep[0], cx->rep[1], cx->rep[2]);
+        return true;
+    }
+    __syncwarp();
+    cx->s_off[lane] = q.ofv; cx->s_ml[lane] = q.ll;
+    __syncwarp();
+    if (lane == 0) {
+        uint32_t r0 = cx->rep[0], r1 = cx->rep[1], r2 = cx->rep[2];
+        for (uint32_t i = 0; i < cnt; i++) {
+            const uint32_t v = cx->s_off[i];
+            uint32_t o;
+            if (v > 3) { o = v - 3; r2 = r1; r1 = r0; r0 = o; }
+            else {
+                const uint32_t idx = v - 1 + (cx->s_ml[i] == 0 ? 1 : 0);     // 0: rep1, 1: rep2, 2: rep3, 3: rep1 - 1
+                if (idx == 0) o = r0;
+                else {
+                    const uint32_t t = idx == 1 ? r1 : idx == 2 ? r2 : SYM ? zd_rep_sub1(r0) : r0 - 1;
+                    if (t == 0) { cx->err = -1; break; }
+                    if (idx != 1) r2 = r1;
+                    r1 = r0; r0 = t; o = t;
+                }
+            }
+            cx->s_off[i] = o;
+        }
+        cx->rep[0] = r0; cx->rep[1] = r1; cx->rep[2] = r2;
+    }
+    __syncwarp();
+    if (cx->err) return false;
+    q.off = q.mine ? cx->s_off[lane] : 1;
+    return true;
+}
+
+// Executes a resolved batch into dst: lane i owns sequence i.  Output/literal positions come from shuffle prefix sums;
+// literal runs are independent; a match may start once its source range lies inside the completed prefix (multi-round
+// resolution: far matches of a batch all copy at once, so their memory latency overlaps).  `hist` bytes before dst may be
+// referenced, at most `limit` produced; advances op / lp.
+__device__ __forceinline__ bool zd_exec_batch(const ZdSeq& q, const ZdLitSrc& src, uint32_t regen, uint8_t* dst, uint64_t hist,
+                                              uint32_t limit, ZdWarpCtx* cx, uint32_t lane, uint32_t& op, uint32_t& lp) {
+    const bool mine = q.mine;
+    const uint32_t ll = q.ll, ml = q.ml, off = q.off;
+    const uint8_t* lit = src.lit;
+    const uint32_t rle_lit = src.rle_lit;
+    __syncwarp();
+    const uint32_t inc_o = warp_inclusive_scan_u32(ll + ml, lane), inc_l = warp_inclusive_scan_u32(ll, lane);
+    const uint32_t tot_o = __shfl_sync(TS_FULL, inc_o, 31), tot_l = __shfl_sync(TS_FULL, inc_l, 31);
+    const uint32_t o_start = op + inc_o - ll - ml, l_start = lp + inc_l - ll, m_start = o_start + ll;
+    const bool bad_off = mine && (uint64_t)off > hist + m_start;
+    const uint32_t any_bad = __ballot_sync(TS_FULL, bad_off);
+    if (lp + tot_l > regen || (uint64_t)op + tot_o > limit || any_bad) {
+        if (lane == 0) cx->err = -1;
+        __syncwarp();
+        return false;
+    }
+    // literals: short runs by their own lane, long runs by the whole warp
+    {
+        const uint32_t quick = min(ll, 32u);
+        if (rle_lit < 0x100) { for (uint32_t k = 0; k < quick; k++) dst[o_start + k] = (uint8_t)rle_lit; }
+        else {                                       // four loads in flight per step (lit and dst never alias)
+            const uint8_t* ls = lit + l_start; uint8_t* ld = dst + o_start;
+            uint32_t k = 0;
+            for (; k + 4 <= quick; k += 4) {
+                const uint8_t b0 = ls[k], b1 = ls[k + 1], b2 = ls[k + 2], b3 = ls[k + 3];
+                ld[k] = b0; ld[k + 1] = b1; ld[k + 2] = b2; ld[k + 3] = b3;
+            }
+            for (; k < quick; k++) ld[k] = ls[k];
+        }
+        uint32_t longs = __ballot_sync(TS_FULL, ll > 32);
+        while (longs) {
+            const uint32_t f = (uint32_t)__ffs((int)longs) - 1;
+            longs &= longs - 1;
+            const uint32_t fo = __shfl_sync(TS_FULL, o_start, f), fl = __shfl_sync(TS_FULL, l_start, f), fn = __shfl_sync(TS_FULL, ll, f);
+            if (rle_lit < 0x100) { for (uint32_t k = 32 + lane; k < fn; k += 32) dst[fo + k] = (uint8_t)rle_lit; }
+            else { for (uint32_t k = 32 + lane; k < fn; k += 32) dst[fo + k] = lit[fl + k]; }
+        }
+    }
+    __syncwarp();
+    // matches
+    bool done = !mine || ml == 0;
+    const int64_t src_end = (int64_t)m_start - (int64_t)off + (int64_t)ml;      // relative to dst
+    while (true) {
+        const uint32_t pending = __ballot_sync(TS_FULL, !done);
+        if (!pending) break;
+        const uint32_t first = (uint32_t)__ffs((int)pending) - 1;
+        const uint32_t frontier = __shfl_sync(TS_FULL, m_start, first);
+        const bool ready = !done && (lane == first || src_end <= (int64_t)frontier);
+        uint8_t* d = dst + m_start;
+        const uint8_t* m = d - off;
+        if (ready && ml <= 64) {
+            uint32_t k = 0;
+            if (off >= 4) {                              // the four source bytes of a step all precede its first store
+                for (; k + 4 <= ml; k += 4) {
+                    const uint8_t b0 = m[k], b1 = m[k + 1], b2 = m[k + 2], b3 = m[k + 3];
+                    d[k] = b0; d[k + 1] = b1; d[k + 2] = b2; d[k + 3] = b3;
+                }
+            }
+            for (; k < ml; k++) d[k] = m[k];             // byte-serial: overlap (off < ml) is fine
+            done = true;
+        }
+        uint32_t big = __ballot_sync(TS_FULL, ready && ml > 64);
+        while (big) {                                                            // long matches: 32 lanes per match
+            const uint32_t f = (uint32_t)__ffs((int)big) - 1;
+            big &= big - 1;
+            const uint32_t fm = __shfl_sync(TS_FULL, m_start, f), fl = __shfl_sync(TS_FULL, ml, f), fo = __shfl_sync(TS_FULL, off, f);
+            uint8_t* dd = dst + fm;
+            const uint8_t* mm = dd - fo;
+            if (fo >= 32) {
+                for (uint32_t k0 = 0; k0 < fl; k0 += 32) {
+                    const uint32_t k = k0 + lane;
+                    if (k < fl) dd[k] = mm[k];
+                    if (fo < fl) __syncwarp();                                   // later strides may read what this one wrote
+                }
+            } else {
+                for (uint32_t k = lane; k < fl; k += 32) dd[k] = mm[k % fo];     // periodic source entirely before dd
+            }
+            if (lane == f) done = true;
+        }
+        __syncwarp();
+    }
+    op += tot_o; lp += tot_l;
+    return true;
+}
+
+// The literals after the last sequence.
+__device__ __forceinline__ bool zd_trailing_literals(const ZdLitSrc& src, uint32_t regen, uint32_t lp, uint8_t* dst, uint32_t limit,
+                                                     ZdWarpCtx* cx, uint32_t lane, uint32_t& op) {
+    const uint32_t ll = regen - lp;
+    if ((uint64_t)op + ll > limit) { if (lane == 0) cx->err = -1; __syncwarp(); return false; }
+    if (src.rle_lit < 0x100) { for (uint32_t k = lane; k < ll; k += 32) dst[op + k] = (uint8_t)src.rle_lit; }
+    else { for (uint32_t k = lane; k < ll; k += 32) dst[op + k] = src.lit[lp + k]; }
+    op += ll;
+    return true;
+}
+
 // ------------------------------------------------------------------------------------------ one compressed block
 // Warp-uniform.  Decodes the Compressed_Block at blk[0..bsize) and appends its output at dst[0..); `hist` bytes
 // before dst belong to this frame and may be referenced; at most `limit` bytes may be produced.
-// Returns the number of bytes produced; cx->err != 0 on failure (<0 corrupt, >0 needs the general path).
+// Returns the number of bytes produced; cx->err != 0 on failure.
 __device__ __forceinline__ uint32_t zd_compressed_block(const uint8_t* blk, uint32_t bsize, uint8_t* dst, uint64_t hist,
-                                                        uint32_t limit, ZdWarpCtx* cx, uint8_t* litbuf, uint32_t litcap,
-                                                        bool fast_nonfirst, uint32_t lane) {
-#include "zd_blk_lit_header.inc"
-#include "zd_blk_lit_decode.inc"
-#include "zd_blk_seq_header.inc"
-#include "zd_blk_seq_init.inc"
-    for (uint32_t s0 = 0; s0 < nseq; s0 += 32) {
-        const uint32_t cnt = min(32u, nseq - s0);
-#include "zd_blk_decode_batch.inc"
-#include "zd_blk_exec_batch.inc"
+                                                        uint32_t limit, ZdWarpCtx* cx, uint8_t* litbuf, uint32_t lane) {
+    ZdLitSec L;
+    ZdLitSrc src;
+    ZdSeqSec S;
+    ZdSeqCursor c;
+    if (!zd_stage_lit_header(blk, bsize, limit, cx, lane, L) || !zd_stage_lit_source(blk, L, cx, litbuf, lane, src) ||
+        !zd_stage_seq_header(blk, bsize, L, cx, lane, S) || !zd_stage_seq_init(S, cx, lane, c)) return 0;
+    uint32_t op = 0, lp = 0;                            // output / literal cursors (uniform)
+    for (uint32_t s0 = 0; s0 < S.nseq; s0 += 32) {
+        const uint32_t cnt = min(32u, S.nseq - s0);
+        ZdSeq q;
+        if (!zd_decode_batch(S, s0, cnt, cx, c, lane, q) || !zd_resolve_reps<false>(q, cnt, cx, lane) ||
+            !zd_exec_batch(q, src, L.regen, dst, hist, limit, cx, lane, op, lp)) return 0;
     }
-#include "zd_blk_trailing.inc"
+    if (!zd_trailing_literals(src, L.regen, lp, dst, limit, cx, lane, op)) return 0;
     __syncwarp();
     return op;
 }
@@ -489,42 +820,28 @@ __device__ __forceinline__ uint32_t zd_compressed_block(const uint8_t* blk, uint
 // warp per frame is slow for a lone frame.  Here every block's ENTROPY decoding (Huffman literals, FSE sequences) runs on its own warp into global scratch:
 // tables a block inherits (treeless literals, Repeat_Mode) are rebuilt by replaying the table definitions of the blocks
 // before it; offsets stay unresolved offset VALUES.  One warp per frame then resolves repeat offsets and executes the
-// sequences in order.  The stages are the same textual includes the serial decoder is made of.
-// Sequence word of the arenas: bits 0..29 offset field, 30..46 literal length, 47..63 match length - 3.
-// Offset field: a concrete offset (< 2^29), or — when the sequence used a repeat offset that reaches back to the state the
-// block STARTED with, which the entropy stage cannot know — bit 29 set, bits 27..28 = which of the three initial repeat
-// offsets (1..3), bits 0..26 = how much was subtracted from it (the "rep1 - 1" form, RFC 8878 §3.1.1.5).
-constexpr uint32_t ZD_OFF_SYM = 1u << 29;
+// sequences in order.  The stages are the same functions the serial decoder is made of.
 struct ZdBlkMeta {
     uint32_t status;                 // 1 decoded, 2 failed, 3 = needs the serial path (a field does not fit the sequence word)
     uint32_t lit_kind, lit_off, regen, nseq, seq_off;      // lit_kind 0 arena, 1 in the block, 2 RLE
-    uint32_t rep[3];                 // repeat offsets after the block, in the offset-field encoding above
+    uint32_t rep[3];                 // repeat offsets after the block, in the offset-field encoding (ZD_OFF_SYM)
     uint32_t pad[3];
 };
 struct ZdParIO { uint8_t* lit_arena; uint32_t lit_cap; uint32_t* lit_bump; uint64_t* seq_arena; uint32_t seq_cap; uint32_t* seq_bump; };
 
-// Table definitions of one Compressed_Block only (Huffman tree, the three FSE tables): what a later block may inherit.
-__device__ __forceinline__ uint32_t zd_block_tables(const uint8_t* blk, uint32_t bsize, ZdWarpCtx* cx, uint32_t lane) {
-    const uint32_t limit = zf::BLOCK_MAX, litcap = zf::BLOCK_MAX;
-    const bool fast_nonfirst = false;
-#include "zd_blk_lit_header.inc"
-    if (ltype == 2) zd_fill_huf_warp(cx, lane);
+// Only the Huffman tree of a Compressed_Block with Compressed_Literals (what treeless blocks after it inherit).
+__device__ __forceinline__ bool zd_block_huf_only(const uint8_t* blk, uint32_t bsize, ZdWarpCtx* cx, uint32_t lane, ZdLitSec& L) {
+    if (!zd_stage_lit_header(blk, bsize, zf::BLOCK_MAX, cx, lane, L)) return false;
+    if (L.type == 2) zd_fill_huf_warp(cx, lane);
     __syncwarp();
-    (void)regen; (void)streams; (void)tree;
-#include "zd_blk_seq_header.inc"
-    (void)nseq; (void)bs; (void)bs_size;
-    return 0;
+    return true;
 }
 
-// Only the Huffman tree of a Compressed_Block with Compressed_Literals (what treeless blocks after it inherit).
-__device__ __forceinline__ uint32_t zd_block_huf_only(const uint8_t* blk, uint32_t bsize, ZdWarpCtx* cx, uint32_t lane) {
-    const uint32_t limit = zf::BLOCK_MAX, litcap = zf::BLOCK_MAX;
-    const bool fast_nonfirst = false;
-#include "zd_blk_lit_header.inc"
-    if (ltype == 2) zd_fill_huf_warp(cx, lane);
-    __syncwarp();
-    (void)lhs; (void)regen; (void)lcomp; (void)streams; (void)tree;
-    return 0;
+// Table definitions of one Compressed_Block only (Huffman tree, the three FSE tables): what a later block may inherit.
+__device__ __forceinline__ void zd_block_tables(const uint8_t* blk, uint32_t bsize, ZdWarpCtx* cx, uint32_t lane) {
+    ZdLitSec L;
+    ZdSeqSec S;
+    if (zd_block_huf_only(blk, bsize, cx, lane, L)) zd_stage_seq_header(blk, bsize, L, cx, lane, S);
 }
 
 // What a Compressed_Block inherits and what it defines.  Lane 0 parses, the warp gets the answer as a mask:
@@ -537,27 +854,14 @@ __device__ __forceinline__ uint32_t zd_block_inherits(const uint8_t* blk, uint32
     uint32_t r = 3;
     if (lane == 0) {
         do {
-            if (bsize < 2) break;
-            const uint32_t b0 = blk[0], type = b0 & 3, sf = (b0 >> 2) & 3;
-            uint32_t hs, regen, comp;
-            if (type < 2) {
-                if ((sf & 1) == 0) { hs = 1; regen = b0 >> 3; }
-                else if (sf == 1) { hs = 2; regen = (b0 >> 4) | ((uint32_t)blk[1] << 4); }
-                else { if (bsize < 3) break; hs = 3; regen = (b0 >> 4) | ((uint32_t)blk[1] << 4) | ((uint32_t)blk[2] << 12); }
-                comp = type == 0 ? regen : 1;
-            } else {
-                if (bsize < 5) break;
-                const uint32_t h = blk[0] | ((uint32_t)blk[1] << 8) | ((uint32_t)blk[2] << 16) | ((uint32_t)blk[3] << 24);
-                if (sf <= 1) { hs = 3; comp = (h >> 14) & 0x3ff; }
-                else if (sf == 2) { hs = 4; comp = h >> 18; }
-                else { hs = 5; comp = (h >> 22) | ((uint32_t)blk[4] << 10); }
-            }
-            if ((uint64_t)hs + comp + 1 > bsize) break;
-            const uint8_t* sp = blk + hs + comp;
-            const uint32_t ssize = bsize - hs - comp;
+            const ZdLitSec L = zd_lit_section(blk, bsize);
+            if (!L.hs) break;
+            if ((uint64_t)L.hs + L.comp + 1 > bsize) break;
+            const uint8_t* sp = blk + L.hs + L.comp;
+            const uint32_t ssize = bsize - L.hs - L.comp;
             uint32_t nseq = sp[0], sh = 1;
             if (nseq >= 128) { sh = nseq == 255 ? 3 : 2; if (ssize < sh) break; nseq = 1; }
-            const uint32_t huf = (type == 3 ? 1u : 0u) | (type == 2 ? 8u : 0u);
+            const uint32_t huf = (L.type == 3 ? 1u : 0u) | (L.type == 2 ? 8u : 0u);
             if (nseq == 0) { r = huf | 4u; break; }
             if (ssize < sh + 1) break;
             const uint32_t modes = sp[sh];
@@ -571,98 +875,55 @@ __device__ __forceinline__ uint32_t zd_block_inherits(const uint8_t* blk, uint32
 // packed words (see ZD_OFF_SYM) into the frame's sequence arena.  Repeat offsets are resolved HERE, per block and in
 // parallel across blocks: the three repeat offsets a block starts with are unknown to it, so they are carried as symbols
 // (initial offset k, minus d) until real offsets have pushed them out; the execution stage substitutes them.
-__device__ __forceinline__ uint32_t zd_rep_sub1(uint32_t v) {            // "rep1 - 1" on an offset field; 0 = invalid
-    if (v & ZD_OFF_SYM) return (v & 0x7ffffffu) == 0x7ffffffu ? 0u : v + 1;   // symbolic: one more subtracted
-    return v - 1;                                                        // concrete: 0 when the offset was 1 (corrupt)
-}
-__device__ __forceinline__ uint32_t zd_block_entropy(const uint8_t* blk, uint32_t bsize, ZdWarpCtx* cx, const ZdParIO& io,
-                                                     ZdBlkMeta* meta, uint32_t lane) {
-    const uint32_t limit = zf::BLOCK_MAX, litcap = zf::BLOCK_MAX;
-    const bool fast_nonfirst = false;
-#include "zd_blk_lit_header.inc"
+__device__ __forceinline__ void zd_block_entropy(const uint8_t* blk, uint32_t bsize, ZdWarpCtx* cx, const ZdParIO& io,
+                                                 ZdBlkMeta* meta, uint32_t lane) {
+    ZdLitSec L;
+    if (!zd_stage_lit_header(blk, bsize, zf::BLOCK_MAX, cx, lane, L)) return;
     uint8_t* litbuf = nullptr;
     uint32_t lit_at = 0;
-    if (ltype >= 2) {
+    if (L.type >= 2) {
         if (lane == 0) {
-            const uint32_t o = atomicAdd(io.lit_bump, (regen + 15) & ~15u);
+            const uint32_t o = atomicAdd(io.lit_bump, (L.regen + 15) & ~15u);
             cx->tmp[7] = o;
-            if ((uint64_t)o + regen + 16 > io.lit_cap) cx->err = -1;
+            if ((uint64_t)o + L.regen + 16 > io.lit_cap) cx->err = -1;
         }
         __syncwarp();
-        if (cx->err) return 0;
+        if (cx->err) return;
         lit_at = cx->tmp[7];
         litbuf = io.lit_arena + lit_at;
     }
-#include "zd_blk_lit_decode.inc"
-#include "zd_blk_seq_header.inc"
+    ZdLitSrc src;
+    ZdSeqSec S;
+    if (!zd_stage_lit_source(blk, L, cx, litbuf, lane, src) || !zd_stage_seq_header(blk, bsize, L, cx, lane, S)) return;
     if (lane == 0) {
-        const uint32_t o = atomicAdd(io.seq_bump, nseq);
+        const uint32_t o = atomicAdd(io.seq_bump, S.nseq);
         cx->tmp[7] = o;
-        if ((uint64_t)o + nseq > io.seq_cap) cx->err = -1;
-        cx->rep[0] = ZD_OFF_SYM | (1u << 27); cx->rep[1] = ZD_OFF_SYM | (2u << 27); cx->rep[2] = ZD_OFF_SYM | (3u << 27);
+        if ((uint64_t)o + S.nseq > io.seq_cap) cx->err = -1;
+        cx->rep[0] = zd_sym_rep(1); cx->rep[1] = zd_sym_rep(2); cx->rep[2] = zd_sym_rep(3);
     }
     __syncwarp();
-    if (cx->err) return 0;
+    if (cx->err) return;
     const uint32_t seq_at = cx->tmp[7];
     uint64_t* sq = io.seq_arena + seq_at;
-#include "zd_blk_seq_init.inc"
-    for (uint32_t s0 = 0; s0 < nseq; s0 += 32) {
-        const uint32_t cnt = min(32u, nseq - s0);
-#include "zd_blk_decode_batch.inc"
-        const bool wide = mine && ((ofv > 3 && ofv - 3 >= ZD_OFF_SYM) || ll >= (1u << 17) || ml - 3 >= (1u << 17));
-        if (__ballot_sync(TS_FULL, wide)) { if (lane == 0) cx->err = 2; __syncwarp(); return 0; }    // does not fit the word: serial path
-        // offset field of every sequence of the batch (concrete or symbolic), and the repeat-offset state after it
-        uint32_t of = off;                                   // ofv - 3 for real offsets
-        const uint32_t rep_mask = __ballot_sync(TS_FULL, mine && ofv <= 3);
-        if (rep_mask == 0) {
-            const uint32_t o1 = __shfl_sync(TS_FULL, of, cnt - 1), o2 = __shfl_sync(TS_FULL, of, cnt >= 2 ? cnt - 2 : 0),
-                           o3 = __shfl_sync(TS_FULL, of, cnt >= 3 ? cnt - 3 : 0);
-            if (lane == 0) {
-                const uint32_t r0 = cx->rep[0], r1 = cx->rep[1];
-                cx->rep[2] = cnt >= 3 ? o3 : cnt == 2 ? r0 : r1;
-                cx->rep[1] = cnt >= 2 ? o2 : r0;
-                cx->rep[0] = o1;
-            }
-        } else {
-            __syncwarp();
-            cx->s_off[lane] = ofv; cx->s_ml[lane] = ll;
-            __syncwarp();
-            if (lane == 0) {
-                uint32_t r0 = cx->rep[0], r1 = cx->rep[1], r2 = cx->rep[2];
-                for (uint32_t i = 0; i < cnt; i++) {
-                    const uint32_t v = cx->s_off[i];
-                    uint32_t o;
-                    if (v > 3) { o = v - 3; r2 = r1; r1 = r0; r0 = o; }
-                    else {
-                        const uint32_t idx = v - 1 + (cx->s_ml[i] == 0 ? 1 : 0);     // 0: rep1, 1: rep2, 2: rep3, 3: rep1 - 1
-                        if (idx == 0) o = r0;
-                        else {
-                            const uint32_t t = idx == 1 ? r1 : idx == 2 ? r2 : zd_rep_sub1(r0);
-                            if (t == 0) { cx->err = -1; break; }
-                            if (idx != 1) r2 = r1;
-                            r1 = r0; r0 = t; o = t;
-                        }
-                    }
-                    cx->s_off[i] = o;
-                }
-                cx->rep[0] = r0; cx->rep[1] = r1; cx->rep[2] = r2;
-            }
-            __syncwarp();
-            if (cx->err) return 0;
-            of = mine ? cx->s_off[lane] : 1;
-        }
-        if (mine) sq[s0 + lane] = (uint64_t)of | ((uint64_t)ll << 30) | ((uint64_t)(ml - 3) << 47);
+    ZdSeqCursor c;
+    if (!zd_stage_seq_init(S, cx, lane, c)) return;
+    for (uint32_t s0 = 0; s0 < S.nseq; s0 += 32) {
+        const uint32_t cnt = min(32u, S.nseq - s0);
+        ZdSeq q;
+        if (!zd_decode_batch(S, s0, cnt, cx, c, lane, q)) return;
+        const bool wide = q.mine && !zd_seq_fits(q.ofv, q.ll, q.ml);
+        if (__ballot_sync(TS_FULL, wide)) { if (lane == 0) cx->err = 2; __syncwarp(); return; }    // does not fit the word: serial path
+        if (!zd_resolve_reps<true>(q, cnt, cx, lane)) return;
+        if (q.mine) sq[s0 + lane] = zd_seq_pack(q.off, q.ll, q.ml);
         __syncwarp();
     }
-    (void)op; (void)lp; (void)lit;
     if (lane == 0) {
-        meta->lit_kind = ltype == 0 ? 1u : ltype == 1 ? 2u : 0u;
-        meta->lit_off = ltype == 0 ? lhs : ltype == 1 ? rle_lit : lit_at;
-        meta->regen = regen; meta->nseq = nseq; meta->seq_off = seq_at;
-        if (nseq) { meta->rep[0] = cx->rep[0]; meta->rep[1] = cx->rep[1]; meta->rep[2] = cx->rep[2]; }
-        else { meta->rep[0] = ZD_OFF_SYM | (1u << 27); meta->rep[1] = ZD_OFF_SYM | (2u << 27); meta->rep[2] = ZD_OFF_SYM | (3u << 27); }
+        meta->lit_kind = L.type == 0 ? 1u : L.type == 1 ? 2u : 0u;
+        meta->lit_off = L.type == 0 ? L.hs : L.type == 1 ? src.rle_lit : lit_at;
+        meta->regen = L.regen; meta->nseq = S.nseq; meta->seq_off = seq_at;
+        if (S.nseq) { meta->rep[0] = cx->rep[0]; meta->rep[1] = cx->rep[1]; meta->rep[2] = cx->rep[2]; }
+        else { meta->rep[0] = zd_sym_rep(1); meta->rep[1] = zd_sym_rep(2); meta->rep[2] = zd_sym_rep(3); }
     }
-    return 0;
 }
 
 // ------------------------------------------------------------------------------------------ execution stage, one CTA
@@ -792,8 +1053,8 @@ __device__ __forceinline__ uint32_t zx_execute_blocks(const uint8_t* frame, cons
     zx_barrier<T>();
     for (uint32_t b = b_first; b < b_last; b++) {
         const uint32_t pos = bo[b];
-        const uint32_t h = frame[pos] | (frame[pos + 1] << 8) | ((uint32_t)frame[pos + 2] << 16);
-        const uint32_t type = (h >> 1) & 3, bsz = h >> 3;
+        const ZdBlkHdr bh = zd_block_header(frame + pos);
+        const uint32_t type = bh.type, bsz = bh.size;
         if (per_block) win_pos0 = op;
         const uint32_t room = min(min((uint32_t)zf::BLOCK_MAX, out_cap - op), win_cap - (op - win_pos0));
         uint8_t* wout = win - win_pos0;                  // wout[position] for positions inside the window
@@ -827,12 +1088,11 @@ __device__ __forceinline__ uint32_t zx_execute_blocks(const uint8_t* frame, cons
             uint32_t ll = 0, ml = 0, off = 1;
             bool bad = false;
             if (mine) {
-                const uint64_t v = sq[i];
-                const uint32_t of = (uint32_t)v & 0x3fffffffu;
-                ll = (uint32_t)(v >> 30) & 0x1ffffu; ml = (uint32_t)(v >> 47) + 3;
+                uint32_t of;
+                zd_seq_unpack(sq[i], of, ll, ml);
                 if (of & ZD_OFF_SYM) {
-                    const uint32_t k = (of >> 27) & 3, d = of & 0x7ffffffu;
-                    const uint32_t r = k == 1 ? R0 : k == 2 ? R1 : R2;
+                    uint32_t d;
+                    const uint32_t r = zd_sym_base(of, R0, R1, R2, &d);
                     if (r <= d || no_carried_reps) bad = true; else off = r - d;      // a region cannot know what earlier regions left behind
                 } else off = of;
                 if (off == 0) bad = true;
@@ -1073,9 +1333,9 @@ __device__ __forceinline__ uint32_t zx_execute_blocks(const uint8_t* frame, cons
             for (int k = 0; k < 3; k++) {                                 // an offset that underflowed is only an error if it is used
                 const uint32_t of = m.rep[k];
                 if (of & ZD_OFF_SYM) {
-                    const uint32_t q = (of >> 27) & 3, dd = of & 0x7ffffffu;
-                    const uint32_t r = q == 1 ? R0 : q == 2 ? R1 : R2;
-                    nr[k] = r > dd ? r - dd : 0;
+                    uint32_t d;
+                    const uint32_t r = zd_sym_base(of, R0, R1, R2, &d);
+                    nr[k] = r > d ? r - d : 0;
                 } else nr[k] = of;
             }
             sh->rep[0] = nr[0]; sh->rep[1] = nr[1]; sh->rep[2] = nr[2];
@@ -1161,9 +1421,9 @@ __global__ void __launch_bounds__(128) zstd_dec_index_kernel(const __grid_consta
     bool ok = true, last = false;
     while (!last) {
         if (pos + 3 > n) { ok = false; break; }
-        const uint32_t h = p[pos] | (p[pos + 1] << 8) | ((uint32_t)p[pos + 2] << 16);
-        last = h & 1;
-        const uint32_t type = (h >> 1) & 3, bsz = h >> 3;
+        const ZdBlkHdr bh = zd_block_header(p + pos);
+        last = bh.last;
+        const uint32_t type = bh.type, bsz = bh.size;
         if (type == 3) { ok = false; break; }
         if (nblk < A.blocks_per_chunk) bo[nblk] = pos;
         nblk++;
@@ -1185,8 +1445,8 @@ __global__ void __launch_bounds__(128) zstd_dec_index_kernel(const __grid_consta
         uint32_t indep = 1;
         if (nblk >= 2) {
             const uint32_t p1 = bo[1];
-            const uint32_t h1 = p[p1] | (p[p1 + 1] << 8) | ((uint32_t)p[p1 + 2] << 16);
-            if (((h1 >> 1) & 3) == 2 && (h1 >> 3) >= 2) {
+            const ZdBlkHdr h1 = zd_block_header(p + p1);
+            if (h1.type == 2 && h1.size >= 2) {
                 const uint32_t t1 = p[p1 + 3] & 3;
                 if (t1 == 3) indep = 0;                                           // Treeless literals
                 // (Repeat_Mode tables behind Raw / RLE literals are found by the entropy stage itself)
@@ -1233,9 +1493,9 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_frames_kernel(const __gr
     bool last = false, bad = false;
     while (!last && !bad) {
         if (pos + 3 > n) { bad = true; break; }
-        const uint32_t h = p[pos] | (p[pos + 1] << 8) | ((uint32_t)p[pos + 2] << 16);
-        last = h & 1;
-        const uint32_t type = (h >> 1) & 3, bsz = h >> 3;
+        const ZdBlkHdr bh = zd_block_header(p + pos);
+        last = bh.last;
+        const uint32_t type = bh.type, bsz = bh.size;
         const uint32_t room = (uint32_t)min((uint64_t)zf::BLOCK_MAX, (uint64_t)fcs - op);
         if (type == 0) {
             if (bsz > room || pos + 3 + bsz > n) { bad = true; break; }
@@ -1248,7 +1508,7 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_frames_kernel(const __gr
             op += bsz; pos += 4;
         } else if (type == 2) {
             if (pos + 3 + bsz > n || bsz > zf::BLOCK_MAX) { bad = true; break; }
-            const uint32_t made = zd_compressed_block(p + pos + 3, bsz, dst + op, op, room, cx, litbuf, zf::BLOCK_MAX, false, lane);
+            const uint32_t made = zd_compressed_block(p + pos + 3, bsz, dst + op, op, room, cx, litbuf, lane);
             if (cx->err) { bad = true; break; }
             op += made; pos += 3 + bsz;
         } else { bad = true; break; }
@@ -1274,8 +1534,8 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_frames_kernel(const __gr
 // everything from the first block of their 64 KiB region.
 __device__ __forceinline__ bool zd_blk_hdr(const uint8_t* p, const uint32_t* bo, uint32_t j, uint32_t* pos, uint32_t* type, uint32_t* bsz) {
     const uint32_t pj = bo[j];
-    const uint32_t hj = p[pj] | (p[pj + 1] << 8) | ((uint32_t)p[pj + 2] << 16);
-    *pos = pj; *type = (hj >> 1) & 3; *bsz = hj >> 3;
+    const ZdBlkHdr h = zd_block_header(p + pj);
+    *pos = pj; *type = h.type; *bsz = h.size;
     return *type == 2 && *bsz <= zf::BLOCK_MAX;
 }
 
@@ -1299,6 +1559,7 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_par_entropy_kernel(const
     __syncwarp();
     const uint32_t inherits = zd_block_inherits(p + pos + 3, bsz, lane);
     if (inherits & 3) {
+        ZdLitSec L;                                                       // (what the tree loads parse; not needed here)
         // j0: where the replay of FSE definitions has to start (none needed: j0 = b)
         uint32_t j0 = b;
         bool tree_in_replay = false;
@@ -1321,7 +1582,7 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_par_entropy_kernel(const
                 uint32_t pj, tj, bj;
                 if (!zd_blk_hdr(p, bo, j, &pj, &tj, &bj) || bj < 1 || (p[pj + 3] & 3) != 2) continue;
                 found = true;
-                zd_block_huf_only(p + pj + 3, bj, cx, lane);
+                zd_block_huf_only(p + pj + 3, bj, cx, lane, L);
                 __syncwarp();
             }
             // not found: fine as long as nothing treeless shows up before a tree (the decode reports it otherwise)
@@ -1331,7 +1592,7 @@ __global__ void __launch_bounds__(ZD_WPB * 32) zstd_dec_par_entropy_kernel(const
             if (!zd_blk_hdr(p, bo, j, &pj, &tj, &bj)) continue;
             if ((inherits & 2) || (p[pj + 3] & 3) == 2) {                 // FSE replay, or at least the trees on the way
                 if (inherits & 2) zd_block_tables(p + pj + 3, bj, cx, lane);
-                else zd_block_huf_only(p + pj + 3, bj, cx, lane);
+                else zd_block_huf_only(p + pj + 3, bj, cx, lane, L);
             }
             __syncwarp();
         }
@@ -1533,29 +1794,6 @@ __device__ __forceinline__ bool zd_huf_stream_staged(const uint16_t* __restrict_
     return b.bits == 0;
 }
 
-// Sizes of the literals section only (no tree): where the sequences section starts.
-__device__ __forceinline__ bool zd_lit_section_size(const uint8_t* blk, uint32_t bsize, uint32_t* total) {
-    if (bsize < 2) return false;
-    const uint32_t b0 = blk[0], type = b0 & 3, sf = (b0 >> 2) & 3;
-    uint32_t hs, comp;
-    if (type < 2) {
-        uint32_t regen;
-        if ((sf & 1) == 0) { hs = 1; regen = b0 >> 3; }
-        else if (sf == 1) { hs = 2; regen = (b0 >> 4) | ((uint32_t)blk[1] << 4); }
-        else { if (bsize < 3) return false; hs = 3; regen = (b0 >> 4) | ((uint32_t)blk[1] << 4) | ((uint32_t)blk[2] << 12); }
-        comp = type == 0 ? regen : 1;
-    } else {
-        if (bsize < 5) return false;
-        const uint32_t h = blk[0] | ((uint32_t)blk[1] << 8) | ((uint32_t)blk[2] << 16) | ((uint32_t)blk[3] << 24);
-        if (sf <= 1) { hs = 3; comp = (h >> 14) & 0x3ff; }
-        else if (sf == 2) { hs = 4; comp = h >> 18; }
-        else { hs = 5; comp = (h >> 22) | ((uint32_t)blk[4] << 10); }
-    }
-    if ((uint64_t)hs + comp > bsize) return false;
-    *total = hs + comp;
-    return true;
-}
-
 // Common prologue: which block this group of four lanes owns.  live: a Compressed_Block to decode; refuse: malformed framing.
 struct ZdiBlock { uint32_t b, blk_off, bsize; bool live; uint32_t refuse; };
 __device__ __forceinline__ ZdiBlock zdi_block(const ZstdDecArgs& A, uint32_t chunk, uint32_t nblk, uint32_t g) {
@@ -1597,15 +1835,15 @@ __global__ void __launch_bounds__(32) zstd_dec_blk_literals_kernel(const __grid_
     uint32_t refuse = B.refuse;
 
     // header + tree description (leaders), table fill (warp), streams (4 lanes per block)
-    uint32_t ltype = 0, lhs = 0, regen = 0, lcomp = 0, streams = 1, tree = 0;
+    ZdLitSec L{0, 0, 0, 0, 1, 0};
     if (live && sub == 0) {
         cx->err = 0; cx->huf_valid = 0;
-        uint32_t h[6];
+        ZdLitSec h;
         if (!zd_parse_lit_header(blk, B.bsize, ZB, ZB, true, cx, h) || cx->err) refuse = 1;
-        else { ltype = h[0]; lhs = h[1]; regen = h[2]; lcomp = h[3]; streams = h[4]; tree = h[5]; }
+        else L = h;
     }
-    ltype = __shfl_sync(TS_FULL, ltype, lead); lhs = __shfl_sync(TS_FULL, lhs, lead); regen = __shfl_sync(TS_FULL, regen, lead);
-    lcomp = __shfl_sync(TS_FULL, lcomp, lead); streams = __shfl_sync(TS_FULL, streams, lead); tree = __shfl_sync(TS_FULL, tree, lead);
+    const uint32_t ltype = __shfl_sync(TS_FULL, L.type, lead), lhs = __shfl_sync(TS_FULL, L.hs, lead), regen = __shfl_sync(TS_FULL, L.regen, lead);
+    const uint32_t lcomp = __shfl_sync(TS_FULL, L.comp, lead), streams = __shfl_sync(TS_FULL, L.streams, lead), tree = __shfl_sync(TS_FULL, L.tree, lead);
     refuse = __shfl_sync(TS_FULL, refuse, lead);
     live = live && !refuse;
     for (uint32_t gg = 0; gg < ZDI_G; gg++) {
@@ -1618,20 +1856,10 @@ __global__ void __launch_bounds__(32) zstd_dec_blk_literals_kernel(const __grid_
         bool ok = true;
         if (streams == 1) {
             if (sub == 0) ok = zd_huf_stream_staged(cx->huf, cx->huf_log, hsrc, hsize, litbuf, regen, stg, base, lim);
-        } else if (hsize < 10) ok = false;
-        else {
-            const uint32_t s1 = hsrc[0] | (hsrc[1] << 8), s2 = hsrc[2] | (hsrc[3] << 8), s3 = hsrc[4] | (hsrc[5] << 8);
-            if (6 + s1 + s2 + s3 > hsize) ok = false;
-            else {
-                const uint32_t s4 = hsize - 6 - s1 - s2 - s3;
-                const uint32_t per = (regen + 3) / 4;
-                const uint32_t o = sub == 0 ? 0 : sub == 1 ? s1 : sub == 2 ? s1 + s2 : s1 + s2 + s3;
-                const uint32_t sz = sub == 0 ? s1 : sub == 1 ? s2 : sub == 2 ? s3 : s4;
-                const uint32_t first = sub * per;
-                if (first > regen || (sub == 3 && 3 * per > regen)) ok = false;
-                else ok = zd_huf_stream_staged(cx->huf, cx->huf_log, hsrc + 6 + o, sz, litbuf + first,
-                                               sub < 3 ? min(per, regen - first) : regen - first, stg, base, lim);
-            }
+        } else {
+            ZdHufStream s;
+            ok = zd_huf4_stream(hsrc, hsize, regen, sub, s) &&
+                 zd_huf_stream_staged(cx->huf, cx->huf_log, hsrc + s.off, s.size, litbuf + s.first, s.count, stg, base, lim);
         }
         if (!ok) refuse = 1;
     }
@@ -1676,9 +1904,13 @@ __global__ void __launch_bounds__(32) zstd_dec_blk_sequences_kernel(const __grid
     if (live && sub == 0) {
         cx->err = 0; cx->ll_valid = 0; cx->ml_valid = 0; cx->of_valid = 0;
         uint32_t h[3];
-        if (!zd_lit_section_size(blk, B.bsize, &lsec)) refuse = 1;
-        else if (!zd_parse_seq_header(blk + lsec, B.bsize - lsec, true, cx, h) || cx->err || h[0] > ZDI_SEQ_SLOT) refuse = 1;
-        else { nseq = h[0]; bs_off = h[1]; pend = h[2]; }
+        const ZdLitSec L = zd_lit_section(blk, B.bsize);
+        if (!L.hs || (uint64_t)L.hs + L.comp > B.bsize) refuse = 1;
+        else {
+            lsec = L.hs + L.comp;                                         // where the sequences section starts
+            if (!zd_parse_seq_header(blk + lsec, B.bsize - lsec, true, cx, h) || cx->err || h[0] > ZDI_SEQ_SLOT) refuse = 1;
+            else { nseq = h[0]; bs_off = h[1]; pend = h[2]; }
+        }
     }
     refuse = __shfl_sync(TS_FULL, refuse, lead);
     live = live && !refuse;
@@ -1704,7 +1936,7 @@ __global__ void __launch_bounds__(32) zstd_dec_blk_sequences_kernel(const __grid
     // ---- rounds of up to 32 sequences per block: the group stages the 128 bytes below the cursor, the leaders walk their
     // chains (a chain stops early when it would leave the staged bytes), then the warp cuts the values out, block after block
     uint32_t s0 = 0;
-    uint32_t r0 = ZD_OFF_SYM | (1u << 27), r1 = ZD_OFF_SYM | (2u << 27), r2 = ZD_OFF_SYM | (3u << 27);   // repeat offsets after the block
+    uint32_t r0 = zd_sym_rep(1), r1 = zd_sym_rep(2), r2 = zd_sym_rep(3);   // repeat offsets after the block
     while (true) {
         const bool more = live && !refuse && sub == 0 && s0 < nseq;
         const uint32_t more_mask = __ballot_sync(TS_FULL, more);
@@ -1782,18 +2014,12 @@ __global__ void __launch_bounds__(32) zstd_dec_blk_sequences_kernel(const __grid
                 ll = g_seq_tables.ll_base[el.sym] + (v & ((1u << el.nb_extra) - 1));
             }
             // a repeat-offset code, or a field the sequence word cannot hold: not a block of this kind
-            const bool odd = mine && (ofv <= 3 || ofv - 3 >= ZD_OFF_SYM || ll >= (1u << 17) || ml - 3 >= (1u << 17));
+            const bool odd = mine && (ofv <= 3 || !zd_seq_fits(ofv, ll, ml));
             const uint32_t any_odd = __ballot_sync(TS_FULL, odd);
             const uint32_t of = ofv - 3;
-            if (mine && !any_odd) sq_base[(size_t)gg * ZDI_SEQ_SLOT + sbase + lane] = (uint64_t)of | ((uint64_t)ll << 30) | ((uint64_t)(ml - 3) << 47);
-            const uint32_t o1 = __shfl_sync(TS_FULL, of, c - 1), o2 = __shfl_sync(TS_FULL, of, c >= 2 ? c - 2 : 0), o3 = __shfl_sync(TS_FULL, of, c >= 3 ? c - 3 : 0);
-            if (g == gg) {
-                if (any_odd) refuse = 1;
-                const uint32_t q0 = r0, q1 = r1;
-                r2 = c >= 3 ? o3 : c == 2 ? q0 : q1;
-                r1 = c >= 2 ? o2 : q0;
-                r0 = o1;
-            }
+            if (mine && !any_odd) sq_base[(size_t)gg * ZDI_SEQ_SLOT + sbase + lane] = zd_seq_pack(of, ll, ml);
+            if (g == gg && any_odd) refuse = 1;
+            zd_shift_in(of, c, g == gg, r0, r1, r2);
         }
         s0 += cnt;
         __syncwarp();                                    // stage / s_ll / s_ml are rewritten by the next round
