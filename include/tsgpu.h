@@ -159,6 +159,38 @@ int tsgpu_transform_cursor(tsgpu_ctx* ctx, uint32_t flags,
                            uint32_t* transformed_sizes, uint32_t* n_chunks,
                            tsgpu_records_cursor* cursor, int segment_ends_here);
 
+/* tsgpu_transform_cursor plus the CRC-32C of the object's upload parts, computed on the GPU from the bytes it copies to dst.
+ * The object is what dst receives, call after call, for one segment (the transformed chunks back to back: the .log object);
+ * part k is its bytes [k * part_size, min((k + 1) * part_size, object length)), as a multipart upload cuts it.  CRC-32C is the
+ * Castagnoli CRC (reflected polynomial 0x82F63B78, init and xorout 0xFFFFFFFF; crc32c("123456789") = 0xE3069283): what S3
+ * UploadPart takes as x-amz-checksum-crc32c and GCS as the object's crc32c (wiring: INTEGRATION.md).  It covers the bytes as
+ * they were in HBM when the library copied them out, so a part damaged on any later hop -- pinned buffer, JVM copies, the
+ * storage client's part buffer -- is refused by the object store while the local segment still exists.
+ *
+ *   part_size      >= 1 and the same for every call of a segment (TSGPU_E_ARG otherwise); no minimum is imposed
+ *   parts          32-byte cursor, zeroed at the start of the object; carries the open part and the object CRC between calls
+ *   part_crc32c    receives, in part order, the CRC of every part whose last byte this call produced; *n_parts is their count
+ *   part_cap       capacity of part_crc32c.  It must be at least
+ *                    floor((carried + tsgpu_transform_bound(flags, src_len, chunk_size)) / part_size) + (segment_ends_here ? 1 : 0)
+ *                  where carried is the open part's length (object bytes so far mod part_size; 0 for a new object, and the
+ *                  bound is 0 when src_len is 0); a smaller part_cap is refused with TSGPU_E_SHORT before any GPU work
+ *   object_crc32c  with segment_ends_here: the open part is emitted too and *object_crc32c is the CRC-32C of the whole object
+ *                  (S3's FULL_OBJECT checksum, GCS's object crc32c).  An empty object has no part and CRC 0.  Without
+ *                  segment_ends_here it is not written.
+ * flags must include ZSTD or AES (TSGPU_E_ARG: with flags 0 no byte reaches the GPU); the call combines with ZSTD_DENSE,
+ * ZSTD_CHECKSUM, VERIFY and VALIDATE_RECORDS, and `records` may be NULL without VALIDATE_RECORDS.  dst, transformed_sizes and
+ * every error are those of tsgpu_transform_cursor with the same arguments.  A failed call writes no part CRC and no object CRC --
+ * not even those of batches before a batch that failed VERIFY or VALIDATE_RECORDS, whose bytes may already be in dst -- and leaves
+ * both cursors without a defined value: the caller discards the object, as with any error.  Cost and memory: DESIGN.md §3, §8. */
+typedef struct tsgpu_parts_cursor { uint64_t opaque[4]; } tsgpu_parts_cursor;
+int tsgpu_transform_parts(tsgpu_ctx* ctx, uint32_t flags,
+                          const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
+                          const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                          uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                          tsgpu_records_cursor* records, int segment_ends_here,
+                          uint64_t part_size, tsgpu_parts_cursor* parts,
+                          uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts, uint32_t* object_crc32c);
+
 /* Ragged variant of tsgpu_transform: chunk i is the next chunk_lens[i] bytes of src (no fixed chunk size).
  * Replaces the per-index chains of RemoteStorageManager.transformIndex (RemoteStorageManager.java:455-490; each Kafka
  * index file is ONE chunk, chunking disabled, encryption only) so the five index blobs of a segment go through one batch. */

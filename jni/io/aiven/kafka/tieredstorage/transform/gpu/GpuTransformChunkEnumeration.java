@@ -25,6 +25,10 @@ import io.aiven.kafka.tieredstorage.transform.TransformChunkEnumeration;
  * <p>One enumeration is one segment, so it keeps one {@link RecordsCursor} across its windows and marks the last (short
  * or empty) window: with record validation on (the validateRecords argument, or TSGPU_VALIDATE_RECORDS=1 in the
  * environment) a record batch that crosses a window is checked whole, and a segment that ends inside a batch fails.
+ *
+ * <p>With a partSize, every window also goes through tsgpu_transform_parts, which hashes the bytes it copies out on the GPU:
+ * {@link #partCrc32c(int)} and {@link #objectCrc32c()} then give the CRC-32C of each upload part of the object and of the whole
+ * object, for the storage backend to send with the parts (INTEGRATION.md).
  */
 public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, AutoCloseable {
     private final long ctx;
@@ -35,6 +39,7 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
     private final DataKeyAndAAD keyAndAad;   // null when encryption is off
     private final int batchChunks;
     private final RecordsCursor records = new RecordsCursor();
+    private final PartsCursor parts;                  // null without part checksums
     private final SecureRandom random = new SecureRandom();
     private final ArrayDeque<byte[]> ready = new ArrayDeque<>();
     private final PinnedPool pool;
@@ -48,11 +53,20 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
         this(ctx, pool, inputStream, originalChunkSize, compression, keyAndAad, batchChunks, false);
     }
 
-    /** validateRecords: check every record batch of the segment on the GPU (TsGpu.FLAG_VALIDATE_RECORDS); it applies when the
-     *  segment is compressed or encrypted, otherwise the bytes are copied on the host and never reach the GPU. */
     public GpuTransformChunkEnumeration(final long ctx, final PinnedPool pool, final InputStream inputStream,
                                         final int originalChunkSize, final boolean compression,
                                         final DataKeyAndAAD keyAndAad, final int batchChunks, final boolean validateRecords) {
+        this(ctx, pool, inputStream, originalChunkSize, compression, keyAndAad, batchChunks, validateRecords, 0);
+    }
+
+    /** validateRecords: check every record batch of the segment on the GPU (TsGpu.FLAG_VALIDATE_RECORDS); it applies when the
+     *  segment is compressed or encrypted, otherwise the bytes are copied on the host and never reach the GPU.
+     *  partSize: the storage backend's multipart part size; above 0 the CRC-32C of every part is computed on the GPU
+     *  ({@link #partCrc32c(int)}), which needs compression or encryption for the same reason.  0 turns it off. */
+    public GpuTransformChunkEnumeration(final long ctx, final PinnedPool pool, final InputStream inputStream,
+                                        final int originalChunkSize, final boolean compression,
+                                        final DataKeyAndAAD keyAndAad, final int batchChunks, final boolean validateRecords,
+                                        final long partSize) {
         if (inputStream == null) {
             throw new NullPointerException("inputStream cannot be null");
         }
@@ -67,6 +81,10 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
         this.originalChunkSize = originalChunkSize;
         final int transforms = (compression ? TsGpu.FLAG_ZSTD : 0) | (keyAndAad != null ? TsGpu.FLAG_AES : 0);
         this.flags = transforms | (validateRecords && transforms != 0 ? TsGpu.FLAG_VALIDATE_RECORDS : 0);
+        if (partSize < 0 || (partSize > 0 && transforms == 0)) {
+            throw new IllegalArgumentException("partSize must be 0, or positive with compression or encryption; " + partSize + " given");
+        }
+        this.parts = partSize > 0 ? new PartsCursor(partSize) : null;
         this.keyAndAad = keyAndAad;
         this.batchChunks = batchChunks;
         if (originalChunkSize > 0) {
@@ -88,6 +106,22 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             return null;
         }
         return (flags & TsGpu.FLAG_AES) != 0 ? originalChunkSize + 28 : originalChunkSize;
+    }
+
+    /** The CRC-32C of upload part partNumber (1-based), valid once the window that ends that part has been transformed. */
+    public int partCrc32c(final int partNumber) {
+        if (parts == null) {
+            throw new IllegalStateException("part checksums were not requested (partSize 0)");
+        }
+        return parts.partCrc32c(partNumber);
+    }
+
+    /** The CRC-32C of the whole object (S3 FULL_OBJECT, GCS crc32c), valid after the last window. */
+    public int objectCrc32c() {
+        if (parts == null) {
+            throw new IllegalStateException("part checksums were not requested (partSize 0)");
+        }
+        return parts.objectCrc32c();
     }
 
     @Override
@@ -125,9 +159,12 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             }
             final long total = in.position();
             if (total == 0) {                            // the segment ended with the previous, full window
-                records.transform(ctx, flags, in, 0, originalChunkSize,
+                if (parts == null) records.transform(ctx, flags, in, 0, originalChunkSize,
                     keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
                     new byte[TsGpu.IV_SIZE], dst.buffer(), new int[0], true);
+                else parts.transform(ctx, flags, in, 0, originalChunkSize,       // ... which also ends the last part
+                    keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                    new byte[TsGpu.IV_SIZE], dst.buffer(), new int[0], records, true);
                 release();
                 return;
             }
@@ -139,9 +176,13 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             random.nextBytes(ivs);
             final int[] sizes = new int[chunks];
             final ByteBuffer out = dst.buffer();
-            final int n = records.transform(ctx, flags, in, total, originalChunkSize,
-                keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
-                ivs, out, sizes, eof);
+            final int n = parts != null                 // with part checksums the window also hashes what it copies out
+                ? parts.transform(ctx, flags, in, total, originalChunkSize,
+                    keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                    ivs, out, sizes, records, eof)
+                : records.transform(ctx, flags, in, total, originalChunkSize,
+                    keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                    ivs, out, sizes, eof);
             out.clear();
             for (int i = 0; i < n; i++) {
                 final byte[] chunk = new byte[sizes[i]];
@@ -167,6 +208,11 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
         try {
             final byte[] all = inputStream.readAllBytes();
             if (all.length == 0) {
+                if (parts != null) {                     // an empty object: no part, CRC 0
+                    parts.transform(ctx, flags, ByteBuffer.allocateDirect(1), 0, 0,
+                        keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                        new byte[TsGpu.IV_SIZE], ByteBuffer.allocateDirect(1), new int[0], records, true);
+                }
                 return;
             }
             src = pool.lease(all.length);
@@ -178,9 +224,13 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             random.nextBytes(ivs);
             final int[] sizes = new int[1];
             final ByteBuffer out = dst.buffer();
-            final int n = records.transform(ctx, flags, in, all.length, 0,
-                keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
-                ivs, out, sizes, true);
+            final int n = parts != null
+                ? parts.transform(ctx, flags, in, all.length, 0,
+                    keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                    ivs, out, sizes, records, true)
+                : records.transform(ctx, flags, in, all.length, 0,
+                    keyAndAad == null ? null : keyAndAad.dataKey.getEncoded(), keyAndAad == null ? null : keyAndAad.aad,
+                    ivs, out, sizes, true);
             out.clear();
             for (int i = 0; i < n; i++) {
                 final byte[] chunk = new byte[sizes[i]];

@@ -20,6 +20,11 @@ public final class RecordsCursor {
         return transformCursor(ctx, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, state, segmentEndsHere);
     }
 
+    /** The cursor's direct buffer, for PartsCursor.transformParts, which continues the same segment. */
+    ByteBuffer buffer() {
+        return state;
+    }
+
     static {
         System.loadLibrary("tsgpu_jni");
     }

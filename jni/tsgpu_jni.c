@@ -3,7 +3,7 @@
  * There is no JDK in this repository's build image: the tests compile this file against a test-only stand-in for
  * <jni.h> and drive it through a fake JNIEnv (tests/cpp/test_jni_shim.c).  Build on the broker host with
  *   gcc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude jni/tsgpu_jni.c -L<pkg> -ltsgpu -o libtsgpu_jni.so
- * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
+ * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
  * (implement TransformChunkEnumeration / DetransformChunkEnumeration of the reference, core/M/transform/TransformChunkEnumeration.java:28-42,
  * DetransformChunkEnumeration.java:28-29) and jni/io/aiven/kafka/tieredstorage/fetch/gpu/GpuChunkManager.java (ChunkManager, fetch/ChunkManager.java).
  *
@@ -60,10 +60,16 @@ JNIEXPORT jlong JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_tr
                                                                                              jlong srcLen, jint chunkSize) {
     return (jlong)tsgpu_transform_bound((uint32_t)flags, (uint64_t)srcLen, (uint32_t)chunkSize);
 }
-/* tsgpu_transform, or tsgpu_transform_cursor when `cursor` is given; returns the number of chunks, or -1 with an exception
- * pending.  transformedSizes (int[]) receives one entry per chunk. */
+/* The part-checksum arguments of tsgpu_transform_parts (PartsCursor.transformParts). */
+typedef struct {
+    uint64_t part_size; tsgpu_parts_cursor* cursor;
+    uint32_t* crcs; uint32_t cap; uint32_t n; uint32_t object_crc;
+} parts_args;
+/* tsgpu_transform, tsgpu_transform_cursor when `cursor` is given, or tsgpu_transform_parts when `parts` is; returns the number
+ * of chunks, or -1 with an exception pending.  transformedSizes (int[]) receives one entry per chunk. */
 static jint transform_call(JNIEnv* env, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
-                           jbyteArray ivs, jobject dst, jintArray transformedSizes, tsgpu_records_cursor* cursor, int segmentEndsHere) {
+                           jbyteArray ivs, jobject dst, jintArray transformedSizes, tsgpu_records_cursor* cursor, int segmentEndsHere,
+                           parts_args* parts) {
     jlong dcap = 0;
     uint8_t* s = direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer");
     if (!s) return -1;
@@ -85,7 +91,12 @@ static jint transform_call(JNIEnv* env, jlong h, jint flags, jobject src, jlong 
         return -1;
     }
     jint* sizes = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
-    int rc = cursor
+    int rc = parts
+        ? tsgpu_transform_parts((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
+                                (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n,
+                                cursor, segmentEndsHere, parts->part_size, parts->cursor, parts->crcs, parts->cap, &parts->n,
+                                &parts->object_crc)
+        : cursor
         ? tsgpu_transform_cursor((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
                                  (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n,
                                  cursor, segmentEndsHere)
@@ -101,7 +112,7 @@ static jint transform_call(JNIEnv* env, jlong h, jint flags, jobject src, jlong 
 JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_transform(
     JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
     jbyteArray ivs, jobject dst, jintArray transformedSizes) {
-    return transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, NULL, 0);
+    return transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, NULL, 0, NULL);
 }
 /* One window of a segment (RecordsCursor.transformCursor): `cursor` is a direct ByteBuffer of at least 64 bytes holding the
  * tsgpu_records_cursor (zeros at the start of the segment), updated in place; segmentEndsHere marks the segment's last window. */
@@ -112,7 +123,37 @@ JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RecordsCu
     tsgpu_records_cursor* cur = (tsgpu_records_cursor*)direct(env, cursor, 0, &ccap, "cursor must be a direct ByteBuffer of 64 bytes");
     if (!cur) return -1;
     if (ccap < (jlong)sizeof(tsgpu_records_cursor)) { throw_arg(env, "cursor must be a direct ByteBuffer of 64 bytes"); return -1; }
-    return transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, cur, segmentEndsHere ? 1 : 0);
+    return transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, cur, segmentEndsHere ? 1 : 0, NULL);
+}
+/* One window of a segment with the CRC-32C of its upload parts (PartsCursor.transformParts): `recordsCursor` as transformCursor
+ * takes it (64 bytes), `partsCursor` a direct ByteBuffer of at least 32 bytes holding the tsgpu_parts_cursor (zeros at the start
+ * of the object), both updated in place.  partCrc32c (int[]) receives the CRCs of the parts the window completed, in part order;
+ * partsOut (int[2]) receives their count and, on the segment's last window, the object's CRC-32C. */
+JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_PartsCursor_transformParts(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
+    jbyteArray ivs, jobject dst, jintArray transformedSizes, jobject recordsCursor, jboolean segmentEndsHere, jlong partSize,
+    jobject partsCursor, jintArray partCrc32c, jintArray partsOut) {
+    jlong rcap = 0, pcap = 0;
+    tsgpu_records_cursor* rcur = (tsgpu_records_cursor*)direct(env, recordsCursor, 0, &rcap, "records cursor must be a direct ByteBuffer of 64 bytes");
+    if (!rcur) return -1;
+    if (rcap < (jlong)sizeof(tsgpu_records_cursor)) { throw_arg(env, "records cursor must be a direct ByteBuffer of 64 bytes"); return -1; }
+    tsgpu_parts_cursor* pcur = (tsgpu_parts_cursor*)direct(env, partsCursor, 0, &pcap, "parts cursor must be a direct ByteBuffer of 32 bytes");
+    if (!pcur) return -1;
+    if (pcap < (jlong)sizeof(tsgpu_parts_cursor)) { throw_arg(env, "parts cursor must be a direct ByteBuffer of 32 bytes"); return -1; }
+    if (partSize < 1) { throw_arg(env, "partSize must be positive"); return -1; }
+    if (!partCrc32c || !partsOut) { throw_arg(env, "partCrc32c and partsOut cannot be null"); return -1; }
+    if ((*env)->GetArrayLength(env, partsOut) < 2) { throw_arg(env, "partsOut must hold 2 ints"); return -1; }
+    parts_args pa = {(uint64_t)partSize, pcur, NULL, (uint32_t)(*env)->GetArrayLength(env, partCrc32c), 0, 0};
+    jint* crcs = (*env)->GetIntArrayElements(env, partCrc32c, NULL);
+    pa.crcs = (uint32_t*)crcs;
+    const jint n = transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, rcur,
+                                  segmentEndsHere ? 1 : 0, &pa);
+    (*env)->ReleaseIntArrayElements(env, partCrc32c, crcs, n < 0 ? JNI_ABORT : 0);
+    if (n < 0) return -1;
+    jint* out = (*env)->GetIntArrayElements(env, partsOut, NULL);
+    out[0] = (jint)pa.n; out[1] = (jint)pa.object_crc;
+    (*env)->ReleaseIntArrayElements(env, partsOut, out, 0);
+    return n;
 }
 JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_detransform(
     JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray transformedSizes, jbyteArray key, jbyteArray aad,

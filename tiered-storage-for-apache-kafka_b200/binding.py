@@ -24,6 +24,7 @@ OK, E_ARG, E_STATE, E_AUTH, E_CORRUPT, E_SHORT, E_NODEVICE, E_CUDA, E_NOMEM = 0,
 E_VERIFY = -9
 E_RECORDS = -10
 CURSOR_SIZE = 64         # tsgpu_records_cursor
+PARTS_CURSOR_SIZE = 32   # tsgpu_parts_cursor
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",
@@ -32,7 +33,7 @@ SYMBOLS = [
     "tsgpu_chunk_sizes_encode", "tsgpu_chunk_sizes_decode", "tsgpu_transformed_chunks_serialize",
     "tsgpu_transformed_chunks_deserialize", "tsgpu_chunk_index_json", "tsgpu_profile_enable", "tsgpu_profile_report",
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
-    "tsgpu_transform_cursor",
+    "tsgpu_transform_cursor", "tsgpu_transform_parts",
 ]
 
 
@@ -69,6 +70,8 @@ def load(path=None):
     L.tsgpu_slot_stride.argtypes = [u32, u32]
     L.tsgpu_transform.argtypes = [vp, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
     L.tsgpu_transform_cursor.argtypes = [vp, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp, vp, C.c_int]
+    L.tsgpu_transform_parts.argtypes = [vp, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp, vp, C.c_int,
+                                        u64, vp, vp, u32, vp, vp]
     L.tsgpu_transform_chunks.argtypes = [vp, u32, vp, vp, u32, vp, vp, u32, vp, vp, u64, vp]
     L.tsgpu_detransform.argtypes = [vp, u32, vp, u64, vp, u32, vp, vp, u32, vp, u64, vp]
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
@@ -187,6 +190,37 @@ class Context:
                                                     cursor.ctypes.data, 1 if segment_ends_here else 0))
         sizes = sizes[:n.value]
         return dst[:int(sizes.sum(dtype=np.uint64))], [int(x) for x in sizes]
+
+    def transform_parts(self, flags, src, chunk_size, part_size, parts_cursor, segment_ends_here, records_cursor=None,
+                        key=None, aad=b"", ivs=None, part_cap=None):
+        """One window of a segment with the CRC-32C of its upload parts: `parts_cursor` is a 32-byte np.uint8 array (zeros at the
+        start of the object), updated in place on success; `records_cursor` a 64-byte one as transform_cursor takes (needed with
+        FLAG_VALIDATE_RECORDS).  Returns (transformed bytes, [transformed sizes], [CRC-32C of the parts this call completed],
+        CRC-32C of the whole object or None when the segment does not end here)."""
+        s = _u8(src)
+        for cur, size in ((parts_cursor, PARTS_CURSOR_SIZE), (records_cursor, CURSOR_SIZE)):
+            if cur is not None and not (isinstance(cur, np.ndarray) and cur.dtype == np.uint8 and cur.size == size
+                                        and cur.flags.c_contiguous):
+                raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % size)
+        cs = chunk_size if chunk_size else max(s.size, 1)
+        n_max = (s.size + cs - 1) // cs + 1
+        bound = int(self.lib.tsgpu_transform_bound(flags, s.size, chunk_size)) if s.size else 0
+        dst = np.empty(bound + 64, dtype=np.uint8)
+        sizes = np.zeros(n_max, dtype=np.uint32)
+        n = C.c_uint32(n_max)
+        if part_cap is None:
+            part_cap = (bound + part_size) // max(part_size, 1) + 1
+        crcs = np.zeros(max(part_cap, 1), dtype=np.uint32)
+        n_parts, obj = C.c_uint32(0), C.c_uint32(0)
+        k, a, iv = _u8(key), _u8(aad), _u8(ivs)
+        self._check(self.lib.tsgpu_transform_parts(
+            self._h, flags, _p(s), s.size, chunk_size, _p(k), _p(a), a.size, _p(iv), dst.ctypes.data, dst.size,
+            sizes.ctypes.data, C.addressof(n), None if records_cursor is None else records_cursor.ctypes.data,
+            1 if segment_ends_here else 0, part_size, None if parts_cursor is None else parts_cursor.ctypes.data,
+            crcs.ctypes.data, part_cap, C.addressof(n_parts), C.addressof(obj)))
+        sizes = sizes[:n.value]
+        return (dst[:int(sizes.sum(dtype=np.uint64))], [int(x) for x in sizes], [int(x) for x in crcs[:n_parts.value]],
+                int(obj.value) if segment_ends_here else None)
 
     def transform_chunks(self, flags, src, chunk_lens, key=None, aad=b"", ivs=None):
         """Ragged chunks (e.g. the index files of a segment): returns (transformed bytes, [transformed sizes])."""

@@ -1,0 +1,140 @@
+// part_crc.cuh — CRC-32C of the upload parts of a transformed object (tsgpu_transform_parts), hashed from the bytes in HBM that
+// one D2H per batch takes home (the slot's d_pack: the batch's transformed chunks back to back).
+//
+// Per batch of L packed bytes, two kernels:
+//   pcrc_tiles  (compute stream, after pack_chunks) one thread per 256-byte piece: its raw CRC-32C by slice-by-8 (eight 1 KiB
+//               tables in shared memory, 128-bit loads), and the inclusive prefix over the 128 pieces of a 32 KiB tile (GF(2)
+//               shifts by x^(8*256*2^r)).  The last CTA to finish turns the tile CRCs into exclusive prefixes over the batch.
+//   pcrc_cuts   (out_stream, at the drain, when the batch's object offset is known) one thread per part boundary inside the
+//               batch and one for its end: the raw CRC of [0, x) of the batch from a tile prefix, a piece prefix and at most 256
+//               bytes.  The host turns consecutive prefixes into the raw CRCs of the part pieces (crc32.cuh) and combines them, in
+//               batch order, into the part CRCs and the object CRC.
+#pragma once
+#include "crc32.cuh"
+
+namespace ts {
+
+constexpr uint32_t PCRC_PIECE = 256;                   // bytes per thread in pcrc_tiles
+constexpr uint32_t PCRC_T = 128;                       // threads per CTA
+constexpr uint32_t PCRC_TILE = PCRC_PIECE * PCRC_T;    // 32 KiB
+constexpr uint32_t PCRC_GRID = 264;                    // pcrc_tiles CTAs at most (they stride over the tiles)
+constexpr uint32_t PCRC_CUTS_T = 128;
+
+struct PcrcArgs {
+    const uint8_t* b;                // the batch's packed transformed bytes (256-byte aligned)
+    const uint32_t* len; uint32_t nb;   // the batch's transformed chunk sizes (device): L = their sum
+    uint32_t* pin;                   // [npieces] raw CRC of [tile start, end of piece q)
+    uint32_t* ttot;                  // [ntiles]  raw CRC of each tile, then (after the last CTA) of [0, tile start)
+    uint32_t* done;                  // CTAs of pcrc_tiles that have finished (the last one resets it to 0)
+};
+
+// Slice-by-8 tables of CRC-32C: T[k][i] is the raw CRC of byte i followed by k zero bytes.  Block-cooperative.
+__device__ __forceinline__ void pcrc_tables(uint32_t (*T)[256]) {
+    for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) T[0][i] = crc_table_entry(i, CRC32C_POLY);
+    __syncthreads();
+    for (int k = 1; k < 8; k++) {
+        for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) { const uint32_t p = T[k - 1][i]; T[k][i] = (p >> 8) ^ T[0][p & 0xffu]; }
+        __syncthreads();
+    }
+}
+__device__ __forceinline__ uint32_t pcrc_8(const uint32_t (*T)[256], uint32_t c, uint32_t lo, uint32_t hi) {   // 8 bytes, little-endian words
+    c ^= lo;
+    return T[7][c & 0xffu] ^ T[6][(c >> 8) & 0xffu] ^ T[5][(c >> 16) & 0xffu] ^ T[4][c >> 24] ^
+           T[3][hi & 0xffu] ^ T[2][(hi >> 8) & 0xffu] ^ T[1][(hi >> 16) & 0xffu] ^ T[0][hi >> 24];
+}
+// The batch's packed length, from its chunk sizes (every thread).
+__device__ __forceinline__ uint32_t pcrc_len(const PcrcArgs& A) {
+    uint32_t L = 0;
+    for (uint32_t i = 0; i < A.nb; i++) L += A.len[i];
+    return L;
+}
+
+// ---------------------------------------------------------------------------------------------------- pcrc_tiles
+__global__ void __launch_bounds__(PCRC_T) pcrc_tiles_kernel(const __grid_constant__ PcrcArgs A) {
+    __shared__ uint32_t T[8][256];
+    __shared__ uint32_t s[PCRC_T];
+    __shared__ uint32_t last;
+    pcrc_tables(T);
+    const uint32_t tid = threadIdx.x, L = pcrc_len(A);
+    const uint32_t ntiles = (L + PCRC_TILE - 1) / PCRC_TILE, npieces = (L + PCRC_PIECE - 1) / PCRC_PIECE;
+    for (uint32_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const uint32_t q = t * PCRC_T + tid;
+        const uint64_t lo64 = (uint64_t)q * PCRC_PIECE;
+        const uint32_t lo = lo64 < L ? (uint32_t)lo64 : L, hi = min(L, lo + PCRC_PIECE);
+        uint32_t c = 0;
+        if (hi - lo == PCRC_PIECE) {
+            const uint4* v = (const uint4*)(A.b + lo);
+#pragma unroll 4
+            for (uint32_t i = 0; i < PCRC_PIECE / 16; i++) {
+                const uint4 w = ldg128_stream(v + i);
+                c = pcrc_8(T, c, w.x, w.y);
+                c = pcrc_8(T, c, w.z, w.w);
+            }
+        } else {
+            c = crc_bytes(T[0], 0, A.b + lo, hi - lo);
+        }
+        // tile-local inclusive prefix: after round r a thread at tid >= 2^r holds 2^r full pieces on its right
+        s[tid] = c;
+        __syncthreads();
+        for (uint32_t r = 0, d = 1; d < PCRC_T; r++, d <<= 1) {
+            const uint32_t a = tid >= d ? s[tid - d] : 0;
+            __syncthreads();
+            if (a) c ^= crc_mult(crc_x2n(0, 11 + r), a, CRC32C_POLY);
+            s[tid] = c;
+            __syncthreads();
+        }
+        if (q < npieces) A.pin[q] = c;
+        if (tid == PCRC_T - 1) A.ttot[t] = c;
+        __syncthreads();                                   // s is reused by the next tile
+    }
+    // the last CTA to finish: exclusive prefixes of the tiles (all full but the batch's last), in place
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) last = atomicAdd(A.done, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    volatile uint32_t* tt = A.ttot;
+    const uint32_t per = (ntiles + PCRC_T - 1) / PCRC_T;
+    const uint32_t t0 = min(ntiles, tid * per), t1 = min(ntiles, t0 + per);
+    uint32_t e = 0;
+    for (uint32_t t = t0; t < t1; t++) e = crc_mult(crc_x2n(0, 18), e, CRC32C_POLY) ^ tt[t];   // this thread's tiles together
+    s[tid] = e;
+    __syncthreads();
+    for (uint32_t d = 1; d < PCRC_T; d <<= 1) {
+        const uint32_t a = tid >= d ? s[tid - d] : 0;
+        __syncthreads();
+        if (tid >= d) e ^= crc_shift(a, (uint64_t)d * per * PCRC_TILE, 0);   // the right operand covers d threads' tiles
+        s[tid] = e;
+        __syncthreads();
+    }
+    uint32_t x = tid ? s[tid - 1] : 0;                     // raw CRC of [0, first tile of this thread)
+    for (uint32_t t = t0; t < t1; t++) {
+        const uint32_t own = tt[t];
+        tt[t] = x;
+        x = crc_mult(crc_x2n(0, 18), x, CRC32C_POLY) ^ own;
+    }
+    if (tid == 0) *A.done = 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- pcrc_cuts
+// out[k] = raw CRC of [0, x_k) of the batch, x_k = first + k * step for k < m, x_m = L.
+__global__ void __launch_bounds__(PCRC_CUTS_T) pcrc_cuts_kernel(const __grid_constant__ PcrcArgs A, uint32_t L, uint32_t first,
+                                                                uint64_t step, uint32_t m, uint32_t* out) {
+    __shared__ uint32_t T[256];
+    for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) T[i] = crc_table_entry(i, CRC32C_POLY);
+    __syncthreads();
+    const uint32_t k = blockIdx.x * PCRC_CUTS_T + threadIdx.x;
+    if (k > m) return;
+    const uint32_t u = k < m ? (uint32_t)(first + k * step) : L;
+    uint32_t c = 0;
+    if (u) {
+        const uint32_t q = (u - 1) / PCRC_PIECE, t = q / PCRC_T, lq = q % PCRC_T;     // the piece holding byte u - 1
+        c = A.ttot[t];
+        if (lq) c = crc_shift(c, (uint64_t)lq * PCRC_PIECE, 0) ^ A.pin[q - 1];
+        c = crc_bytes(T, c, A.b + (uint64_t)q * PCRC_PIECE, u - q * PCRC_PIECE);
+    }
+    out[k] = c;
+}
+
+}  // namespace ts

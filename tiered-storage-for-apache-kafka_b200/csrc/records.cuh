@@ -4,7 +4,7 @@
 // A segment is a sequence of entries `offset i64 | size i32 | ...`, each 12 + size bytes, ending exactly at the segment's end:
 //   magic 2 at +16: size >= 49, CRC-32C (Castagnoli) at +17 over [+21, end)        (DefaultRecordBatch.ensureValid)
 //   magic 0/1:      size >= 14, CRC-32 (IEEE) at +12 over [+16, end)                (legacy message sets)
-// Nothing inside a batch is parsed.
+// Nothing inside a batch is parsed.  Polynomial index 0 is CRC-32C (magic 2), 1 is CRC-32 (magic 0/1); the GF(2) arithmetic is crc32.cuh.
 //
 // The work does not follow the length chain hop by hop (a dependent load per entry).  Per batch of L bytes:
 //   rec_scan    one thread per 256-byte piece: raw CRC-32C and CRC-32 of the piece (tables in shared memory, 128-bit loads),
@@ -22,7 +22,7 @@
 //               entry (header bytes, running CRC), looks the entry position up in the orbit table and leaves the verdict and
 //               the next carry.  One thread, a few hundred bytes of CRC at most outside the prefixes.
 #pragma once
-#include "ts_common.cuh"
+#include "crc32.cuh"
 
 namespace ts {
 
@@ -35,26 +35,8 @@ constexpr uint32_t REC_JUMPS = 16;                  // hops per node per rec_jum
 constexpr uint32_t REC_NONE = 0xffffffffu;
 constexpr uint32_t REC_TERM = 0x80000000u;          // node index flag: terminal
 constexpr uint32_t REC_HDR = 21;                    // header bytes up to the end of the v2 CRC field
-__device__ __forceinline__ uint32_t rec_poly(int pi) { return pi ? 0xEDB88320u : 0x82F63B78u; }   // 0: CRC-32C (magic 2), 1: CRC-32 (magic 0/1)
 
 enum RecKind : uint32_t { REC_OK = 0, REC_LENGTH = 1, REC_MAGIC = 2, REC_CRC = 3, REC_INTERNAL = 4 };
-
-// x^(2^k) mod P, k = 0..63, for the two reflected polynomials (shift of a CRC by n bytes: product over the bits of 8n)
-__constant__ uint32_t g_rec_x2n[2][64] = {
-    {0x40000000u, 0x20000000u, 0x08000000u, 0x00800000u, 0x00008000u, 0x82f63b78u, 0x6ea2d55cu, 0x18b8ea18u, 0x510ac59au, 0xb82be955u,
-     0xb8fdb1e7u, 0x88e56f72u, 0x74c360a4u, 0xe4172b16u, 0x0d65762au, 0x35d73a62u, 0x28461564u, 0xbf455269u, 0xe2ea32dcu, 0xfe7740e6u,
-     0xf946610bu, 0x3c204f8fu, 0x538586e3u, 0x59726915u, 0x734d5309u, 0xbc1ac763u, 0x7d0722ccu, 0xd289cabeu, 0xe94ca9bcu, 0x05b74f3fu,
-     0xa51e1f42u, 0x40000000u, 0x20000000u, 0x08000000u, 0x00800000u, 0x00008000u, 0x82f63b78u, 0x6ea2d55cu, 0x18b8ea18u, 0x510ac59au,
-     0xb82be955u, 0xb8fdb1e7u, 0x88e56f72u, 0x74c360a4u, 0xe4172b16u, 0x0d65762au, 0x35d73a62u, 0x28461564u, 0xbf455269u, 0xe2ea32dcu,
-     0xfe7740e6u, 0xf946610bu, 0x3c204f8fu, 0x538586e3u, 0x59726915u, 0x734d5309u, 0xbc1ac763u, 0x7d0722ccu, 0xd289cabeu, 0xe94ca9bcu,
-     0x05b74f3fu, 0xa51e1f42u, 0x40000000u, 0x20000000u},
-    {0x40000000u, 0x20000000u, 0x08000000u, 0x00800000u, 0x00008000u, 0xedb88320u, 0xb1e6b092u, 0xa06a2517u, 0xed627daeu, 0x88d14467u,
-     0xd7bbfe6au, 0xec447f11u, 0x8e7ea170u, 0x6427800eu, 0x4d47bae0u, 0x09fe548fu, 0x83852d0fu, 0x30362f1au, 0x7b5a9cc3u, 0x31fec169u,
-     0x9fec022au, 0x6c8dedc4u, 0x15d6874du, 0x5fde7a4eu, 0xbad90e37u, 0x2e4e5eefu, 0x4eaba214u, 0xa8a472c0u, 0x429a969eu, 0x148d302au,
-     0xc40ba6d0u, 0xc4e22c3cu, 0x40000000u, 0x20000000u, 0x08000000u, 0x00800000u, 0x00008000u, 0xedb88320u, 0xb1e6b092u, 0xa06a2517u,
-     0xed627daeu, 0x88d14467u, 0xd7bbfe6au, 0xec447f11u, 0x8e7ea170u, 0x6427800eu, 0x4d47bae0u, 0x09fe548fu, 0x83852d0fu, 0x30362f1au,
-     0x7b5a9cc3u, 0x31fec169u, 0x9fec022au, 0x6c8dedc4u, 0x15d6874du, 0x5fde7a4eu, 0xbad90e37u, 0x2e4e5eefu, 0x4eaba214u, 0xa8a472c0u,
-     0x429a969eu, 0x148d302au, 0xc40ba6d0u, 0xc4e22c3cu}};
 
 // The state of a segment between batches and between calls: the public tsgpu_records_cursor (64 bytes, zero = start).
 struct RecCarry {
@@ -93,37 +75,7 @@ struct RecArgs {
     uint32_t npieces, ntiles;
 };
 
-__device__ __forceinline__ uint32_t rec_mult(uint32_t a, uint32_t b, uint32_t poly) {       // a * b mod P (reflected)
-    uint32_t p = 0;
-#pragma unroll 4
-    for (int i = 0; i < 32; i++) {
-        p ^= (0u - ((a >> (31 - i)) & 1u)) & b;
-        b = (b >> 1) ^ (poly & (0u - (b & 1u)));
-    }
-    return p;
-}
-__device__ __forceinline__ uint32_t rec_xn(uint64_t bytes, int pi) {   // x^(8 * bytes) mod P
-    uint32_t p = 0x80000000u;
-    for (int k = 3; bytes; bytes >>= 1, k++)
-        if (bytes & 1) p = rec_mult(g_rec_x2n[pi][k], p, rec_poly(pi));
-    return p;
-}
-__device__ __forceinline__ uint32_t rec_shift(uint32_t crc, uint64_t bytes, int pi) { return crc ? rec_mult(rec_xn(bytes, pi), crc, rec_poly(pi)) : 0; }
 __device__ __forceinline__ uint32_t rec_be32(const uint8_t* p) { return (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | p[3]; }
-__device__ __forceinline__ uint32_t rec_upd(const uint32_t* T, uint32_t c, uint32_t byte) { return T[(c ^ byte) & 0xffu] ^ (c >> 8); }
-__device__ __forceinline__ uint32_t rec_bytes(const uint32_t* T, uint32_t c, const uint8_t* p, uint32_t n) {
-    for (uint32_t i = 0; i < n; i++) c = rec_upd(T, c, p[i]);
-    return c;
-}
-__device__ __forceinline__ void rec_tables(uint32_t (*T)[256]) {        // byte tables of both polynomials, block-cooperative
-    for (uint32_t i = threadIdx.x; i < 512; i += blockDim.x) {
-        const uint32_t pi = i >> 8, poly = rec_poly(pi);
-        uint32_t c = i & 255;
-        for (int k = 0; k < 8; k++) c = (c >> 1) ^ (poly & (0u - (c & 1u)));
-        T[pi][i & 255] = c;
-    }
-    __syncthreads();
-}
 // A plausible header at x: what a candidate is.  Needs x + REC_HDR <= L.
 __device__ __forceinline__ bool rec_plausible(const uint8_t* b, uint32_t x) {
     const uint32_t m = b[x + 16];
@@ -136,7 +88,7 @@ __device__ __forceinline__ bool rec_plausible(const uint8_t* b, uint32_t x) {
 __global__ void __launch_bounds__(REC_T) rec_scan_kernel(const __grid_constant__ RecArgs A) {
     __shared__ uint32_t T[2][256];
     __shared__ uint32_t s0[REC_T], s1[REC_T], sc[REC_T];
-    rec_tables(T);
+    crc_tables(T);
     const uint32_t tid = threadIdx.x, q = blockIdx.x * REC_T + tid;
     const uint64_t lo64 = (uint64_t)q * REC_PIECE;
     const uint32_t lo = lo64 < A.L ? (uint32_t)lo64 : A.L, hi = min(A.L, lo + REC_PIECE);
@@ -149,11 +101,11 @@ __global__ void __launch_bounds__(REC_T) rec_scan_kernel(const __grid_constant__
             for (int k = 0; k < 4; k++)
                 for (int j = 0; j < 4; j++) {
                     const uint32_t byte = (ws[k] >> (8 * j)) & 0xffu;
-                    c0 = rec_upd(T[0], c0, byte); c1 = rec_upd(T[1], c1, byte);
+                    c0 = crc_upd(T[0], c0, byte); c1 = crc_upd(T[1], c1, byte);
                 }
         }
     } else {
-        for (uint32_t x = lo; x < hi; x++) { c0 = rec_upd(T[0], c0, A.b[x]); c1 = rec_upd(T[1], c1, A.b[x]); }
+        for (uint32_t x = lo; x < hi; x++) { c0 = crc_upd(T[0], c0, A.b[x]); c1 = crc_upd(T[1], c1, A.b[x]); }
     }
     const uint32_t last = A.L >= REC_HDR ? A.L - REC_HDR : 0;       // candidates x <= last
     if (A.L >= REC_HDR) for (uint32_t x = lo; x < hi && x <= last; x++) n += rec_plausible(A.b, x) ? 1u : 0u;
@@ -165,8 +117,8 @@ __global__ void __launch_bounds__(REC_T) rec_scan_kernel(const __grid_constant__
         if (tid >= d) { a0 = s0[tid - d]; a1 = s1[tid - d]; an = sc[tid - d]; }
         __syncthreads();
         if (tid >= d) {
-            c0 ^= a0 ? rec_mult(g_rec_x2n[0][11 + r], a0, rec_poly(0)) : 0;
-            c1 ^= a1 ? rec_mult(g_rec_x2n[1][11 + r], a1, rec_poly(1)) : 0;
+            c0 ^= a0 ? crc_mult(crc_x2n(0, 11 + r), a0, crc_poly(0)) : 0;
+            c1 ^= a1 ? crc_mult(crc_x2n(1, 11 + r), a1, crc_poly(1)) : 0;
             n += an;
         }
         s0[tid] = c0; s1[tid] = c1; sc[tid] = n;
@@ -188,8 +140,8 @@ __global__ void __launch_bounds__(REC_TILES_T) rec_tiles_kernel(const __grid_con
     uint32_t e0 = 0, e1 = 0, en = 0;
     for (uint32_t t = t0; t < t1; t++) {              // thread-local exclusive prefix over its tiles (all full but the batch's last)
         A.tex[t] = e0; A.tex[nt + t] = e1; A.tbase[t] = en;
-        e0 = rec_mult(g_rec_x2n[0][18], e0, rec_poly(0)) ^ A.ttot[t];
-        e1 = rec_mult(g_rec_x2n[1][18], e1, rec_poly(1)) ^ A.ttot[nt + t];
+        e0 = crc_mult(crc_x2n(0, 18), e0, crc_poly(0)) ^ A.ttot[t];
+        e1 = crc_mult(crc_x2n(1, 18), e1, crc_poly(1)) ^ A.ttot[nt + t];
         en += A.cnt[t];
     }
     s0[tid] = e0; s1[tid] = e1; sc[tid] = en;
@@ -200,7 +152,7 @@ __global__ void __launch_bounds__(REC_TILES_T) rec_tiles_kernel(const __grid_con
         __syncthreads();
         if (tid >= d) {                                // the right operand covers d threads' tiles
             const uint64_t bytes = (uint64_t)d * per * REC_TILE;
-            e0 ^= rec_shift(a0, bytes, 0); e1 ^= rec_shift(a1, bytes, 1); en += an;
+            e0 ^= crc_shift(a0, bytes, 0); e1 ^= crc_shift(a1, bytes, 1); en += an;
         }
         s0[tid] = e0; s1[tid] = e1; sc[tid] = en;
         __syncthreads();
@@ -208,7 +160,7 @@ __global__ void __launch_bounds__(REC_TILES_T) rec_tiles_kernel(const __grid_con
     const uint32_t x0 = tid ? s0[tid - 1] : 0, x1 = tid ? s1[tid - 1] : 0, xn = tid ? sc[tid - 1] : 0;
     for (uint32_t t = t0; t < t1; t++) {
         const uint64_t bytes = (uint64_t)(t - t0) * REC_TILE;
-        A.tex[t] ^= rec_shift(x0, bytes, 0); A.tex[nt + t] ^= rec_shift(x1, bytes, 1); A.tbase[t] += xn;
+        A.tex[t] ^= crc_shift(x0, bytes, 0); A.tex[nt + t] ^= crc_shift(x1, bytes, 1); A.tbase[t] += xn;
     }
     if (tid == REC_TILES_T - 1) A.tbase[nt] = sc[tid];
 }
@@ -241,13 +193,13 @@ __device__ __forceinline__ uint32_t rec_prefix(const RecArgs& A, const uint32_t*
     if (u == 0) return 0;
     const uint32_t q = (u - 1) / REC_PIECE, t = q / REC_T, lq = q % REC_T;     // the piece holding byte u - 1
     uint32_t c = A.tex[pi * A.ntiles + t];
-    if (lq) c = rec_shift(c, (uint64_t)lq * REC_PIECE, pi) ^ A.pin[pi * A.npieces + q - 1];
-    return rec_bytes(T, c, A.b + (uint64_t)q * REC_PIECE, u - q * REC_PIECE);
+    if (lq) c = crc_shift(c, (uint64_t)lq * REC_PIECE, pi) ^ A.pin[pi * A.npieces + q - 1];
+    return crc_bytes(T, c, A.b + (uint64_t)q * REC_PIECE, u - q * REC_PIECE);
 }
 // Raw CRC (register starting at 0) of [u, v) of the batch.
 __device__ __forceinline__ uint32_t rec_raw(const RecArgs& A, const uint32_t* T, int pi, uint32_t u, uint32_t v) {
-    if (v - u <= 2 * REC_PIECE) return rec_bytes(T, 0, A.b + u, v - u);
-    return rec_prefix(A, T, pi, v) ^ rec_shift(rec_prefix(A, T, pi, u), v - u, pi);
+    if (v - u <= 2 * REC_PIECE) return crc_bytes(T, 0, A.b + u, v - u);
+    return rec_prefix(A, T, pi, v) ^ crc_shift(rec_prefix(A, T, pi, u), v - u, pi);
 }
 // The CRC an entry of magic m at x (ending at e <= L) stores and the one its bytes have.
 __device__ __forceinline__ void rec_entry_crc(const RecArgs& A, const uint32_t (*T)[256], uint32_t x, uint32_t e, uint32_t* stored,
@@ -256,13 +208,13 @@ __device__ __forceinline__ void rec_entry_crc(const RecArgs& A, const uint32_t (
     const int pi = m == 2 ? 0 : 1;
     const uint32_t from = x + (m == 2 ? 21 : 16);
     *stored = rec_be32(A.b + x + (m == 2 ? 17 : 12));
-    *computed = ~(rec_raw(A, T[pi], pi, from, e) ^ rec_shift(0xffffffffu, e - from, pi));
+    *computed = ~(rec_raw(A, T[pi], pi, from, e) ^ crc_shift(0xffffffffu, e - from, pi));
 }
 
 // ---------------------------------------------------------------------------------------------------- rec_link
 __global__ void __launch_bounds__(REC_LINK_T) rec_link_kernel(const __grid_constant__ RecArgs A) {
     __shared__ uint32_t T[2][256];
-    rec_tables(T);
+    crc_tables(T);
     const uint32_t K = A.tbase[A.ntiles];
     for (uint32_t k = blockIdx.x * REC_LINK_T + threadIdx.x; k < K; k += gridDim.x * REC_LINK_T) {
         const uint32_t x = A.cpos[k];
@@ -335,7 +287,7 @@ __device__ __forceinline__ void rec_open(const RecArgs& A, const uint32_t (*T)[2
 
 __global__ void __launch_bounds__(32) rec_resolve_kernel(const __grid_constant__ RecArgs A, const RecCarry in, RecOut* out) {
     __shared__ uint32_t T[2][256];
-    rec_tables(T);
+    crc_tables(T);
     if (threadIdx.x != 0) return;
     RecOut o{};
     o.fail = ~0ull; o.kind = REC_OK;
@@ -356,15 +308,15 @@ __global__ void __launch_bounds__(32) rec_resolve_kernel(const __grid_constant__
             c.end = c.start + 12 + (uint32_t)size;
             c.stored = rec_be32(c.hdr + (m == 2 ? 17 : 12));
             const uint32_t from = m == 2 ? 21 : 16;            // covered header bytes that came before this batch
-            c.run = had > from ? rec_bytes(T[m == 2 ? 0 : 1], 0, c.hdr + from, had - from) : 0;
+            c.run = had > from ? crc_bytes(T[m == 2 ? 0 : 1], 0, c.hdr + from, had - from) : 0;
         }
         const int pi = c.magic == 2 ? 0 : 1;
         const uint64_t crc_from = c.start + (c.magic == 2 ? 21 : 16);
         const uint32_t from = crc_from > c.base ? (uint32_t)(crc_from - c.base) : 0;
         const uint32_t to = c.end - c.base < L ? (uint32_t)(c.end - c.base) : L;
-        if (to > from) c.run = rec_shift(c.run, to - from, pi) ^ rec_raw(A, T[pi], pi, from, to);
+        if (to > from) c.run = crc_shift(c.run, to - from, pi) ^ rec_raw(A, T[pi], pi, from, to);
         if (c.end - c.base > L) { c.base += L; o.carry = c; *out = o; return; }
-        const uint32_t computed = ~(c.run ^ rec_shift(0xffffffffu, c.end - crc_from, pi));
+        const uint32_t computed = ~(c.run ^ crc_shift(0xffffffffu, c.end - crc_from, pi));
         if (computed != c.stored) {
             rec_fail(o, c.start, REC_CRC, c.hdr, REC_HDR); o.stored = c.stored; o.computed = computed;
             *out = o; return;

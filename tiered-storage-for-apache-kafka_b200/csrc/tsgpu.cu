@@ -9,7 +9,8 @@
 //   up to (devices x slots) batches are in flight so copies overlap kernels.  With TSGPU_FLAG_VERIFY each batch is
 //   detransformed on the device and compared with its input before any of its bytes are copied out.  With
 //   TSGPU_FLAG_VALIDATE_RECORDS the Kafka log entries of each batch are checked on the device (records.cuh) and the batch's
-//   verdict is resolved, in batch order, before its bytes are copied out.
+//   verdict is resolved, in batch order, before its bytes are copied out.  tsgpu_transform_parts also hashes each packed batch
+//   (part_crc.cuh) and combines the CRC-32C of the object's upload parts on the host once the call's streams are idle.
 #include <condition_variable>
 #include <mutex>
 #include <new>
@@ -25,6 +26,7 @@
 #include "pack.cuh"
 #include "verify.cuh"
 #include "records.cuh"
+#include "part_crc.cuh"
 #include "rt.h"
 #include "launch_prof.h"
 #include "zstd_enc.cuh"
@@ -76,6 +78,17 @@ struct RecScratch {
     RecOut* h_out = nullptr;       // pinned
 };
 
+// Device arrays of the upload-part checksums of one slot (part_crc.cuh), sized for batches of up to `cap` packed bytes.
+struct PcrcScratch {
+    uint8_t* d = nullptr;
+    uint64_t cap = 0;
+    PcrcArgs a{};                  // the batch last enqueued on the slot: pcrc_cuts reads the same arrays at its drain
+    uint32_t* d_cuts = nullptr;    // pcrc_cuts output and its pinned copy, cuts_cap words
+    uint32_t* h_cuts = nullptr;
+    uint32_t cuts_cap = 0;
+    int32_t pending = -1;          // the call's batch whose prefixes h_cuts receives (collected at the slot's next drain or at the end)
+};
+
 struct Work {
     int device = 0;
     rt::stream_t stream{}, out_stream{};   // out_stream: copies of finished chunks back to the host
@@ -100,6 +113,7 @@ struct Work {
     ZstdDecScratch zdec{};
     uint32_t* h_sizes = nullptr;   // pinned: sizes/status (and the verify stage's first differing bytes) coming back
     RecScratch rec{};              // TSGPU_FLAG_VALIDATE_RECORDS, allocated on first use
+    PcrcScratch pcrc{};            // tsgpu_transform_parts, allocated on first use
 };
 
 struct Lane { int device = 0; Work w[NSLOT_MAX]; };
@@ -180,6 +194,7 @@ static void work_free(Work& w) {
     rt::free_device(w.d_partials); rt::free_device(w.d_keyctx); rt::free_host(w.h_sizes);
     zstd_enc_scratch_free(w.zenc); zstd_blk_scratch_free(w.zblk); zstd_dec_scratch_free(w.zdec);
     rt::free_device(w.rec.d); rt::free_device(w.rec.d_out); rt::free_host(w.rec.h_out); w.rec = RecScratch{};
+    rt::free_device(w.pcrc.d); rt::free_device(w.pcrc.d_cuts); rt::free_host(w.pcrc.h_cuts); w.pcrc = PcrcScratch{};
     memset(&w.key_rk, 0, sizeof w.key_rk); w.key_valid = false;
     rt::event_destroy(w.ev_sizes); rt::event_destroy(w.ev_done);
     rt::event_destroy(w.ev_dev_desc); rt::event_destroy(w.ev_dev_done);
@@ -454,9 +469,11 @@ struct Batch { Work* w; uint32_t c0, nb; };      // chunks [c0, c0 + nb) of a ca
 
 // Cuts n chunks into batches of max_batch and deals them round-robin over the slots it claims.  issue(batch) enqueues a
 // batch on its slot's stream and ends with the D2H of its sizes (ev_sizes); drain(batch) runs once those sizes are on the
-// host, in batch order, and sends the batch's bytes home (copy_out).  Returns with every claimed slot idle.
-template <class Issue, class Drain>
-static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain) {
+// host, in batch order, and sends the batch's bytes home (copy_out).  idle(slots, rc) runs once every claimed slot is idle,
+// before the slots are given back.  Returns with every claimed slot idle.
+namespace { struct NoIdle { int operator()(const std::vector<Work*>&, int rc) const { return rc; } }; }
+template <class Issue, class Drain, class Idle = NoIdle>
+static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain, Idle idle = Idle()) {
     const uint32_t nbatches = (n + c->max_batch - 1) / c->max_batch;
     SlotClaim claim;
     { int rcc = claim_slots(c, nbatches, claim); if (rcc) return rcc; }
@@ -488,7 +505,7 @@ static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain) {
         if (e && rc == TSGPU_OK) rc = fail(TSGPU_E_CUDA, "stream_sync: %s", e);
         w->out_pending = false;
     }
-    return rc;
+    return idle(claim.slots, rc);
 }
 
 // A drained batch's `total` bytes at `from` go to dst + dst_off on the slot's copy-out stream (the sizes event has
@@ -611,6 +628,106 @@ static int records_segment_end(const RecCarry& carry) {
     return records_failure(o);
 }
 
+// ------------------------------------------------------------------------------------------ upload-part checksums
+// The state of an object between calls: the public tsgpu_parts_cursor (32 bytes, zero = start of the object).
+struct PartsCarry {
+    uint64_t obj_len;      // object bytes so far
+    uint64_t part_size;    // the segment's part size (checked against every later call)
+    uint32_t part_raw;     // raw CRC-32C of the open part's bytes (obj_len % part_size of them)
+    uint32_t obj_raw;      // raw CRC-32C of the object so far
+    uint64_t reserved;
+};
+static_assert(sizeof(PartsCarry) == sizeof(tsgpu_parts_cursor), "the cursor holds the carry");
+
+// One batch of a tsgpu_transform_parts call, L packed bytes: words[k] is the raw CRC of [0, x_k) of the batch,
+// x_k = first + k * part_size for k < m (the part boundaries strictly inside it), x_m = L.
+struct PcrcBatch { uint32_t L = 0, first = 0, m = 0; std::vector<uint32_t> words; };
+struct PartsRun {
+    uint64_t part_size = 0;
+    uint64_t obj0 = 0;                 // object bytes before the call
+    std::vector<PcrcBatch> batches;    // by batch index
+};
+
+static int parts_alloc(PcrcScratch& r, uint64_t cap, rt::stream_t st) {
+    if (r.cap >= cap) return TSGPU_OK;
+    rt::free_device(r.d); r.d = nullptr; r.cap = 0;
+    const uint64_t np = (cap + PCRC_PIECE - 1) / PCRC_PIECE, nt = (cap + PCRC_TILE - 1) / PCRC_TILE;
+    const uint64_t sz[3] = {4 * np, 4 * nt, 4};
+    uint64_t total = 0;
+    for (uint64_t b : sz) total += align_up(b, 256);
+    RT(rt::malloc_device((void**)&r.d, total));
+    uint8_t* p = r.d;
+    auto take = [&](uint64_t b) { uint8_t* q = p; p += align_up(b, 256); return q; };
+    r.a.pin = (uint32_t*)take(sz[0]); r.a.ttot = (uint32_t*)take(sz[1]); r.a.done = (uint32_t*)take(sz[2]);
+    RT(rt::memset_async(r.a.done, 0, 4, st));
+    r.cap = cap;
+    return TSGPU_OK;
+}
+
+// Enqueues pcrc_tiles over the batch's packed chunks (d_pack, sizes `len` on the device, at most `bound` bytes in all).
+static int parts_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint32_t* len, uint32_t nb, uint64_t bound) {
+    { int rc = parts_alloc(w.pcrc, (uint64_t)c->max_batch * c->slot_stride, st); if (rc) return rc; }
+    PcrcArgs& a = w.pcrc.a;
+    a.b = w.d_pack; a.len = len; a.nb = nb;
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(PCRC_GRID, (bound + PCRC_TILE - 1) / PCRC_TILE);
+    TS_LAUNCH_P(c->prof, "pcrc_tiles", pcrc_tiles_kernel, dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
+    CHECK_LAUNCH("pcrc_tiles_kernel");
+    return TSGPU_OK;
+}
+
+// The prefixes of the slot's previous batch are on the host once this slot's sizes event has completed: the batch's first
+// kernel that rewrites d_pack waited for the previous copy-out (wait_copies_out), and pcrc_cuts and its D2H precede that copy.
+static void parts_collect(Work& w, PartsRun& pr) {
+    PcrcScratch& p = w.pcrc;
+    if (p.pending < 0) return;
+    PcrcBatch& b = pr.batches[(size_t)p.pending];
+    b.words.assign(p.h_cuts, p.h_cuts + b.m + 1);
+    p.pending = -1;
+}
+
+// At the drain of batch `bi` (L packed bytes at object offset `at`): pcrc_cuts and the D2H of its m + 1 words on out_stream,
+// ahead of the batch's copy-out.
+static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun& pr, uint32_t bi, uint64_t at, uint64_t L) {
+    parts_collect(w, pr);
+    PcrcScratch& p = w.pcrc;
+    const uint64_t P = pr.part_size;
+    const uint64_t first = P - at % P;                                   // the first part boundary after the batch's start
+    const uint32_t m = first < L ? (uint32_t)((L - 1 - first) / P + 1) : 0;
+    if (m + 1 > p.cuts_cap) {                                            // nothing on the slot reads the old arrays any more
+        rt::free_device(p.d_cuts); rt::free_host(p.h_cuts); p.d_cuts = nullptr; p.h_cuts = nullptr; p.cuts_cap = 0;
+        const uint32_t cap = std::max<uint32_t>(64, m + 1);
+        RT(rt::malloc_device((void**)&p.d_cuts, 4ull * cap));
+        RT(rt::malloc_host((void**)&p.h_cuts, 4ull * cap));
+        p.cuts_cap = cap;
+    }
+    TS_LAUNCH_P(c->prof, "pcrc_cuts", pcrc_cuts_kernel, dim3((m + PCRC_CUTS_T) / PCRC_CUTS_T), dim3(PCRC_CUTS_T), 0, w.out_stream,
+                p.a, (uint32_t)L, m ? (uint32_t)first : 0u, P, m, p.d_cuts);
+    CHECK_LAUNCH("pcrc_cuts_kernel");
+    RT(rt::d2h(p.h_cuts, p.d_cuts, 4ull * (m + 1), w.out_stream));
+    PcrcBatch& b = pr.batches[bi];
+    b.L = (uint32_t)L; b.first = m ? (uint32_t)first : 0u; b.m = m; b.words.clear();
+    p.pending = (int32_t)bi;
+    return TSGPU_OK;
+}
+
+// The call's batches in order: their pieces extend the open part and the object; a part whose last byte arrives is emitted.
+static void parts_combine(const PartsRun& pr, PartsCarry& cur, std::vector<uint32_t>& emitted) {
+    const uint64_t P = pr.part_size;
+    for (const PcrcBatch& b : pr.batches) {
+        uint32_t prev = 0, prev_x = 0;
+        for (uint32_t k = 0; k <= b.m; k++) {
+            const uint32_t x = k < b.m ? (uint32_t)(b.first + k * P) : b.L;
+            const uint32_t n = x - prev_x;
+            const uint32_t raw = b.words[k] ^ crc_shift(prev, n, 0);      // raw CRC of [prev_x, x)
+            cur.part_raw = crc_shift(cur.part_raw, n, 0) ^ raw;
+            cur.obj_len += n;
+            if (n && cur.obj_len % P == 0) { emitted.push_back(crc_finish(cur.part_raw, P, 0)); cur.part_raw = 0; }
+            prev = b.words[k]; prev_x = x;
+        }
+        cur.obj_raw = crc_shift(cur.obj_raw, b.L, 0) ^ b.words[b.m];
+    }
+}
+
 #ifdef TSGPU_SIMT
 // TEST-ONLY fault injection, compiled into the emulator build alone (device memory is host memory there and every kernel
 // has finished when its launch returns).  TSGPU_SIMT_FLIP=<chunk>:<offset> flips the low bit of one byte of that chunk's
@@ -629,7 +746,7 @@ static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
 // One batch: copy in, fill the descriptors, enqueue the stages, pack the transformed chunks, [verify them,] D2H of their
 // sizes (and of the verify stage's verdicts).
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
-static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, const uint8_t* src, const uint64_t* off,
+static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, bool parts, const uint8_t* src, const uint64_t* off,
                            const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
                            const uint8_t* ivs) {
     Work& w = *bt.w;
@@ -668,6 +785,7 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool v
         const uint64_t longest = (flags & TSGPU_FLAG_ZSTD) ? frame_bound(cs) + 28 : (uint64_t)cs + 28;
         TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
         CHECK_LAUNCH("pack_chunks_kernel");
+        if (parts) { int rc = parts_stage(c, w, st, fin.len, nb, longest * nb); if (rc) return rc; }
     }
     if (verify) {
         int rc = verify_stage(c, w, st, flags, nb, cs, rk, aad_len, fin);
@@ -705,7 +823,7 @@ static int verify_verdict(const Batch& bt, const uint32_t* len) {
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                             const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
-                            RecCarry* records);
+                            RecCarry* records, PartsRun* parts = nullptr);
 
 static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint8_t* key, const uint8_t* aad,
                              uint32_t aad_len, const uint8_t* ivs, uint32_t* transformed_sizes, uint32_t* n_chunks) {
@@ -720,10 +838,15 @@ static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
 }
 
 static_assert(sizeof(tsgpu_records_cursor) == sizeof(RecCarry), "the cursor holds the carry");
+// The part-checksum arguments of tsgpu_transform_parts.
+struct PartsReq {
+    uint64_t part_size; tsgpu_parts_cursor* cursor;
+    uint32_t* crcs; uint32_t cap; uint32_t* n; uint32_t* object_crc;
+};
 static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
                              const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
                              uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
-                             bool env_default);
+                             bool env_default, const struct PartsReq* parts = nullptr);
 
 extern "C" int tsgpu_transform(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
                                const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
@@ -744,10 +867,55 @@ extern "C" int tsgpu_transform_cursor(tsgpu_ctx* c, uint32_t flags, const uint8_
                              cursor, segment_ends_here, /*env_default=*/true);
 }
 
+extern "C" int tsgpu_transform_parts(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
+                                     const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                                     uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                                     tsgpu_records_cursor* records, int segment_ends_here,
+                                     uint64_t part_size, tsgpu_parts_cursor* parts,
+                                     uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts, uint32_t* object_crc32c) {
+    const PartsReq req{part_size, parts, part_crc32c, part_cap, n_parts, object_crc32c};
+    return transform_segment(c, flags, src, src_len, chunk_size, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, n_chunks,
+                             records, segment_ends_here, /*env_default=*/true, &req);
+}
+
+// The part-checksum arguments, checked before any GPU work.  `bound`: the most bytes the call can add to the object.
+static int parts_args_ok(const PartsReq& q, uint32_t flags, uint64_t bound, int segment_ends_here) {
+    if (!(flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)))
+        return fail(TSGPU_E_ARG, "tsgpu_transform_parts needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU");
+    if (q.part_size == 0) return fail(TSGPU_E_ARG, "part_size must be at least 1");
+    if (!q.cursor || !q.n || !q.object_crc) return fail(TSGPU_E_ARG, "parts cursor, n_parts and object_crc32c cannot be null");
+    PartsCarry cur;
+    memcpy(&cur, q.cursor, sizeof cur);
+    if (cur.obj_len && cur.part_size != q.part_size)
+        return fail(TSGPU_E_ARG, "part_size %llu differs from the %llu the object started with", (unsigned long long)q.part_size,
+                    (unsigned long long)cur.part_size);
+    const uint64_t most = (cur.obj_len % q.part_size + bound) / q.part_size + (segment_ends_here ? 1 : 0);
+    if (most > q.cap) return fail(TSGPU_E_SHORT, "part_crc32c too small: the call may complete %llu parts, part_cap is %u",
+                                  (unsigned long long)most, q.cap);
+    if (q.cap && !q.crcs) return fail(TSGPU_E_ARG, "part_crc32c cannot be null");
+    return TSGPU_OK;
+}
+
+// After a successful call: the completed parts (and at the segment's end the open part and the object CRC) go out, and the
+// cursor moves on.  Nothing is written before: a failed call leaves part_crc32c and object_crc32c as they were.
+static void parts_finish(const PartsReq& q, PartsCarry cur, const PartsRun* run, int segment_ends_here) {
+    std::vector<uint32_t> emitted;
+    if (run) parts_combine(*run, cur, emitted);
+    cur.part_size = q.part_size;
+    if (segment_ends_here) {
+        const uint64_t open = cur.obj_len % q.part_size;
+        if (open) { emitted.push_back(crc_finish(cur.part_raw, open, 0)); cur.part_raw = 0; }
+        *q.object_crc = crc_finish(cur.obj_raw, cur.obj_len, 0);
+    }
+    if (!emitted.empty()) memcpy(q.crcs, emitted.data(), 4 * emitted.size());
+    *q.n = (uint32_t)emitted.size();
+    memcpy(q.cursor, &cur, sizeof cur);
+}
+
 static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
                              const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
                              uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
-                             bool env_default) try {
+                             bool env_default, const PartsReq* parts) try {
     int rc = transform_args_ok(c, flags, src, src_len, key, aad, aad_len, ivs, transformed_sizes, n_chunks);
     if (rc) return rc;
     const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
@@ -758,29 +926,42 @@ static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     if (records && !cursor) return fail(TSGPU_E_ARG, "cursor cannot be null when record batches are validated");
     RecCarry carry{};
     if (records) memcpy(&carry, cursor, sizeof carry);
+    PartsCarry pcarry{};
+    if (parts) {
+        rc = parts_args_ok(*parts, flags, src_len ? tsgpu_transform_bound(flags, src_len, chunk_size) : 0, segment_ends_here);
+        if (rc) return rc;
+        memcpy(&pcarry, parts->cursor, sizeof pcarry);
+    }
     // BaseTransformChunkEnumeration: originalChunkSize 0 disables chunking (one chunk = whole stream)
     uint64_t cs64 = chunk_size ? chunk_size : src_len;
     if (src_len == 0) {
         if (records && segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
         *n_chunks = 0;
+        if (parts) parts_finish(*parts, pcarry, nullptr, segment_ends_here);
         return TSGPU_OK;
     }
     if (cs64 > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk size %llu exceeds the context's max_chunk_bytes %u", (unsigned long long)cs64, c->chunk_cap);
     const uint32_t cs = (uint32_t)cs64;
     if (records && (uint64_t)c->max_batch * cs > REC_MAX_BATCH)
         return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch, cs);
+    if (parts && (uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
+        return fail(TSGPU_E_ARG, "part checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
+                    (unsigned long long)c->slot_stride);
     const uint64_t n64 = (src_len + cs - 1) / cs;
     if (n64 > *n_chunks) return fail(TSGPU_E_SHORT, "transformed_sizes too small: %llu chunks", (unsigned long long)n64);
     std::vector<uint64_t> off(n64);
     std::vector<uint32_t> len(n64);
     for (uint64_t i = 0; i < n64; i++) { off[i] = i * cs; len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - i * cs); }
+    PartsRun run;
+    if (parts) { run.part_size = parts->part_size; run.obj0 = pcarry.obj_len; }
     rc = transform_common(c, flags & ~TSGPU_FLAG_VALIDATE_RECORDS, src, src_len, off, len, cs, key, aad, aad_len, ivs, dst, dst_cap,
-                          transformed_sizes, n_chunks, records ? &carry : nullptr);
+                          transformed_sizes, n_chunks, records ? &carry : nullptr, parts ? &run : nullptr);
     if (rc) return rc;
     if (records) {
         if (segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
         memcpy(cursor, &carry, sizeof carry);
     }
+    if (parts) parts_finish(*parts, pcarry, &run, segment_ends_here);
     return TSGPU_OK;
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
@@ -812,7 +993,7 @@ extern "C" int tsgpu_transform_chunks(tsgpu_ctx* c, uint32_t flags, const uint8_
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                             const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
-                            RecCarry* records) {
+                            RecCarry* records, PartsRun* parts) {
     const uint32_t n = (uint32_t)len.size();
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
     if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~ZSTD_MODIFIERS;         // modifiers of ZSTD: meaningless (and harmless) without it
@@ -830,15 +1011,24 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
 
     uint64_t dst_off = 0;
+    if (parts) parts->batches.assign((n + c->max_batch - 1) / c->max_batch, PcrcBatch{});
     const int rc = run_batches(c, n,
-        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, records != nullptr, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
+        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, records != nullptr, parts != nullptr, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
         [&](const Batch& bt) {
             Work& w = *bt.w;
             if (records) { int rcr = records_resolve(c, w, *records); if (rcr) return rcr; }   // the input first: none of the batch's bytes leave
             if (verify) { int rcv = verify_verdict(bt, len.data()); if (rcv) return rcv; }   // none of the batch's bytes leave
             uint64_t total = 0;
             for (uint32_t i = 0; i < bt.nb; i++) { transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
+            if (parts && dst_off + total <= dst_cap) {
+                int rcp = parts_drain(c, w, *parts, bt.c0 / c->max_batch, parts->obj0 + dst_off, total);
+                if (rcp) return rcp;
+            }
             return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);     // one copy per batch: packed on the device
+        },
+        [&](const std::vector<Work*>& slots, int rcb) {                     // the last batches' part prefixes, once all is idle
+            if (parts) for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, *parts); w->pcrc.pending = -1; }
+            return rcb;
         });
     if (rc) return rc;
     *n_chunks = n;

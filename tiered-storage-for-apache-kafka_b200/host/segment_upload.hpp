@@ -145,8 +145,9 @@ private:
     int64_t last_;
 };
 
-// S3MultiPartOutputStream: the object goes out in parts of exactly partSize bytes, the last one may be shorter.
-struct UploadPart { int partNumber; uint64_t offset; uint64_t size; };
+// S3MultiPartOutputStream: the object goes out in parts of exactly partSize bytes, the last one may be shorter.  With
+// SegmentLogUploader::partChecksums a part carries the CRC-32C of its bytes, computed on the GPU (tsgpu_transform_parts).
+struct UploadPart { int partNumber; uint64_t offset; uint64_t size; std::optional<uint32_t> crc32c = std::nullopt; };
 inline std::vector<UploadPart> multipartPlan(uint64_t objectBytes, uint64_t partSize) {
     if (partSize == 0) throw IllegalArgumentException("partSize must be positive");
     std::vector<UploadPart> parts;
@@ -164,6 +165,7 @@ struct SegmentLogUpload {
     uint64_t objectBytes = 0;
     bool compressed = false;
     std::vector<int32_t> transformedSizes;
+    std::optional<uint32_t> objectCrc32c;                // with partChecksums: CRC-32C of the whole object (S3 FULL_OBJECT, GCS crc32c)
 };
 class SegmentLogUploader {
 public:
@@ -179,6 +181,11 @@ public:
     // upload with InvalidRecordBatchException, so the copy is retried and the local segment kept.  It applies when the segment
     // is compressed or encrypted: otherwise the transform is a plain copy on the host and no byte reaches the GPU.
     bool validateRecords = false;
+    // Hand every part to the sink with the CRC-32C of its bytes, and the object's CRC-32C in the result, both computed on the GPU
+    // from the bytes it copied out (tsgpu_transform_parts with this uploader's partSize): the storage client sends them with the
+    // part (S3 x-amz-checksum-crc32c, GCS crc32c; INTEGRATION.md), so damage on any later hop is refused by the object store.
+    // Like validateRecords it applies when the segment is compressed or encrypted; otherwise no byte reaches the GPU.
+    bool partChecksums = false;
     // `log`/`n`: the segment file (ideally in memory from tsgpu_host_alloc); `ivs`: 12 bytes per chunk when encrypting.
     SegmentLogUpload upload(const uint8_t* log, uint64_t n, const DataKeyAndAAD* key, const uint8_t* ivs, const PartSink& sink) {
         if (n > 0x7fffffffull) throw IllegalArgumentException("originalFileSize must fit an int");
@@ -199,8 +206,24 @@ public:
         uint32_t nChunks = (uint32_t)((n + per - 1) / per);
         std::vector<uint32_t> sizes(nChunks ? nChunks : 1);
         uint32_t got = (uint32_t)sizes.size();
-        const int rc = tsgpu_transform(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
-                                       key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got);
+        const bool checksums = partChecksums && flags;
+        std::vector<uint32_t> partCrcs;
+        uint32_t objectCrc = 0;
+        int rc;
+        if (checksums) {
+            if (partSize == 0) throw IllegalArgumentException("partSize must be positive");
+            tsgpu_records_cursor records{};
+            tsgpu_parts_cursor parts{};
+            partCrcs.resize(bound / partSize + 2);
+            uint32_t nParts = 0;
+            rc = tsgpu_transform_parts(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
+                                       key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got, &records, 1,
+                                       partSize, &parts, partCrcs.data(), (uint32_t)partCrcs.size(), &nParts, &objectCrc);
+            partCrcs.resize(rc ? 0 : nParts);
+        } else {
+            rc = tsgpu_transform(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
+                                 key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got);
+        }
         if (rc == TSGPU_E_RECORDS) throw InvalidRecordBatchException(tsgpu_last_error());
         if (rc) throw std::runtime_error(tsgpu_last_error());            // RuntimeException in the reference
         // TransformFinisher: fixed index when every chunk has the same known transformed size, variable after compression
@@ -219,7 +242,13 @@ public:
             for (uint32_t i = 0; i + 1 < got; i++) b.addChunk((int)sizes[i]);
             r.chunkIndex = b.finish((int)sizes[got - 1]);
         }
-        for (const UploadPart& p : multipartPlan(r.objectBytes, partSize)) {
+        std::vector<UploadPart> plan = multipartPlan(r.objectBytes, partSize);
+        if (checksums) {
+            if (partCrcs.size() != plan.size()) throw std::runtime_error("part checksums do not match the multipart plan");
+            for (size_t i = 0; i < plan.size(); i++) plan[i].crc32c = partCrcs[i];
+            r.objectCrc32c = objectCrc;
+        }
+        for (const UploadPart& p : plan) {
             if (bucket) bucket->consume((int64_t)p.size);
             sink(p, dst + p.offset);
         }
