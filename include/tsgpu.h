@@ -221,6 +221,44 @@ int tsgpu_detransform(tsgpu_ctx* ctx, uint32_t flags,
                       uint8_t* dst, uint64_t dst_cap, uint32_t* original_sizes);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * tsgpu_check_object — proof that a stored .log object still decodes to a valid segment, without its plaintext leaving the GPU.
+ * It reads what tsgpu_detransform reads and runs the same stages, but copies nothing back except sizes, statuses, record verdicts
+ * and CRC words: for an object that is the only copy of its segment (after local.retention), one moved between buckets or
+ * providers, or one written by the Java plugin before the broker used this library.  Every chunk is checked, in object order:
+ *   1. its GCM tag (AES);  2. its zstd frame, and the frame's Content_Checksum when it carries one (ZSTD);
+ *   3. its decoded size against the manifest's chunk index (AbstractChunkIndex.materializeChunks): ceil(original_file_size /
+ *      original_chunk_size) chunks, each of original_chunk_size bytes but the last, which holds the remainder; an empty segment
+ *      has no chunk (or the index's one chunk of 0 transformed bytes, which a caller may pass);
+ *   4. with TSGPU_FLAG_VALIDATE_RECORDS: every record batch of the decoded segment, with the rules and messages of that flag on
+ *      the upload side (a segment that ends inside an entry fails with check "length").
+ *
+ *   flags          the manifest's compression (TSGPU_FLAG_ZSTD; ZSTD_DENSE and ZSTD_CHECKSUM are accepted and ignored) and
+ *                  encryption (TSGPU_FLAG_AES), plus TSGPU_FLAG_VALIDATE_RECORDS; any other bit fails with TSGPU_E_ARG.  Flags 0
+ *                  is a plain object: it is the segment, and only the size, record and CRC checks apply.
+ *   src, transformed_sizes, n_chunks, key, aad   one window of the object, as tsgpu_detransform takes it (n_chunks may be 0)
+ *   original_chunk_size, original_file_size      the manifest's chunk index (original_chunk_size <= the context's max_chunk_bytes)
+ *   cursor         128 bytes, zeroed at the start of the object; a caller checks an object in windows of chunks, in order,
+ *                  passing the same cursor (chunks and bytes so far, the two running CRCs, the record-validation state).  It is
+ *                  updated on success; after a failure it has no defined value.
+ *   object_ends_here  != 0 on the last window (which may be empty): the chunk count must then match the index, and
+ *                  *object_crc32c receives the CRC-32C of the object's bytes (compare with S3's FULL_OBJECT checksum, GCS's crc32c
+ *                  or the object CRC of tsgpu_transform_parts recorded at upload) and *segment_crc32c that of the decoded segment
+ *                  (compare with the local segment file before it is deleted).  Neither is written before the end or on failure.
+ * Returns the first failure in object order: TSGPU_E_AUTH (a tag), TSGPU_E_CORRUPT (a frame, a Content_Checksum, or a decoded
+ * size or chunk count that disagrees with the index; the message names the chunk and both sizes), TSGPU_E_RECORDS (the message
+ * names the segment position), TSGPU_E_SHORT (src_len below the sum of transformed_sizes).  Within a batch of chunks, a tag, frame
+ * or size failure is reported before the batch's record verdict.  TSGPU_E_ARG as tsgpu_detransform for sizes beyond the
+ * context's capacity.  Cost and memory: DESIGN.md §3, §8.
+ * --------------------------------------------------------------------------------------------------------- */
+typedef struct tsgpu_check_cursor { uint64_t opaque[16]; } tsgpu_check_cursor;
+int tsgpu_check_object(tsgpu_ctx* ctx, uint32_t flags,
+                       const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes, uint32_t n_chunks,
+                       uint32_t original_chunk_size, uint64_t original_file_size,
+                       const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
+                       tsgpu_check_cursor* cursor, int object_ends_here,
+                       uint32_t* object_crc32c, uint32_t* segment_crc32c);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Device-resident variants (inputs and outputs already in HBM of device `device_index` of the context; used by
  * bench.py for the kernel-side throughput and by callers that keep segments on the GPU).  Layouts:
  *   original side     contiguous, chunk i at i * chunk_size

@@ -3,7 +3,7 @@
  * There is no JDK in this repository's build image: the tests compile this file against a test-only stand-in for
  * <jni.h> and drive it through a fake JNIEnv (tests/cpp/test_jni_shim.c).  Build on the broker host with
  *   gcc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude jni/tsgpu_jni.c -L<pkg> -ltsgpu -o libtsgpu_jni.so
- * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
+ * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
  * (implement TransformChunkEnumeration / DetransformChunkEnumeration of the reference, core/M/transform/TransformChunkEnumeration.java:28-42,
  * DetransformChunkEnumeration.java:28-29) and jni/io/aiven/kafka/tieredstorage/fetch/gpu/GpuChunkManager.java (ChunkManager, fetch/ChunkManager.java).
  *
@@ -179,4 +179,41 @@ JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_det
     if (k) (*env)->ReleaseByteArrayElements(env, key, k, JNI_ABORT);
     if (a) (*env)->ReleaseByteArrayElements(env, aad, a, JNI_ABORT);
     if (rc) throw_rt(env, rc);
+}
+
+/* One window of a stored object checked against its chunk index (CheckCursor.checkObject, tsgpu_check_object): `cursor` a direct
+ * ByteBuffer of at least 128 bytes holding the tsgpu_check_cursor (zeros at the start of the object), updated in place;
+ * crcsOut (int[2]) receives, on the object's last window, the CRC-32C of the object and of the decoded segment. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_CheckCursor_checkObject(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray transformedSizes, jint originalChunkSize,
+    jlong originalFileSize, jbyteArray key, jbyteArray aad, jobject cursor, jboolean objectEndsHere, jintArray crcsOut) {
+    jlong ccap = 0;
+    uint8_t* s = srcLen ? direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer") : NULL;
+    if (srcLen && !s) return;
+    tsgpu_check_cursor* cur = (tsgpu_check_cursor*)direct(env, cursor, 0, &ccap, "check cursor must be a direct ByteBuffer of 128 bytes");
+    if (!cur) return;
+    if (ccap < (jlong)sizeof(tsgpu_check_cursor)) { throw_arg(env, "check cursor must be a direct ByteBuffer of 128 bytes"); return; }
+    if (!transformedSizes) { throw_arg(env, "chunks cannot be null"); return; }
+    if (!crcsOut || (*env)->GetArrayLength(env, crcsOut) < 2) { throw_arg(env, "crcsOut must hold 2 ints"); return; }
+    if (originalChunkSize < 1) { throw_arg(env, "Original chunk size must be positive"); return; }
+    if (originalFileSize < 0) { throw_arg(env, "Original file size must be non-negative"); return; }
+    if ((flags & TSGPU_FLAG_AES) && key && (*env)->GetArrayLength(env, key) != 32) { throw_arg(env, "data key must be 32 bytes"); return; }
+    jbyte* k = key ? (*env)->GetByteArrayElements(env, key, NULL) : NULL;
+    jbyte* a = aad ? (*env)->GetByteArrayElements(env, aad, NULL) : NULL;
+    jint alen = aad ? (*env)->GetArrayLength(env, aad) : 0;
+    uint32_t n = (uint32_t)(*env)->GetArrayLength(env, transformedSizes);
+    jint* ts = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
+    uint32_t crcs[2] = {0, 0};
+    int rc = tsgpu_check_object((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (const uint32_t*)ts, n,
+                                (uint32_t)originalChunkSize, (uint64_t)originalFileSize, (const uint8_t*)k, (const uint8_t*)a,
+                                (uint32_t)alen, cur, objectEndsHere ? 1 : 0, &crcs[0], &crcs[1]);
+    (*env)->ReleaseIntArrayElements(env, transformedSizes, ts, JNI_ABORT);
+    if (k) (*env)->ReleaseByteArrayElements(env, key, k, JNI_ABORT);
+    if (a) (*env)->ReleaseByteArrayElements(env, aad, a, JNI_ABORT);
+    if (rc) { throw_rt(env, rc); return; }
+    if (objectEndsHere) {
+        jint* out = (*env)->GetIntArrayElements(env, crcsOut, NULL);
+        out[0] = (jint)crcs[0]; out[1] = (jint)crcs[1];
+        (*env)->ReleaseIntArrayElements(env, crcsOut, out, 0);
+    }
 }

@@ -25,6 +25,7 @@ E_VERIFY = -9
 E_RECORDS = -10
 CURSOR_SIZE = 64         # tsgpu_records_cursor
 PARTS_CURSOR_SIZE = 32   # tsgpu_parts_cursor
+CHECK_CURSOR_SIZE = 128  # tsgpu_check_cursor
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",
@@ -33,7 +34,7 @@ SYMBOLS = [
     "tsgpu_chunk_sizes_encode", "tsgpu_chunk_sizes_decode", "tsgpu_transformed_chunks_serialize",
     "tsgpu_transformed_chunks_deserialize", "tsgpu_chunk_index_json", "tsgpu_profile_enable", "tsgpu_profile_report",
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
-    "tsgpu_transform_cursor", "tsgpu_transform_parts",
+    "tsgpu_transform_cursor", "tsgpu_transform_parts", "tsgpu_check_object",
 ]
 
 
@@ -74,6 +75,7 @@ def load(path=None):
                                         u64, vp, vp, u32, vp, vp]
     L.tsgpu_transform_chunks.argtypes = [vp, u32, vp, vp, u32, vp, vp, u32, vp, vp, u64, vp]
     L.tsgpu_detransform.argtypes = [vp, u32, vp, u64, vp, u32, vp, vp, u32, vp, u64, vp]
+    L.tsgpu_check_object.argtypes = [vp, u32, vp, u64, vp, u32, u32, u64, vp, vp, u32, vp, C.c_int, vp, vp]
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
     L.tsgpu_detransform_device.argtypes = [vp, C.c_int, u32, vp, u64, vp, u32, u32, vp, vp, u32, vp, vp, vp, vp]
     L.tsgpu_launch_count.restype = u64
@@ -247,6 +249,25 @@ class Context:
                                                dst.ctypes.data, int(dst_cap), osz.ctypes.data))
         osz = osz[:ts.size]
         return dst[:int(osz.sum(dtype=np.uint64))], [int(x) for x in osz]
+
+    def check_object(self, flags, src, transformed_sizes, original_chunk_size, original_file_size, cursor=None,
+                     object_ends_here=True, key=None, aad=b""):
+        """Checks one window of a stored object against its chunk index on the GPU (tsgpu_check_object) without copying its
+        plaintext back.  `cursor`: a 128-byte np.uint8 array (zeros at the start of the object), updated in place on success; None
+        checks a whole object.  Returns (object CRC-32C, segment CRC-32C) when the object ends here, else None."""
+        s = _u8(src)
+        if cursor is None:
+            cursor = np.zeros(CHECK_CURSOR_SIZE, np.uint8)
+        if not (isinstance(cursor, np.ndarray) and cursor.dtype == np.uint8 and cursor.size == CHECK_CURSOR_SIZE
+                and cursor.flags.c_contiguous):
+            raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % CHECK_CURSOR_SIZE)
+        ts = np.ascontiguousarray(transformed_sizes, dtype=np.uint32)
+        obj, seg = C.c_uint32(0), C.c_uint32(0)
+        k, a = _u8(key), _u8(aad)
+        self._check(self.lib.tsgpu_check_object(self._h, flags, _p(s), s.size, _p(ts), ts.size, original_chunk_size,
+                                                original_file_size, _p(k), _p(a), a.size, cursor.ctypes.data,
+                                                1 if object_ends_here else 0, C.addressof(obj), C.addressof(seg)))
+        return (int(obj.value), int(seg.value)) if object_ends_here else None
 
     # ---- device-resident API (raw device pointers as ints; bench.py passes torch data_ptr()) ----
     def slot_stride(self, flags, chunk_size):

@@ -9,7 +9,10 @@
 //               batch and one for its end: the raw CRC of [0, x) of the batch from a tile prefix, a piece prefix and at most 256
 //               bytes.  The host turns consecutive prefixes into the raw CRCs of the part pieces (crc32.cuh) and combines them, in
 //               batch order, into the part CRCs and the object CRC.
+// With SLOTS (tsgpu_check_object) both kernels read the batch's chunks in place instead of packed: chunk i at b + off[i], as
+// the fetched object sits in its transformed slots.  The bytes hashed are the same, the chunks taken back to back.
 #pragma once
+#include <type_traits>
 #include "crc32.cuh"
 
 namespace ts {
@@ -27,6 +30,10 @@ struct PcrcArgs {
     uint32_t* ttot;                  // [ntiles]  raw CRC of each tile, then (after the last CTA) of [0, tile start)
     uint32_t* done;                  // CTAs of pcrc_tiles that have finished (the last one resets it to 0)
 };
+struct PcrcSlotsArgs : PcrcArgs {
+    const uint64_t* off;             // chunk i starts at b + off[i] (device)
+};
+template <bool SLOTS> using PcrcIn = typename std::conditional<SLOTS, PcrcSlotsArgs, PcrcArgs>::type;
 
 // Slice-by-8 tables of CRC-32C: T[k][i] is the raw CRC of byte i followed by k zero bytes.  Block-cooperative.
 __device__ __forceinline__ void pcrc_tables(uint32_t (*T)[256]) {
@@ -49,8 +56,43 @@ __device__ __forceinline__ uint32_t pcrc_len(const PcrcArgs& A) {
     return L;
 }
 
+// SLOTS: raw CRC update by bytes [lo, hi) of the batch's chunks taken back to back, each read where it sits.
+__device__ __forceinline__ uint32_t pcrc_slots_bytes(const uint32_t* T, uint32_t c, const PcrcSlotsArgs& A, uint32_t lo, uint32_t hi) {
+    uint32_t start = 0;
+    for (uint32_t i = 0; i < A.nb && lo < hi; i++) {
+        const uint32_t end = start + A.len[i];
+        if (lo < end) {
+            const uint32_t n = min(hi, end) - lo;
+            c = crc_bytes(T, c, A.b + A.off[i] + (lo - start), n);
+            lo += n;
+        }
+        start = end;
+    }
+    return c;
+}
+// SLOTS: raw CRC of the piece [lo, hi).  A full piece inside one chunk is read as aligned words joined by funnel shifts (a chunk
+// starts 4 bytes into its slot, and a piece anywhere in it); the word after the piece is still inside the slot, whose stride leaves
+// at least 16 bytes after the largest chunk it accepts.  Pieces across a chunk end and the batch's last piece go byte by byte.
+__device__ __forceinline__ uint32_t pcrc_slots_piece(const uint32_t (*T)[256], const PcrcSlotsArgs& A, uint32_t lo, uint32_t hi) {
+    uint32_t i = 0, start = 0;
+    while (i + 1 < A.nb && start + A.len[i] <= lo) start += A.len[i++];
+    if (hi - lo != PCRC_PIECE || hi > start + A.len[i]) return pcrc_slots_bytes(T[0], 0, A, lo, hi);
+    const uint8_t* p = A.b + A.off[i] + (lo - start);
+    const uint32_t* W = (const uint32_t*)((uintptr_t)p & ~(uintptr_t)3);
+    const uint32_t sh = (uint32_t)((uintptr_t)p & 3) * 8;
+    uint32_t c = 0, prev = __ldg(W);
+#pragma unroll 4
+    for (uint32_t k = 1; k <= PCRC_PIECE / 4; k += 2) {
+        const uint32_t w1 = __ldg(W + k), w2 = __ldg(W + k + 1);
+        c = pcrc_8(T, c, __funnelshift_r(prev, w1, sh), __funnelshift_r(w1, w2, sh));
+        prev = w2;
+    }
+    return c;
+}
+
 // ---------------------------------------------------------------------------------------------------- pcrc_tiles
-__global__ void __launch_bounds__(PCRC_T) pcrc_tiles_kernel(const __grid_constant__ PcrcArgs A) {
+template <bool SLOTS>
+__global__ void __launch_bounds__(PCRC_T) pcrc_tiles_kernel(const __grid_constant__ PcrcIn<SLOTS> A) {
     __shared__ uint32_t T[8][256];
     __shared__ uint32_t s[PCRC_T];
     __shared__ uint32_t last;
@@ -62,7 +104,9 @@ __global__ void __launch_bounds__(PCRC_T) pcrc_tiles_kernel(const __grid_constan
         const uint64_t lo64 = (uint64_t)q * PCRC_PIECE;
         const uint32_t lo = lo64 < L ? (uint32_t)lo64 : L, hi = min(L, lo + PCRC_PIECE);
         uint32_t c = 0;
-        if (hi - lo == PCRC_PIECE) {
+        if constexpr (SLOTS) {
+            c = pcrc_slots_piece(T, A, lo, hi);
+        } else if (hi - lo == PCRC_PIECE) {
             const uint4* v = (const uint4*)(A.b + lo);
 #pragma unroll 4
             for (uint32_t i = 0; i < PCRC_PIECE / 16; i++) {
@@ -119,7 +163,8 @@ __global__ void __launch_bounds__(PCRC_T) pcrc_tiles_kernel(const __grid_constan
 
 // ---------------------------------------------------------------------------------------------------- pcrc_cuts
 // out[k] = raw CRC of [0, x_k) of the batch, x_k = first + k * step for k < m, x_m = L.
-__global__ void __launch_bounds__(PCRC_CUTS_T) pcrc_cuts_kernel(const __grid_constant__ PcrcArgs A, uint32_t L, uint32_t first,
+template <bool SLOTS>
+__global__ void __launch_bounds__(PCRC_CUTS_T) pcrc_cuts_kernel(const __grid_constant__ PcrcIn<SLOTS> A, uint32_t L, uint32_t first,
                                                                 uint64_t step, uint32_t m, uint32_t* out) {
     __shared__ uint32_t T[256];
     for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) T[i] = crc_table_entry(i, CRC32C_POLY);
@@ -132,7 +177,8 @@ __global__ void __launch_bounds__(PCRC_CUTS_T) pcrc_cuts_kernel(const __grid_con
         const uint32_t q = (u - 1) / PCRC_PIECE, t = q / PCRC_T, lq = q % PCRC_T;     // the piece holding byte u - 1
         c = A.ttot[t];
         if (lq) c = crc_shift(c, (uint64_t)lq * PCRC_PIECE, 0) ^ A.pin[q - 1];
-        c = crc_bytes(T, c, A.b + (uint64_t)q * PCRC_PIECE, u - q * PCRC_PIECE);
+        if constexpr (SLOTS) c = pcrc_slots_bytes(T, c, A, q * PCRC_PIECE, u);
+        else c = crc_bytes(T, c, A.b + (uint64_t)q * PCRC_PIECE, u - q * PCRC_PIECE);
     }
     out[k] = c;
 }

@@ -670,7 +670,7 @@ static int parts_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint32_t* l
     PcrcArgs& a = w.pcrc.a;
     a.b = w.d_pack; a.len = len; a.nb = nb;
     const uint32_t grid = (uint32_t)std::min<uint64_t>(PCRC_GRID, (bound + PCRC_TILE - 1) / PCRC_TILE);
-    TS_LAUNCH_P(c->prof, "pcrc_tiles", pcrc_tiles_kernel, dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
+    TS_LAUNCH_P(c->prof, "pcrc_tiles", pcrc_tiles_kernel<false>, dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
     CHECK_LAUNCH("pcrc_tiles_kernel");
     return TSGPU_OK;
 }
@@ -700,7 +700,7 @@ static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun& pr, uint32_t bi, uint64_
         RT(rt::malloc_host((void**)&p.h_cuts, 4ull * cap));
         p.cuts_cap = cap;
     }
-    TS_LAUNCH_P(c->prof, "pcrc_cuts", pcrc_cuts_kernel, dim3((m + PCRC_CUTS_T) / PCRC_CUTS_T), dim3(PCRC_CUTS_T), 0, w.out_stream,
+    TS_LAUNCH_P(c->prof, "pcrc_cuts", pcrc_cuts_kernel<false>, dim3((m + PCRC_CUTS_T) / PCRC_CUTS_T), dim3(PCRC_CUTS_T), 0, w.out_stream,
                 p.a, (uint32_t)L, m ? (uint32_t)first : 0u, P, m, p.d_cuts);
     CHECK_LAUNCH("pcrc_cuts_kernel");
     RT(rt::d2h(p.h_cuts, p.d_cuts, 4ull * (m + 1), w.out_stream));
@@ -1036,14 +1036,12 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
 }
 
 // ------------------------------------------------------------------------------------------ detransform (host)
-// One batch: bound the sizes, copy the chunks in, fill the descriptors, enqueue the stages, D2H of sizes and status.
+// A batch's transformed chunks into the slot's d_xf, one per slot at i * slot_stride + TSGPU_SLOT_HEAD (16-byte aligned ciphertext
+// for the GCM kernel), and the descriptor block filled for detransform_enqueue (not yet uploaded).  Returns the bounds of the stages.
 // `src`: the batch's first transformed chunk.
-static int detransform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
-                             const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len) {
-    Work& w = *bt.w;
+static int dx_load(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
+                   const uint8_t* aad, uint32_t aad_len, DxBounds& lim) {
     const uint32_t c0 = bt.c0, nb = bt.nb;
-    RT(rt::set_device(w.device));
-    rt::stream_t st = w.stream;
     // Sizes come from a manifest, i.e. from outside: bound them per mode BEFORE any kernel writes (the GCM kernel
     // releases plaintext into the next buffer before the tag is checked).  AES only: plaintext lands in d_orig
     // (chunk_cap per chunk); AES+zstd: in a d_frames slot; zstd only: the frame is read in place from d_xf.
@@ -1065,9 +1063,21 @@ static int detransform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, cons
         max_t = std::max(max_t, t);
     }
     if ((flags & TSGPU_FLAG_AES) && aad_len) memcpy(w.hd.aad, aad, aad_len);
+    lim = DxBounds{max_t, room, 0xffffffffu, c->chunk_cap};
+    return TSGPU_OK;
+}
+
+// One batch: bound the sizes, copy the chunks in, fill the descriptors, enqueue the stages, D2H of sizes and status.
+static int detransform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
+                             const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len) {
+    Work& w = *bt.w;
+    const uint32_t nb = bt.nb;
+    RT(rt::set_device(w.device));
+    rt::stream_t st = w.stream;
+    DxBounds lim;
+    { int rc = dx_load(c, w, st, bt, flags, src, tsizes, aad, aad_len, lim); if (rc) return rc; }
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
     RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
-    const DxBounds lim{max_t, room, 0xffffffffu, c->chunk_cap};
     { int rc = detransform_enqueue(c, w, st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
                                    ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len}, w.dd.status, lim, /*packed=*/true); if (rc) return rc; }
     RT(rt::d2h(w.h_sizes, w.dd.a_len, 4ull * nb, st));
@@ -1129,6 +1139,196 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
         memset(dst, 0, (size_t)dst_off);
     }
     return rc;
+} catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
+
+// ------------------------------------------------------------------------------------------ object check (host)
+// tsgpu_check_object: the detransform of a stored object with nothing copied out.  Per batch, on the compute stream: the
+// transformed chunks into d_xf (flags 0: the plain chunks straight into d_orig), pcrc over them in their slots (the object
+// word), the detransform stages into d_orig packed, pcrc over d_orig (the segment word), [the record kernels,] and one D2H each
+// of the decoded sizes, the statuses and the two words.  At the drain, in object order: tag and frame statuses, decoded sizes
+// against the chunk index, the record verdict, then the words extend the cursor's CRCs.
+
+// The state of an object between calls: the public tsgpu_check_cursor (128 bytes, zero = start of the object).
+struct CheckCarry {
+    uint64_t chunks;       // chunks checked so far
+    uint64_t obj_len;      // object bytes so far
+    uint64_t seg_len;      // decoded segment bytes so far
+    uint32_t obj_raw;      // raw CRC-32C of the object so far
+    uint32_t seg_raw;      //   ... and of the decoded segment so far
+    RecCarry rec;          // TSGPU_FLAG_VALIDATE_RECORDS
+    uint64_t reserved[4];
+};
+static_assert(sizeof(CheckCarry) == sizeof(tsgpu_check_cursor), "the cursor holds the carry");
+
+// The chunk index of the manifest (AbstractChunkIndex.materializeChunks): ceil(ofs / ocs) chunks of ocs original bytes, the
+// last one holding the remainder; an empty segment has none.
+struct ChunkLayout {
+    uint32_t ocs; uint64_t ofs, count;
+    uint32_t size(uint64_t g) const { return g + 1 < count ? ocs : g + 1 == count ? (uint32_t)(ofs - g * ocs) : 0u; }
+};
+
+// The raw CRC-32C of a batch's L bytes into pcrc.d_cuts[k]: pcrc_tiles, then pcrc_cuts without part boundaries.
+template <bool SLOTS>
+static int check_crc_word(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint8_t* b, const uint64_t* off, const uint32_t* len,
+                          uint32_t nb, uint64_t L, uint32_t k) {
+    PcrcScratch& p = w.pcrc;
+    { int rc = parts_alloc(p, (uint64_t)c->max_batch * c->slot_stride, st); if (rc) return rc; }
+    if (!p.d_cuts) {
+        RT(rt::malloc_device((void**)&p.d_cuts, 4ull * 64));
+        RT(rt::malloc_host((void**)&p.h_cuts, 4ull * 64));
+        p.cuts_cap = 64;
+    }
+    p.a.b = b; p.a.len = len; p.a.nb = nb;
+    PcrcIn<SLOTS> a{};
+    static_cast<PcrcArgs&>(a) = p.a;
+    if constexpr (SLOTS) a.off = off;
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(PCRC_GRID, (L + PCRC_TILE - 1) / PCRC_TILE);
+    TS_LAUNCH_P(c->prof, SLOTS ? "pcrc_tiles_slots" : "pcrc_tiles", pcrc_tiles_kernel<SLOTS>, dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
+    CHECK_LAUNCH("pcrc_tiles_kernel");
+    TS_LAUNCH_P(c->prof, SLOTS ? "pcrc_cuts_slots" : "pcrc_cuts", pcrc_cuts_kernel<SLOTS>, dim3(1), dim3(PCRC_CUTS_T), 0, st,
+                a, (uint32_t)L, 0u, (uint64_t)1, 0u, p.d_cuts + k);
+    CHECK_LAUNCH("pcrc_cuts_kernel");
+    return TSGPU_OK;
+}
+
+// One batch of a check.  `src`: the batch's first transformed chunk; `g0`: the object's chunk number of the call's first chunk.
+// h_sizes receives the decoded sizes, the statuses and the object and segment words.
+static int check_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool records, const uint8_t* src, const uint32_t* tsizes,
+                       const ChunkLayout& index, uint64_t g0, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len) {
+    Work& w = *bt.w;
+    const uint32_t nb = bt.nb;
+    RT(rt::set_device(w.device));
+    rt::stream_t st = w.stream;
+    uint64_t L = 0, obj = 0;                 // the batch's length by the chunk index (what it decodes to when it is sound)
+    for (uint32_t i = 0; i < nb; i++) {
+        w.hd.v_len[i] = index.size(g0 + bt.c0 + i);
+        L += w.hd.v_len[i];
+        obj += tsizes[bt.c0 + i];
+    }
+    DxBounds lim{};
+    if (flags) {
+        int rc = dx_load(c, w, st, bt, flags, src, tsizes, aad, aad_len, lim);
+        if (rc) return rc;
+    } else {                                 // a plain object is the segment: its chunks go to d_orig back to back
+        for (uint32_t i = 0; i < nb; i++) {
+            if (tsizes[bt.c0 + i] > c->chunk_cap)
+                return fail(TSGPU_E_ARG, "transformed chunk of %u bytes exceeds the context's capacity", tsizes[bt.c0 + i]);
+            w.h_sizes[i] = tsizes[bt.c0 + i];
+            w.h_sizes[nb + i] = 0;
+        }
+        if (obj) RT(rt::h2d(w.d_orig, src, obj, st));
+    }
+    RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
+    if (flags) {
+        { int rc = check_crc_word<true>(c, w, st, w.d_xf, w.dd.c_off, w.dd.c_len, nb, obj, 0); if (rc) return rc; }
+        RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
+        int rc = detransform_enqueue(c, w, st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
+                                     ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len}, w.dd.status, lim, /*packed=*/true);
+        if (rc) return rc;
+    }
+    // The segment word and the records over the L bytes the index gives: a batch that decodes to another length fails first.
+    { int rc = check_crc_word<false>(c, w, st, w.d_orig, nullptr, w.dd.v_len, nb, L, 1); if (rc) return rc; }
+    if (records && L) {
+        int rc = records_alloc(w.rec, (uint64_t)c->max_batch * index.ocs);
+        if (!rc) rc = records_stage(c, w, st, L);
+        if (rc) return rc;
+    }
+    if (flags) {
+        RT(rt::d2h(w.h_sizes, w.dd.a_len, 4ull * nb, st));
+        RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
+    }
+    RT(rt::d2h(w.h_sizes + 2 * nb, w.pcrc.d_cuts, 8, st));
+    RT(rt::event_record(w.ev_sizes, st));
+    return TSGPU_OK;
+}
+
+// A drained batch in object order: every chunk's tag, frame and decoded size, then the record verdict, then the CRC words.
+static int check_drain(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool records, const uint32_t* tsizes, const ChunkLayout& index,
+                       CheckCarry& cur) {
+    Work& w = *bt.w;
+    const uint32_t nb = bt.nb;
+    const uint32_t* got = w.h_sizes;
+    const uint32_t* status = w.h_sizes + nb;
+    uint64_t L = 0, obj = 0;
+    for (uint32_t i = 0; i < nb; i++) {
+        const unsigned long long g = cur.chunks + bt.c0 + i;
+        if (status[i] == 1) return fail(TSGPU_E_AUTH, "Tag mismatch in chunk %llu", g);
+        if (status[i] > 1) return fail(TSGPU_E_CORRUPT, "Invalid zstd frame in chunk %llu (code %u)", g, status[i]);
+        if (g >= index.count)
+            return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, but the chunk index (original chunk size %u, original file "
+                        "size %llu) has %llu chunks", g, got[i], index.ocs, (unsigned long long)index.ofs, (unsigned long long)index.count);
+        if (got[i] != index.size(g))
+            return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, the chunk index gives %u", g, got[i], index.size(g));
+        L += got[i];
+        obj += tsizes[bt.c0 + i];
+    }
+    if (records) { int rc = records_resolve(c, w, cur.rec); if (rc) return rc; }
+    const uint32_t seg_word = w.h_sizes[2 * nb + 1], obj_word = flags ? w.h_sizes[2 * nb] : seg_word;
+    cur.obj_raw = crc_shift(cur.obj_raw, obj, 0) ^ obj_word;
+    cur.seg_raw = crc_shift(cur.seg_raw, L, 0) ^ seg_word;
+    return TSGPU_OK;
+}
+
+extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                                  uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
+                                  const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
+                                  tsgpu_check_cursor* cursor, int object_ends_here, uint32_t* object_crc32c, uint32_t* segment_crc32c) try {
+    if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
+    if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VALIDATE_RECORDS)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
+    if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
+    if (object_ends_here && (!object_crc32c || !segment_crc32c)) return fail(TSGPU_E_ARG, "object_crc32c/segment_crc32c cannot be null");
+    if (n_chunks && !transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
+    if (original_chunk_size == 0) return fail(TSGPU_E_ARG, "Original chunk size must be positive, 0 given");
+    if (original_chunk_size > c->chunk_cap)
+        return fail(TSGPU_E_ARG, "original chunk size %u exceeds the context's max_chunk_bytes %u", original_chunk_size, c->chunk_cap);
+    if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
+    if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
+    if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
+    const bool records = flags & TSGPU_FLAG_VALIDATE_RECORDS;
+    if (records && (uint64_t)c->max_batch * original_chunk_size > REC_MAX_BATCH)
+        return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch,
+                    original_chunk_size);
+    if ((uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
+        return fail(TSGPU_E_ARG, "object checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
+                    (unsigned long long)c->slot_stride);
+    flags &= ~(ZSTD_MODIFIERS | TSGPU_FLAG_VALIDATE_RECORDS);      // how a frame was compressed does not matter to the reader
+    uint64_t need = 0;
+    for (uint32_t i = 0; i < n_chunks; i++) need += transformed_sizes[i];
+    if (need && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
+    if (need > src_len) return fail(TSGPU_E_SHORT, "Stream has fewer bytes than expected");
+    const ChunkLayout index{original_chunk_size, original_file_size, (original_file_size + original_chunk_size - 1) / original_chunk_size};
+    CheckCarry cur;
+    memcpy(&cur, cursor, sizeof cur);
+    // The index of an empty segment materialises one chunk of 0 transformed bytes: a caller that walks it passes that chunk.
+    uint32_t n = n_chunks;
+    if (index.count == 0 && cur.chunks == 0 && n == 1 && transformed_sizes[0] == 0) n = 0;
+
+    Aes256RoundKeys rk{};
+    if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
+    if (n) {
+        uint64_t in_off = 0;                                     // batches are issued in order: in_off walks src with them
+        const int rc = run_batches(c, n,
+            [&](const Batch& bt) {
+                const int r = check_issue(c, bt, flags, records, src + in_off, transformed_sizes, index, cur.chunks, rk, aad, aad_len);
+                for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
+                return r;
+            },
+            [&](const Batch& bt) { return check_drain(c, bt, flags, records, transformed_sizes, index, cur); });
+        if (rc) return rc;
+        cur.chunks += n;
+        cur.obj_len += need;
+        for (uint32_t i = 0; i < n; i++) cur.seg_len += index.size(cur.chunks - n + i);
+    }
+    if (object_ends_here) {
+        if (cur.chunks != index.count)
+            return fail(TSGPU_E_CORRUPT, "the object has %llu chunks, the chunk index (original chunk size %u, original file size %llu) "
+                        "has %llu", (unsigned long long)cur.chunks, index.ocs, (unsigned long long)index.ofs, (unsigned long long)index.count);
+        if (records) { int rc = records_segment_end(cur.rec); if (rc) return rc; }
+        *object_crc32c = crc_finish(cur.obj_raw, cur.obj_len, 0);
+        *segment_crc32c = crc_finish(cur.seg_raw, cur.seg_len, 0);
+    }
+    memcpy(cursor, &cur, sizeof cur);
+    return TSGPU_OK;
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
 // ------------------------------------------------------------------------------------------ device-resident API
