@@ -60,3 +60,9 @@ tests/cpp/test_check_mirror_simt: tests/cpp/test_check_mirror.cpp $(PKG)/host/ch
 # JNI glue's object-check path (CheckCursor.checkObject) in the window flow of an operator tool, same fake JNIEnv
 tests/cpp/test_jni_check_simt: tests/cpp/test_jni_check.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so
 	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_check.c -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'
+# Host mirror of the object rewrite (RemoteSegmentRewriter, tsgpu_rewrite_object), on the emulator build
+tests/cpp/test_rewrite_mirror_simt: tests/cpp/test_rewrite_mirror.cpp $(PKG)/host/chunk_transform.hpp $(PKG)/host/segment_upload.hpp $(PKG)/host/segment_rewrite.hpp include/tsgpu.h tests/simt/libtsgpu_simt.so
+	g++ -O1 -g -std=c++17 -o $@ tests/cpp/test_rewrite_mirror.cpp -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'
+# JNI glue's object-rewrite path (RewriteCursor.rewriteObject) in the window flow of an operator tool, same fake JNIEnv
+tests/cpp/test_jni_rewrite_simt: tests/cpp/test_jni_rewrite.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so
+	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_rewrite.c -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'

@@ -245,7 +245,8 @@ int tsgpu_detransform(tsgpu_ctx* ctx, uint32_t flags,
  *                  or the object CRC of tsgpu_transform_parts recorded at upload) and *segment_crc32c that of the decoded segment
  *                  (compare with the local segment file before it is deleted).  Neither is written before the end or on failure.
  * Returns the first failure in object order: TSGPU_E_AUTH (a tag), TSGPU_E_CORRUPT (a frame, a Content_Checksum, or a decoded
- * size or chunk count that disagrees with the index; the message names the chunk and both sizes), TSGPU_E_RECORDS (the message
+ * size or chunk count that disagrees with the index; the message names the chunk and both sizes -- a frame that would decode to
+ * more than original_chunk_size bytes is refused as an invalid frame), TSGPU_E_RECORDS (the message
  * names the segment position), TSGPU_E_SHORT (src_len below the sum of transformed_sizes).  Within a batch of chunks, a tag, frame
  * or size failure is reported before the batch's record verdict.  TSGPU_E_ARG as tsgpu_detransform for sizes beyond the
  * context's capacity.  Cost and memory: DESIGN.md §3, §8.
@@ -257,6 +258,61 @@ int tsgpu_check_object(tsgpu_ctx* ctx, uint32_t flags,
                        const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                        tsgpu_check_cursor* cursor, int object_ends_here,
                        uint32_t* object_crc32c, uint32_t* segment_crc32c);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * tsgpu_rewrite_object — a stored .log object rewritten on the GPU under a new data key, or with compression or encryption
+ * added, without its plaintext leaving the GPU: for encryption or compression turned on after the fact, a data key that must be
+ * replaced because it was exposed, or a migration between buckets, regions or providers that copies every object anyway.  Each
+ * window is checked exactly as tsgpu_check_object checks it, then transformed as tsgpu_transform_parts transforms a segment,
+ * batch by batch in HBM; the host sees only the old and the new transformed bytes.
+ *
+ * Source side: from_flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, from_key, from_aad,
+ *   the cursor walk and the empty-segment rule are those of tsgpu_check_object (flags 0 is a plain object; VALIDATE_RECORDS
+ *   checks every record batch).  Every source chunk passes all of that call's checks before any byte of its batch is released.
+ * Target side:
+ *   to_flags       TSGPU_FLAG_ZSTD, ZSTD_DENSE, ZSTD_CHECKSUM, AES and VERIFY; it must contain ZSTD or AES (the plain object is
+ *                  what tsgpu_detransform gives).  Any other bit fails with TSGPU_E_ARG.  New chunk i holds the same original
+ *                  bytes as old chunk i: the chunk size and the file size do not change.
+ *                  When both from_flags and to_flags have ZSTD, every source frame goes into the new object byte for byte (it
+ *                  is still decoded, for the size, record and segment-CRC checks, but not re-encoded: objects the Java plugin
+ *                  wrote are libzstd level 3, denser than this library's speed mode).  ZSTD_DENSE or ZSTD_CHECKSUM then fail with
+ *                  TSGPU_E_ARG, having nothing to act on.  Only a source without ZSTD is compressed, by the selected compressor.
+ *                  The context's TSGPU_ZSTD_MODE=dense and TSGPU_ZSTD_CHECKSUM=1 act where a chunk is compressed, and
+ *                  TSGPU_VERIFY=1 turns on VERIFY, as for tsgpu_transform_parts.
+ *   to_key, to_aad, to_ivs   with AES: the new data key, AAD and one 12-byte IV per chunk of the window.  One GCM key must never
+ *                  encrypt two plaintexts under one IV, so before any GPU work the call fails with TSGPU_E_ARG when two entries of
+ *                  to_ivs are equal, or, with AES on both sides and to_key equal to from_key, when an entry equals the IV of any
+ *                  source chunk of the window (its first 12 bytes).  IVs of other windows are not seen: a caller draws them at
+ *                  random (or never reuses to_key for another object).
+ *   dst, dst_cap, new_transformed_sizes   the window's new chunks back to back and their sizes (n_chunks entries; the empty
+ *                  segment's one empty chunk gets size 0), as tsgpu_transform_parts gives them.
+ *   part_size, part_crc32c, part_cap, n_parts   as tsgpu_transform_parts, with the bound's src_len taken from the chunk index:
+ *                  part_cap >= floor((carried + B) / part_size) + (object_ends_here ? 1 : 0), B = tsgpu_transform_bound(to_flags,
+ *                  L, original_chunk_size) with L the window's original bytes by the index -- or, when the frames are kept, the
+ *                  window's exact new length (its frames, plus 28 bytes each with AES), which is no more for frames within the
+ *                  zstd bound.  A smaller part_cap fails with TSGPU_E_SHORT before any GPU work.  A caller that uploads in one
+ *                  PUT passes a part_size no smaller than the object's bound.
+ *   cursor         192 bytes, zeroed at the start of the object, passed to every window in order; updated on success, without a
+ *                  defined value after a failure.
+ *   object_ends_here  != 0 on the last window (which may be empty): the chunk count must match the index, and then
+ *                  *source_crc32c is the CRC-32C of the old object (compare with the store's checksum of what was read),
+ *                  *object_crc32c that of the new object (FULL_OBJECT) and *segment_crc32c that of the decoded segment (equal
+ *                  to the segment CRC of tsgpu_check_object over either object).  None is written before the end or on failure.
+ * Returns the first failure in object order; within a batch: the source's tag, frame and size (TSGPU_E_AUTH, TSGPU_E_CORRUPT, as
+ * tsgpu_check_object names them), then its records (TSGPU_E_RECORDS), then VERIFY of the new chunks (TSGPU_E_VERIFY).  No byte of
+ * a failing batch reaches dst; earlier batches may already be there.  A failed call writes no CRC.  TSGPU_E_SHORT for a short src
+ * or dst.  Buffers and cost: DESIGN.md §3, §8.
+ * --------------------------------------------------------------------------------------------------------- */
+typedef struct tsgpu_rewrite_cursor { uint64_t opaque[24]; } tsgpu_rewrite_cursor;
+int tsgpu_rewrite_object(tsgpu_ctx* ctx,
+                         uint32_t from_flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes, uint32_t n_chunks,
+                         uint32_t original_chunk_size, uint64_t original_file_size,
+                         const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                         uint32_t to_flags, const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len, const uint8_t* to_ivs,
+                         uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                         uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
+                         tsgpu_rewrite_cursor* cursor, int object_ends_here,
+                         uint32_t* source_crc32c, uint32_t* object_crc32c, uint32_t* segment_crc32c);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Device-resident variants (inputs and outputs already in HBM of device `device_index` of the context; used by

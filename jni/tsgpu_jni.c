@@ -217,3 +217,74 @@ JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_CheckCurs
         (*env)->ReleaseIntArrayElements(env, crcsOut, out, 0);
     }
 }
+
+/* One window of a stored object rewritten under a new key or with compression or encryption added (RewriteCursor.rewriteObject,
+ * tsgpu_rewrite_object): `cursor` a direct ByteBuffer of at least 192 bytes holding the tsgpu_rewrite_cursor (zeros at the start
+ * of the object), updated in place; dst a direct ByteBuffer receiving the window's new chunks, newTransformedSizes their sizes
+ * (one per chunk of the window), partCrcs the CRC-32C of every upload part the window completes (its length is part_cap) and
+ * nPartsOut[0] their count; crcsOut (int[3]) receives, on the object's last window, the CRC-32C of the old object, of the new
+ * object and of the decoded segment.  toIvs: 12 bytes per chunk of the window when toFlags has AES. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RewriteCursor_rewriteObject(
+    JNIEnv* env, jclass c, jlong h, jint fromFlags, jobject src, jlong srcLen, jintArray transformedSizes, jint originalChunkSize,
+    jlong originalFileSize, jbyteArray fromKey, jbyteArray fromAad, jint toFlags, jbyteArray toKey, jbyteArray toAad,
+    jbyteArray toIvs, jobject dst, jlong dstCap, jintArray newTransformedSizes, jlong partSize, jintArray partCrcs,
+    jintArray nPartsOut, jobject cursor, jboolean objectEndsHere, jintArray crcsOut) {
+    jlong ccap = 0;
+    uint8_t* s = srcLen ? direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer") : NULL;
+    if (srcLen && !s) return;
+    uint8_t* d = dstCap ? direct(env, dst, dstCap, NULL, "dst must be a direct ByteBuffer") : NULL;
+    if (dstCap && !d) return;
+    tsgpu_rewrite_cursor* cur = (tsgpu_rewrite_cursor*)direct(env, cursor, 0, &ccap, "rewrite cursor must be a direct ByteBuffer of 192 bytes");
+    if (!cur) return;
+    if (ccap < (jlong)sizeof(tsgpu_rewrite_cursor)) { throw_arg(env, "rewrite cursor must be a direct ByteBuffer of 192 bytes"); return; }
+    if (!transformedSizes) { throw_arg(env, "chunks cannot be null"); return; }
+    const uint32_t n = (uint32_t)(*env)->GetArrayLength(env, transformedSizes);
+    if (!newTransformedSizes || (uint32_t)(*env)->GetArrayLength(env, newTransformedSizes) < n) {
+        throw_arg(env, "newTransformedSizes must hold one int per chunk"); return;
+    }
+    if (!partCrcs) { throw_arg(env, "partCrcs cannot be null"); return; }
+    if (!nPartsOut || (*env)->GetArrayLength(env, nPartsOut) < 1) { throw_arg(env, "nPartsOut must hold 1 int"); return; }
+    if (!crcsOut || (*env)->GetArrayLength(env, crcsOut) < 3) { throw_arg(env, "crcsOut must hold 3 ints"); return; }
+    if (originalChunkSize < 1) { throw_arg(env, "Original chunk size must be positive"); return; }
+    if (originalFileSize < 0) { throw_arg(env, "Original file size must be non-negative"); return; }
+    if (partSize < 1) { throw_arg(env, "partSize must be positive"); return; }
+    if ((fromFlags & TSGPU_FLAG_AES) && fromKey && (*env)->GetArrayLength(env, fromKey) != 32) { throw_arg(env, "data key must be 32 bytes"); return; }
+    if ((toFlags & TSGPU_FLAG_AES) && toKey && (*env)->GetArrayLength(env, toKey) != 32) { throw_arg(env, "data key must be 32 bytes"); return; }
+    if ((toFlags & TSGPU_FLAG_AES) && n && (!toIvs || (uint32_t)(*env)->GetArrayLength(env, toIvs) < 12 * n)) {
+        throw_arg(env, "toIvs must hold 12 bytes per chunk"); return;
+    }
+    jbyte* fk = fromKey ? (*env)->GetByteArrayElements(env, fromKey, NULL) : NULL;
+    jbyte* fa = fromAad ? (*env)->GetByteArrayElements(env, fromAad, NULL) : NULL;
+    jint falen = fromAad ? (*env)->GetArrayLength(env, fromAad) : 0;
+    jbyte* tk = toKey ? (*env)->GetByteArrayElements(env, toKey, NULL) : NULL;
+    jbyte* ta = toAad ? (*env)->GetByteArrayElements(env, toAad, NULL) : NULL;
+    jint talen = toAad ? (*env)->GetArrayLength(env, toAad) : 0;
+    jbyte* iv = toIvs ? (*env)->GetByteArrayElements(env, toIvs, NULL) : NULL;
+    jint* ts = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
+    jint* nts = (*env)->GetIntArrayElements(env, newTransformedSizes, NULL);
+    const uint32_t cap = (uint32_t)(*env)->GetArrayLength(env, partCrcs);
+    jint* pc = (*env)->GetIntArrayElements(env, partCrcs, NULL);
+    uint32_t nParts = 0, crcs[3] = {0, 0, 0};
+    int rc = tsgpu_rewrite_object((tsgpu_ctx*)(intptr_t)h, (uint32_t)fromFlags, s, (uint64_t)srcLen, (const uint32_t*)ts, n,
+                                  (uint32_t)originalChunkSize, (uint64_t)originalFileSize, (const uint8_t*)fk, (const uint8_t*)fa,
+                                  (uint32_t)falen, (uint32_t)toFlags, (const uint8_t*)tk, (const uint8_t*)ta, (uint32_t)talen,
+                                  (const uint8_t*)iv, d, (uint64_t)dstCap, (uint32_t*)nts, (uint64_t)partSize, (uint32_t*)pc, cap,
+                                  &nParts, cur, objectEndsHere ? 1 : 0, &crcs[0], &crcs[1], &crcs[2]);
+    (*env)->ReleaseIntArrayElements(env, transformedSizes, ts, JNI_ABORT);
+    (*env)->ReleaseIntArrayElements(env, newTransformedSizes, nts, rc ? JNI_ABORT : 0);
+    (*env)->ReleaseIntArrayElements(env, partCrcs, pc, rc ? JNI_ABORT : 0);
+    if (fk) (*env)->ReleaseByteArrayElements(env, fromKey, fk, JNI_ABORT);
+    if (fa) (*env)->ReleaseByteArrayElements(env, fromAad, fa, JNI_ABORT);
+    if (tk) (*env)->ReleaseByteArrayElements(env, toKey, tk, JNI_ABORT);
+    if (ta) (*env)->ReleaseByteArrayElements(env, toAad, ta, JNI_ABORT);
+    if (iv) (*env)->ReleaseByteArrayElements(env, toIvs, iv, JNI_ABORT);
+    if (rc) { throw_rt(env, rc); return; }
+    jint* np = (*env)->GetIntArrayElements(env, nPartsOut, NULL);
+    np[0] = (jint)nParts;
+    (*env)->ReleaseIntArrayElements(env, nPartsOut, np, 0);
+    if (objectEndsHere) {
+        jint* out = (*env)->GetIntArrayElements(env, crcsOut, NULL);
+        out[0] = (jint)crcs[0]; out[1] = (jint)crcs[1]; out[2] = (jint)crcs[2];
+        (*env)->ReleaseIntArrayElements(env, crcsOut, out, 0);
+    }
+}

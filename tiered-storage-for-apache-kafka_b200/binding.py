@@ -26,6 +26,7 @@ E_RECORDS = -10
 CURSOR_SIZE = 64         # tsgpu_records_cursor
 PARTS_CURSOR_SIZE = 32   # tsgpu_parts_cursor
 CHECK_CURSOR_SIZE = 128  # tsgpu_check_cursor
+REWRITE_CURSOR_SIZE = 192  # tsgpu_rewrite_cursor
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",
@@ -34,7 +35,7 @@ SYMBOLS = [
     "tsgpu_chunk_sizes_encode", "tsgpu_chunk_sizes_decode", "tsgpu_transformed_chunks_serialize",
     "tsgpu_transformed_chunks_deserialize", "tsgpu_chunk_index_json", "tsgpu_profile_enable", "tsgpu_profile_report",
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
-    "tsgpu_transform_cursor", "tsgpu_transform_parts", "tsgpu_check_object",
+    "tsgpu_transform_cursor", "tsgpu_transform_parts", "tsgpu_check_object", "tsgpu_rewrite_object",
 ]
 
 
@@ -76,6 +77,8 @@ def load(path=None):
     L.tsgpu_transform_chunks.argtypes = [vp, u32, vp, vp, u32, vp, vp, u32, vp, vp, u64, vp]
     L.tsgpu_detransform.argtypes = [vp, u32, vp, u64, vp, u32, vp, vp, u32, vp, u64, vp]
     L.tsgpu_check_object.argtypes = [vp, u32, vp, u64, vp, u32, u32, u64, vp, vp, u32, vp, C.c_int, vp, vp]
+    L.tsgpu_rewrite_object.argtypes = [vp, u32, vp, u64, vp, u32, u32, u64, vp, vp, u32, u32, vp, vp, u32, vp, vp, u64, vp,
+                                       u64, vp, u32, vp, vp, C.c_int, vp, vp, vp]
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
     L.tsgpu_detransform_device.argtypes = [vp, C.c_int, u32, vp, u64, vp, u32, u32, vp, vp, u32, vp, vp, vp, vp]
     L.tsgpu_launch_count.restype = u64
@@ -268,6 +271,41 @@ class Context:
                                                 original_file_size, _p(k), _p(a), a.size, cursor.ctypes.data,
                                                 1 if object_ends_here else 0, C.addressof(obj), C.addressof(seg)))
         return (int(obj.value), int(seg.value)) if object_ends_here else None
+
+    def rewrite_object(self, from_flags, src, transformed_sizes, original_chunk_size, original_file_size, to_flags, part_size,
+                       cursor=None, object_ends_here=True, from_key=None, from_aad=b"", to_key=None, to_aad=b"", to_ivs=None,
+                       part_cap=None):
+        """Rewrites one window of a stored object on the GPU (tsgpu_rewrite_object): checked as check_object checks it, then
+        transformed with `to_flags` under `to_key` / `to_ivs` (one 12-byte IV per chunk of the window).  `cursor`: a 192-byte
+        np.uint8 array (zeros at the start of the object), updated in place on success; None rewrites a whole object.  Returns
+        (new bytes, [new transformed sizes], [CRC-32C of the parts this call completed], (source, object, segment) CRC-32C or None
+        when the object does not end here)."""
+        s = _u8(src)
+        if cursor is None:
+            cursor = np.zeros(REWRITE_CURSOR_SIZE, np.uint8)
+        if not (isinstance(cursor, np.ndarray) and cursor.dtype == np.uint8 and cursor.size == REWRITE_CURSOR_SIZE
+                and cursor.flags.c_contiguous):
+            raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % REWRITE_CURSOR_SIZE)
+        ts = np.ascontiguousarray(transformed_sizes, dtype=np.uint32)
+        n = ts.size
+        # every chunk of the window at most a frame bound (or its source frame, when frames are kept) plus IV and tag
+        per = int(self.lib.tsgpu_transform_bound(to_flags | FLAG_ZSTD, original_chunk_size, original_chunk_size)) + 28
+        cap = max(n * per, int(ts.sum(dtype=np.uint64)) + 28 * n) + 64
+        dst = np.empty(cap, dtype=np.uint8)
+        sizes = np.zeros(max(n, 1), dtype=np.uint32)
+        if part_cap is None:
+            part_cap = (cap + part_size) // max(part_size, 1) + 1
+        crcs = np.zeros(max(part_cap, 1), dtype=np.uint32)
+        n_parts, src_crc, obj_crc, seg_crc = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        fk, fa, tk, ta, iv = _u8(from_key), _u8(from_aad), _u8(to_key), _u8(to_aad), _u8(to_ivs)
+        self._check(self.lib.tsgpu_rewrite_object(
+            self._h, from_flags, _p(s), s.size, _p(ts), n, original_chunk_size, original_file_size, _p(fk), _p(fa), fa.size,
+            to_flags, _p(tk), _p(ta), ta.size, _p(iv), dst.ctypes.data, dst.size, sizes.ctypes.data, part_size,
+            crcs.ctypes.data, part_cap, C.addressof(n_parts), cursor.ctypes.data, 1 if object_ends_here else 0,
+            C.addressof(src_crc), C.addressof(obj_crc), C.addressof(seg_crc)))
+        sizes = sizes[:n]
+        crc3 = (int(src_crc.value), int(obj_crc.value), int(seg_crc.value)) if object_ends_here else None
+        return dst[:int(sizes.sum(dtype=np.uint64))], [int(x) for x in sizes], [int(x) for x in crcs[:n_parts.value]], crc3
 
     # ---- device-resident API (raw device pointers as ints; bench.py passes torch data_ptr()) ----
     def slot_stride(self, flags, chunk_size):

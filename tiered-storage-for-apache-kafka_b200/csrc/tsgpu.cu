@@ -11,6 +11,8 @@
 //   TSGPU_FLAG_VALIDATE_RECORDS the Kafka log entries of each batch are checked on the device (records.cuh) and the batch's
 //   verdict is resolved, in batch order, before its bytes are copied out.  tsgpu_transform_parts also hashes each packed batch
 //   (part_crc.cuh) and combines the CRC-32C of the object's upload parts on the host once the call's streams are idle.
+#include <algorithm>
+#include <array>
 #include <condition_variable>
 #include <mutex>
 #include <new>
@@ -89,6 +91,16 @@ struct PcrcScratch {
     int32_t pending = -1;          // the call's batch whose prefixes h_cuts receives (collected at the slot's next drain or at the end)
 };
 
+// One AES-GCM key of a slot: the key tables (H powers, Shoup table) of the last key it ran, so consecutive calls with one
+// segment's data key skip the set-up kernel, and the AAD the GCM kernels read.
+struct GcmKeys {
+    Aes256RoundKeys rk{};          // the key `ctx` was built for
+    bool valid = false;
+    GcmKeyCtx* ctx = nullptr;
+    uint8_t* d_aad = nullptr;      // [0]: the descriptor block's; [1]: its own MAX_AAD bytes, uploaded from h_aad (pinned)
+    uint8_t* h_aad = nullptr;
+};
+
 struct Work {
     int device = 0;
     rt::stream_t stream{}, out_stream{};   // out_stream: copies of finished chunks back to the host
@@ -98,8 +110,7 @@ struct Work {
     bool out_pending = false;              // a copy-out on out_stream still reads this slot's final buffer
     bool ready = false;
     bool claimed = false;                  // owned by a call in progress (guarded by tsgpu_ctx::mu)
-    Aes256RoundKeys key_rk{};      // the key this slot's GcmKeyCtx (H powers, Shoup table) was built for
-    bool key_valid = false;        //   ... consecutive calls with one segment's data key skip the set-up kernel
+    GcmKeys keys[2];               // [0] every call's; [1] the new key of tsgpu_rewrite_object (allocated on first use)
     uint8_t* d_orig = nullptr;     // max_batch * chunk_cap
     uint8_t* d_frames = nullptr;   // max_batch * frame_stride        (zstd frames, 16-byte aligned slots)
     uint8_t* d_xf = nullptr;       // max_batch * slot_stride         (transformed slots)
@@ -107,7 +118,6 @@ struct Work {
     uint8_t* d_desc = nullptr;  uint8_t* h_desc = nullptr;  size_t desc_bytes = 0;
     Desc dd{}, hd{};               // device / pinned-host views of the descriptor block
     uint4* d_partials = nullptr;  uint32_t max_ranges = 0;
-    GcmKeyCtx* d_keyctx = nullptr;
     ZstdEncScratch zenc{};         // region kernel (TSGPU_FLAG_ZSTD_DENSE), allocated on first use
     ZstdBlkScratch zblk{};         // block kernel (default), allocated on first use
     ZstdDecScratch zdec{};
@@ -177,8 +187,9 @@ static int work_init_impl(tsgpu_ctx* c, Work& w, int device) {
     carve_desc(w.h_desc, c->max_batch, w.hd, nullptr);
     w.max_ranges = (uint32_t)((frame_bound(c->chunk_cap) / 16 + GH_RANGE_BLOCKS) / GH_RANGE_BLOCKS) + 1;
     RT(rt::malloc_device((void**)&w.d_partials, sizeof(uint4) * (size_t)w.max_ranges * nb));
-    RT(rt::malloc_device((void**)&w.d_keyctx, sizeof(GcmKeyCtx)));
-    RT(rt::malloc_host((void**)&w.h_sizes, 4ull * nb * 3 + 64));
+    RT(rt::malloc_device((void**)&w.keys[0].ctx, sizeof(GcmKeyCtx)));
+    w.keys[0].d_aad = w.dd.aad;
+    RT(rt::malloc_host((void**)&w.h_sizes, 4ull * nb * 5 + 64));
     const char* e = zstd_dec_scratch_alloc(w.zdec, c->chunk_cap, c->max_batch);
     if (e) return fail(TSGPU_E_CUDA, "zstd dec scratch: %s", e);
     return TSGPU_OK;
@@ -191,11 +202,12 @@ static void work_free(Work& w) {
     if (w.out_stream) rt::stream_sync(w.out_stream);
     rt::free_device(w.d_orig); rt::free_device(w.d_frames); rt::free_device(w.d_xf); rt::free_device(w.d_pack);
     rt::free_device(w.d_desc); rt::free_host(w.h_desc);
-    rt::free_device(w.d_partials); rt::free_device(w.d_keyctx); rt::free_host(w.h_sizes);
+    rt::free_device(w.d_partials); rt::free_device(w.keys[0].ctx); rt::free_host(w.h_sizes);
+    rt::free_device(w.keys[1].ctx); rt::free_device(w.keys[1].d_aad); rt::free_host(w.keys[1].h_aad);
     zstd_enc_scratch_free(w.zenc); zstd_blk_scratch_free(w.zblk); zstd_dec_scratch_free(w.zdec);
     rt::free_device(w.rec.d); rt::free_device(w.rec.d_out); rt::free_host(w.rec.h_out); w.rec = RecScratch{};
     rt::free_device(w.pcrc.d); rt::free_device(w.pcrc.d_cuts); rt::free_host(w.pcrc.h_cuts); w.pcrc = PcrcScratch{};
-    memset(&w.key_rk, 0, sizeof w.key_rk); w.key_valid = false;
+    for (GcmKeys& k : w.keys) k = GcmKeys{};                // forgets the keys too
     rt::event_destroy(w.ev_sizes); rt::event_destroy(w.ev_done);
     rt::event_destroy(w.ev_dev_desc); rt::event_destroy(w.ev_dev_done);
     rt::stream_destroy(w.stream); rt::stream_destroy(w.out_stream);
@@ -314,35 +326,36 @@ static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, Ch
     return TSGPU_OK;
 }
 
-// AES-GCM: key set-up, the main kernel over (ranges x chunks) and the finalize kernel.  IVs (ENC) and AAD come from the
-// slot's descriptor block.  The slot keeps the key tables of the last key it ran: consecutive calls with one segment's data
-// key skip the set-up kernel.  Host and device calls share slot 0's tables; that is safe because device calls are ordered
-// behind each other by events (dev_call_begin) and a host call takes the slot only once device work on it has completed.
+// AES-GCM: key set-up, the main kernel over (ranges x chunks) and the finalize kernel.  IVs (ENC) come from the slot's
+// descriptor block, the AAD from `k`.  The slot keeps the key tables of the last key each of its GcmKeys ran: consecutive calls
+// with one segment's data key skip the set-up kernel.  Host and device calls share slot 0's tables; that is safe because device
+// calls are ordered behind each other by events (dev_call_begin) and a host call takes the slot only once device work on it has
+// completed.
 template <bool ENC>
-static int gcm_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Aes256RoundKeys& rk, ChunksIn in, ChunksOut out,
+static int gcm_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, const Aes256RoundKeys& rk, ChunksIn in, ChunksOut out,
                      uint32_t aad_len, uint32_t* d_status, uint32_t n_chunks, uint32_t max_payload, uint32_t out_cap) {
-    const bool key_ready = w.key_valid && memcmp(&w.key_rk, &rk, sizeof rk) == 0;
-    w.key_rk = rk; w.key_valid = false;                      // valid again once the whole stage has been enqueued
+    const bool key_ready = k.valid && memcmp(&k.rk, &rk, sizeof rk) == 0;
+    k.rk = rk; k.valid = false;                              // valid again once the whole stage has been enqueued
     if (!key_ready) {
-        TS_LAUNCH_P(c->prof, "gcm_key_setup", gcm_key_setup_kernel, dim3(1), dim3(GH_T), 0, st, rk, w.d_keyctx);
+        TS_LAUNCH_P(c->prof, "gcm_key_setup", gcm_key_setup_kernel, dim3(1), dim3(GH_T), 0, st, rk, k.ctx);
         CHECK_LAUNCH("gcm_key_setup_kernel");
     }
     GcmBatch B;
     B.in_base = in.base; B.in_off = in.off; B.in_len = in.len;
     B.out_base = out.base; B.out_off = out.off; B.out_len = out.len;
-    B.ivs = ENC ? w.dd.ivs : nullptr; B.aad = w.dd.aad; B.aad_len = aad_len;
+    B.ivs = ENC ? w.dd.ivs : nullptr; B.aad = k.d_aad; B.aad_len = aad_len;
     B.partials = w.d_partials; B.max_ranges = w.max_ranges; B.status = d_status; B.n_chunks = n_chunks; B.out_cap = out_cap;
     uint32_t ranges = (uint32_t)(((uint64_t)max_payload + 15) / 16 + GH_RANGE_BLOCKS - 1) / GH_RANGE_BLOCKS;
     if (ranges > w.max_ranges) return fail(TSGPU_E_ARG, "chunk too large for this context");
     if (ranges) {
         TS_LAUNCH_P(c->prof, ENC ? "gcm_main_enc" : "gcm_main_dec", gcm_main_kernel<ENC>, dim3(ranges, n_chunks), dim3(GH_T),
-                    GCM_SMEM_BYTES, st, rk, w.d_keyctx, B);
+                    GCM_SMEM_BYTES, st, rk, k.ctx, B);
         CHECK_LAUNCH("gcm_main_kernel");
     }
     TS_LAUNCH_P(c->prof, ENC ? "gcm_finalize_enc" : "gcm_finalize_dec", gcm_finalize_kernel<ENC>, dim3((n_chunks + 3) / 4),
-                dim3(128), 0, st, rk, w.d_keyctx, B);
+                dim3(128), 0, st, rk, k.ctx, B);
     CHECK_LAUNCH("gcm_finalize_kernel");
-    w.key_valid = true;
+    k.valid = true;
     return TSGPU_OK;
 }
 
@@ -358,7 +371,7 @@ static int wait_copies_out(Work& w, rt::stream_t st) {
 // Between the two stages the chunks sit in the slot's frame buffer (16-byte aligned slots of frame_stride).
 
 // [zstd ->] [AES-GCM encrypt]: nb chunks of at most cs bytes from `src` into `dst`.
-static int transform_enqueue(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, uint32_t nb, uint32_t cs,
+static int transform_enqueue(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, uint32_t nb, uint32_t cs,
                              const Aes256RoundKeys& rk, uint32_t aad_len, ChunksIn src, ChunksOut dst) {
     const bool aes = flags & TSGPU_FLAG_AES;
     uint32_t max_payload = cs;
@@ -368,19 +381,19 @@ static int transform_enqueue(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t fl
         if (rc) return rc;
         src = frames; max_payload = (uint32_t)frame_bound(cs);
     }
-    if (aes) return gcm_stage<true>(c, w, st, rk, src, dst, aad_len, w.dd.status, nb, max_payload, 0xffffffffu);
+    if (aes) return gcm_stage<true>(c, w, k, st, rk, src, dst, aad_len, w.dd.status, nb, max_payload, 0xffffffffu);
     return TSGPU_OK;
 }
 
 // [AES-GCM decrypt ->] [zstd]: nb chunks from `src` into `dst`.  packed: dst.off is written on the device as the running sum
 // of the original sizes (chunks back to back) instead of being read as given.
-static int detransform_enqueue(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, uint32_t nb, const Aes256RoundKeys& rk,
+static int detransform_enqueue(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, uint32_t nb, const Aes256RoundKeys& rk,
                                uint32_t aad_len, ChunksIn src, ChunksOut dst, uint32_t* d_status, const DxBounds& lim, bool packed) {
     const bool zstd = flags & TSGPU_FLAG_ZSTD;
     if (flags & TSGPU_FLAG_AES) {
         const ChunksOut plain = zstd ? ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len} : dst;
         if (!zstd) { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }                        // dst is the final buffer
-        int rc = gcm_stage<false>(c, w, st, rk, src, plain, aad_len, d_status, nb, lim.max_in, lim.aes_room);
+        int rc = gcm_stage<false>(c, w, k, st, rk, src, plain, aad_len, d_status, nb, lim.max_in, lim.aes_room);
         if (rc) return rc;
         src = plain;
     }
@@ -525,18 +538,19 @@ static int copy_out(Work& w, const uint8_t* from, uint64_t total, uint8_t* dst, 
 // d_frames and decodes that into d_xf; A decrypts d_xf into d_frames; Z decodes d_frames into d_xf.  The read-back chunk i
 // lands at b_off[i] (a 16-byte aligned frame slot; d_xf's slots are larger) with its size in v_len, so a_len survives.
 // Leaves per chunk: status 0 / 1 tag / 2 frame / VERIFY_ST_SIZE, and v_diff = first differing byte or VERIFY_NO_DIFF.
-static int verify_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, uint32_t nb, uint32_t cs,
+// `payload`: the largest transformed chunk without IV and tag.
+static int verify_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, uint32_t nb, uint32_t cs, uint64_t payload,
                         const Aes256RoundKeys& rk, uint32_t aad_len, ChunksOut fin) {
     const bool zstd = flags & TSGPU_FLAG_ZSTD;
     RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
     RT(rt::memset_async(w.dd.v_diff, 0xff, 4ull * nb, st));
     DxBounds lim;
-    lim.max_in = (uint32_t)((zstd ? frame_bound(cs) : cs) + TSGPU_IV_SIZE + TSGPU_TAG_SIZE);
+    lim.max_in = (uint32_t)(payload + TSGPU_IV_SIZE + TSGPU_TAG_SIZE);
     lim.aes_room = zstd ? (uint32_t)(c->frame_stride - 16) : c->chunk_cap;
     lim.zstd_in = (uint32_t)(c->frame_stride - 16);
     lim.zstd_out = cs;                                        // a frame claiming more than the batch's largest chunk is wrong
     const ChunksOut back{zstd ? w.d_xf : w.d_frames, w.dd.b_off, w.dd.v_len};
-    { int rc = detransform_enqueue(c, w, st, flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES), nb, rk, aad_len, fin, back, w.dd.status,
+    { int rc = detransform_enqueue(c, w, k, st, flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES), nb, rk, aad_len, fin, back, w.dd.status,
                                    lim, /*packed=*/false); if (rc) return rc; }
     VerifyArgs V;
     V.orig = w.d_orig; V.orig_off = w.dd.a_off; V.orig_len = w.dd.a_len;
@@ -743,8 +757,54 @@ static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
 }
 #endif
 
-// One batch: copy in, fill the descriptors, enqueue the stages, pack the transformed chunks, [verify them,] D2H of their
-// sizes (and of the verify stage's verdicts).
+// The target half of a batch whose original chunks are `orig` in d_orig (each at most cs bytes): [zstd ->] [AES-GCM encrypt]
+// with the keys `k`, or with `kept` the batch's frames in the d_frames slots (b_off, b_len; frames_max bytes at most) as they are
+// [-> AES-GCM encrypt]; the transformed chunks packed into d_pack, [pcrc_tiles over them,] [the verify stage and the D2H of its
+// verdicts to h_sizes + nb.]  `fin` receives the transformed chunks in their slots.
+static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, bool verify, bool parts, uint32_t c0,
+                        uint32_t nb, uint32_t cs, const Aes256RoundKeys& rk, uint32_t aad_len, ChunksIn orig, bool kept,
+                        uint64_t frames_max, ChunksOut& fin) {
+    const bool aes = flags & TSGPU_FLAG_AES;
+    // encrypted chunks land in the transformed slots; zstd alone leaves its frames in the frame slots
+    fin = aes ? ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len} : ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len};
+    uint64_t payload;                        // the largest transformed chunk without IV and tag
+    if (kept) {
+        payload = frames_max;
+        if (aes) {
+            int rc = gcm_stage<true>(c, w, k, st, rk, ChunksIn{w.d_frames, w.dd.b_off, w.dd.b_len}, fin, aad_len, w.dd.status, nb,
+                                     (uint32_t)payload, 0xffffffffu);
+            if (rc) return rc;
+        }
+    } else {
+        payload = (flags & TSGPU_FLAG_ZSTD) ? frame_bound(cs) : cs;
+        int rc = transform_enqueue(c, w, k, st, flags, nb, cs, rk, aad_len, orig, fin);
+        if (rc) return rc;
+    }
+#ifdef TSGPU_SIMT
+    simt_inject_fault(fin, c0, nb);
+#endif
+    // the transformed chunks, back to back, so the batch leaves in one copy (the previous batch's copy-out may still be
+    // reading d_pack: this is the first kernel of the batch that has to wait for it)
+    { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
+    {
+        PackArgs P;
+        P.base = fin.base; P.stride = aes ? c->slot_stride : c->frame_stride; P.head = aes ? TSGPU_SLOT_HEAD : 0;
+        P.len = fin.len; P.n = nb; P.out = w.d_pack;
+        const uint64_t longest = payload + 28;
+        TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
+        CHECK_LAUNCH("pack_chunks_kernel");
+        if (parts) { int rc = parts_stage(c, w, st, fin.len, nb, longest * nb); if (rc) return rc; }
+    }
+    if (verify) {
+        int rc = verify_stage(c, w, k, st, flags, nb, cs, payload, rk, aad_len, fin);
+        if (rc) return rc;
+        RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.h_sizes + 2 * nb, w.dd.v_diff, 4ull * nb, st));
+    }
+    return TSGPU_OK;
+}
+
+// One batch: copy in, fill the descriptors, the target half, [the record kernels,] D2H of the transformed sizes.
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
 static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, bool parts, const uint8_t* src, const uint64_t* off,
                            const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
@@ -763,36 +823,14 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool v
         w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
         w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
     }
-    const bool aes = flags & TSGPU_FLAG_AES;
-    if (aes) {
+    if (flags & TSGPU_FLAG_AES) {
         memcpy(w.hd.ivs, ivs + (size_t)c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
         if (aad_len) memcpy(w.hd.aad, aad, aad_len);
     }
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
-    // encrypted chunks land in the transformed slots; zstd alone leaves its frames in the frame slots
-    const ChunksOut fin = aes ? ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len} : ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len};
-    { int rc = transform_enqueue(c, w, st, flags, nb, cs, rk, aad_len, ChunksIn{w.d_orig, w.dd.a_off, w.dd.a_len}, fin); if (rc) return rc; }
-#ifdef TSGPU_SIMT
-    simt_inject_fault(fin, c0, nb);
-#endif
-    // the transformed chunks, back to back, so the batch leaves in one copy (the previous batch's copy-out may still be
-    // reading d_pack: this is the first kernel of the batch that has to wait for it)
-    { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
-    {
-        PackArgs P;
-        P.base = fin.base; P.stride = aes ? c->slot_stride : c->frame_stride; P.head = aes ? TSGPU_SLOT_HEAD : 0;
-        P.len = fin.len; P.n = nb; P.out = w.d_pack;
-        const uint64_t longest = (flags & TSGPU_FLAG_ZSTD) ? frame_bound(cs) + 28 : (uint64_t)cs + 28;
-        TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
-        CHECK_LAUNCH("pack_chunks_kernel");
-        if (parts) { int rc = parts_stage(c, w, st, fin.len, nb, longest * nb); if (rc) return rc; }
-    }
-    if (verify) {
-        int rc = verify_stage(c, w, st, flags, nb, cs, rk, aad_len, fin);
-        if (rc) return rc;
-        RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
-        RT(rt::d2h(w.h_sizes + 2 * nb, w.dd.v_diff, 4ull * nb, st));
-    }
+    ChunksOut fin;
+    { int rc = target_stage(c, w, w.keys[0], st, flags, verify, parts, c0, nb, cs, rk, aad_len, ChunksIn{w.d_orig, w.dd.a_off, w.dd.a_len},
+                            /*kept=*/false, 0, fin); if (rc) return rc; }
     if (records) {
         int rc = records_alloc(w.rec, (uint64_t)c->max_batch * cs);
         if (!rc) rc = records_stage(c, w, st, byte1 - byte0);
@@ -804,18 +842,19 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool v
 }
 
 // The verify stage's verdict on a drained batch (h_sizes: sizes, status, first differing bytes); TSGPU_OK if every chunk
-// read back.  `len`: the original chunk sizes of the call.
-static int verify_verdict(const Batch& bt, const uint32_t* len) {
+// read back.  `len`: the original chunk sizes of the call; `first`: the number the call's first chunk has in the messages.
+static int verify_verdict(const Batch& bt, const uint32_t* len, uint64_t first = 0) {
     const uint32_t* status = bt.w->h_sizes + bt.nb;
     const uint32_t* diff = bt.w->h_sizes + 2 * bt.nb;
     for (uint32_t i = 0; i < bt.nb; i++) {
         const uint32_t k = bt.c0 + i;
-        if (status[i] == 1) return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: tag check failed", k);
+        const unsigned long long g = first + k;
+        if (status[i] == 1) return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: tag check failed", g);
         if (status[i] == VERIFY_ST_SIZE)
-            return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: size check failed (original %u bytes)", k, len[k]);
-        if (status[i] != 0) return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: frame check failed (code %u)", k, status[i]);
+            return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: size check failed (original %u bytes)", g, len[k]);
+        if (status[i] != 0) return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: frame check failed (code %u)", g, status[i]);
         if (diff[i] != VERIFY_NO_DIFF)
-            return fail(TSGPU_E_VERIFY, "verify: chunk %u did not read back: bytes differ from offset %u", k, diff[i]);
+            return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: bytes differ from offset %u", g, diff[i]);
     }
     return TSGPU_OK;
 }
@@ -1038,9 +1077,9 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
 // ------------------------------------------------------------------------------------------ detransform (host)
 // A batch's transformed chunks into the slot's d_xf, one per slot at i * slot_stride + TSGPU_SLOT_HEAD (16-byte aligned ciphertext
 // for the GCM kernel), and the descriptor block filled for detransform_enqueue (not yet uploaded).  Returns the bounds of the stages.
-// `src`: the batch's first transformed chunk.
+// `src`: the batch's first transformed chunk.  to_frames (zstd only): the frames go to the d_frames slots (b_off, b_len) instead.
 static int dx_load(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
-                   const uint8_t* aad, uint32_t aad_len, DxBounds& lim) {
+                   const uint8_t* aad, uint32_t aad_len, DxBounds& lim, bool to_frames = false) {
     const uint32_t c0 = bt.c0, nb = bt.nb;
     // Sizes come from a manifest, i.e. from outside: bound them per mode BEFORE any kernel writes (the GCM kernel
     // releases plaintext into the next buffer before the tag is checked).  AES only: plaintext lands in d_orig
@@ -1056,8 +1095,9 @@ static int dx_load(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, uint
         w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
         w.hd.c_len[i] = t;
         w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
+        w.hd.b_len[i] = (uint32_t)payload;               // what the GCM stage writes there (AES), or the frame (to_frames)
         w.hd.a_off[i] = op;                              // used when there is no zstd stage (sizes are known)
-        if (t) RT(rt::h2d(w.d_xf + w.hd.c_off[i], src + ip, t, st));
+        if (t) RT(rt::h2d((to_frames ? w.d_frames + w.hd.b_off[i] : w.d_xf + w.hd.c_off[i]), src + ip, t, st));
         ip += t;
         op += payload;
         max_t = std::max(max_t, t);
@@ -1078,7 +1118,7 @@ static int detransform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, cons
     { int rc = dx_load(c, w, st, bt, flags, src, tsizes, aad, aad_len, lim); if (rc) return rc; }
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
     RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
-    { int rc = detransform_enqueue(c, w, st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
+    { int rc = detransform_enqueue(c, w, w.keys[0], st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
                                    ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len}, w.dd.status, lim, /*packed=*/true); if (rc) return rc; }
     RT(rt::d2h(w.h_sizes, w.dd.a_len, 4ull * nb, st));
     RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
@@ -1142,11 +1182,12 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
 // ------------------------------------------------------------------------------------------ object check (host)
-// tsgpu_check_object: the detransform of a stored object with nothing copied out.  Per batch, on the compute stream: the
-// transformed chunks into d_xf (flags 0: the plain chunks straight into d_orig), pcrc over them in their slots (the object
-// word), the detransform stages into d_orig packed, pcrc over d_orig (the segment word), [the record kernels,] and one D2H each
-// of the decoded sizes, the statuses and the two words.  At the drain, in object order: tag and frame statuses, decoded sizes
-// against the chunk index, the record verdict, then the words extend the cursor's CRCs.
+// tsgpu_check_object: the detransform of a stored object with nothing copied out.  Per batch, on the compute stream, the source
+// half (source_stage): the transformed chunks into d_xf (flags 0: the plain chunks straight into d_orig), pcrc over them where
+// they sit (the object word), the detransform stages into d_orig at the chunk index's offsets, pcrc over d_orig by the index's
+// sizes (the segment word), [the record kernels,] and one D2H each of the decoded sizes, the statuses and the two words.  At the
+// drain (source_drain), in object order: tag and frame statuses, decoded sizes against the chunk index, the record verdict, then
+// the words extend the cursor's CRCs.
 
 // The state of an object between calls: the public tsgpu_check_cursor (128 bytes, zero = start of the object).
 struct CheckCarry {
@@ -1166,6 +1207,52 @@ struct ChunkLayout {
     uint32_t ocs; uint64_t ofs, count;
     uint32_t size(uint64_t g) const { return g + 1 < count ? ocs : g + 1 == count ? (uint32_t)(ofs - g * ocs) : 0u; }
 };
+
+// One window of a stored object, its arguments checked (source_args).
+struct SourceReq {
+    uint32_t flags;                  // ZSTD and AES of the object (0: plain)
+    bool records;                    // TSGPU_FLAG_VALIDATE_RECORDS
+    const uint8_t* src; const uint32_t* tsizes;
+    uint32_t n;                      // chunks of the window (the empty segment's one empty chunk is not one)
+    uint64_t need;                   // bytes of the window
+    ChunkLayout index;
+    Aes256RoundKeys rk;
+    const uint8_t* aad; uint32_t aad_len;
+};
+
+static int source_args(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                       uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size, const uint8_t* key,
+                       const uint8_t* aad, uint32_t aad_len, const CheckCarry& cur, SourceReq& q) {
+    if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VALIDATE_RECORDS)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
+    if (n_chunks && !transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
+    if (original_chunk_size == 0) return fail(TSGPU_E_ARG, "Original chunk size must be positive, 0 given");
+    if (original_chunk_size > c->chunk_cap)
+        return fail(TSGPU_E_ARG, "original chunk size %u exceeds the context's max_chunk_bytes %u", original_chunk_size, c->chunk_cap);
+    if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
+    if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
+    if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
+    q.records = flags & TSGPU_FLAG_VALIDATE_RECORDS;
+    if (q.records && (uint64_t)c->max_batch * original_chunk_size > REC_MAX_BATCH)
+        return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch,
+                    original_chunk_size);
+    if ((uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
+        return fail(TSGPU_E_ARG, "object checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
+                    (unsigned long long)c->slot_stride);
+    q.flags = flags & ~(ZSTD_MODIFIERS | TSGPU_FLAG_VALIDATE_RECORDS);   // how a frame was compressed does not matter to the reader
+    q.need = 0;
+    for (uint32_t i = 0; i < n_chunks; i++) q.need += transformed_sizes[i];
+    if (q.need && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
+    if (q.need > src_len) return fail(TSGPU_E_SHORT, "Stream has fewer bytes than expected");
+    q.src = src; q.tsizes = transformed_sizes;
+    q.index = ChunkLayout{original_chunk_size, original_file_size, (original_file_size + original_chunk_size - 1) / original_chunk_size};
+    // The index of an empty segment materialises one chunk of 0 transformed bytes: a caller that walks it passes that chunk.
+    q.n = n_chunks;
+    if (q.index.count == 0 && cur.chunks == 0 && q.n == 1 && transformed_sizes[0] == 0) q.n = 0;
+    q.rk = Aes256RoundKeys{};
+    if (q.flags & TSGPU_FLAG_AES) q.rk = aes256_expand_key(key);
+    q.aad = aad; q.aad_len = aad_len;
+    return TSGPU_OK;
+}
 
 // The raw CRC-32C of a batch's L bytes into pcrc.d_cuts[k]: pcrc_tiles, then pcrc_cuts without part boundaries.
 template <bool SLOTS>
@@ -1191,64 +1278,74 @@ static int check_crc_word(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint8_t*
     return TSGPU_OK;
 }
 
-// One batch of a check.  `src`: the batch's first transformed chunk; `g0`: the object's chunk number of the call's first chunk.
-// h_sizes receives the decoded sizes, the statuses and the object and segment words.
-static int check_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool records, const uint8_t* src, const uint32_t* tsizes,
-                       const ChunkLayout& index, uint64_t g0, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len) {
-    Work& w = *bt.w;
-    const uint32_t nb = bt.nb;
-    RT(rt::set_device(w.device));
-    rt::stream_t st = w.stream;
+// The source half of one batch.  `src`: the batch's first transformed chunk; `g0`: the object's chunk number of the call's first
+// chunk.  A zstd-only object's frames go to the d_frames slots with to_frames, else in place in d_xf.  Chunk i decodes to
+// d_orig + a_off[i], the offset the chunk index gives it, and v_len[i] holds its size by the index: what later stages read, so a
+// damaged chunk cannot steer them (its batch fails at the drain).  The descriptor block is uploaded here: a caller fills its
+// other fields first.  out[0, nb) receives the decoded sizes, out[nb, 2 nb) the statuses, out[2 nb, 2 nb + 2) the object and
+// segment words.
+static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, const SourceReq& q, const uint8_t* src, uint64_t g0,
+                        bool to_frames, uint32_t* out) {
+    const uint32_t nb = bt.nb, flags = q.flags;
     uint64_t L = 0, obj = 0;                 // the batch's length by the chunk index (what it decodes to when it is sound)
     for (uint32_t i = 0; i < nb; i++) {
-        w.hd.v_len[i] = index.size(g0 + bt.c0 + i);
+        w.hd.v_len[i] = q.index.size(g0 + bt.c0 + i);
         L += w.hd.v_len[i];
-        obj += tsizes[bt.c0 + i];
+        obj += q.tsizes[bt.c0 + i];
     }
     DxBounds lim{};
     if (flags) {
-        int rc = dx_load(c, w, st, bt, flags, src, tsizes, aad, aad_len, lim);
+        int rc = dx_load(c, w, st, bt, flags, src, q.tsizes, q.aad, q.aad_len, lim, to_frames);
         if (rc) return rc;
+        // Chunk i decodes to a_off[i] = i * ocs: a frame may not write past ocs bytes, or it would overwrite the next chunk's
+        // region while that one decodes (and reads its own output back).  A larger frame is refused as an invalid frame.
+        lim.zstd_out = q.index.ocs;
     } else {                                 // a plain object is the segment: its chunks go to d_orig back to back
         for (uint32_t i = 0; i < nb; i++) {
-            if (tsizes[bt.c0 + i] > c->chunk_cap)
-                return fail(TSGPU_E_ARG, "transformed chunk of %u bytes exceeds the context's capacity", tsizes[bt.c0 + i]);
-            w.h_sizes[i] = tsizes[bt.c0 + i];
-            w.h_sizes[nb + i] = 0;
+            if (q.tsizes[bt.c0 + i] > c->chunk_cap)
+                return fail(TSGPU_E_ARG, "transformed chunk of %u bytes exceeds the context's capacity", q.tsizes[bt.c0 + i]);
+            out[i] = w.hd.a_len[i] = q.tsizes[bt.c0 + i];         // a_len: the decoded sizes, as the stages write them
+            out[nb + i] = 0;
+            w.hd.b_off[i] = (uint64_t)i * c->frame_stride;      // the slots a target half writes
+            w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
         }
         if (obj) RT(rt::h2d(w.d_orig, src, obj, st));
     }
+    for (uint64_t i = 0, a = 0; i < nb; a += w.hd.v_len[i++]) w.hd.a_off[i] = a;
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
+    // the slot's previous batch may still be copying out, its part prefixes read from the pcrc scratch this batch rewrites
+    { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
     if (flags) {
-        { int rc = check_crc_word<true>(c, w, st, w.d_xf, w.dd.c_off, w.dd.c_len, nb, obj, 0); if (rc) return rc; }
+        const ChunksIn in = to_frames ? ChunksIn{w.d_frames, w.dd.b_off, w.dd.b_len} : ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len};
+        { int rc = check_crc_word<true>(c, w, st, in.base, in.off, in.len, nb, obj, 0); if (rc) return rc; }
         RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
-        int rc = detransform_enqueue(c, w, st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
-                                     ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len}, w.dd.status, lim, /*packed=*/true);
+        int rc = detransform_enqueue(c, w, w.keys[0], st, flags, nb, q.rk, q.aad_len, in, ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len},
+                                     w.dd.status, lim, /*packed=*/false);
         if (rc) return rc;
     }
     // The segment word and the records over the L bytes the index gives: a batch that decodes to another length fails first.
     { int rc = check_crc_word<false>(c, w, st, w.d_orig, nullptr, w.dd.v_len, nb, L, 1); if (rc) return rc; }
-    if (records && L) {
-        int rc = records_alloc(w.rec, (uint64_t)c->max_batch * index.ocs);
+    if (q.records && L) {
+        int rc = records_alloc(w.rec, (uint64_t)c->max_batch * q.index.ocs);
         if (!rc) rc = records_stage(c, w, st, L);
         if (rc) return rc;
     }
     if (flags) {
-        RT(rt::d2h(w.h_sizes, w.dd.a_len, 4ull * nb, st));
-        RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(out, w.dd.a_len, 4ull * nb, st));
+        RT(rt::d2h(out + nb, w.dd.status, 4ull * nb, st));
     }
-    RT(rt::d2h(w.h_sizes + 2 * nb, w.pcrc.d_cuts, 8, st));
-    RT(rt::event_record(w.ev_sizes, st));
+    RT(rt::d2h(out + 2 * nb, w.pcrc.d_cuts, 8, st));
     return TSGPU_OK;
 }
 
-// A drained batch in object order: every chunk's tag, frame and decoded size, then the record verdict, then the CRC words.
-static int check_drain(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool records, const uint32_t* tsizes, const ChunkLayout& index,
-                       CheckCarry& cur) {
+// A drained batch in object order (`out` as source_stage filled it): every chunk's tag, frame and decoded size, then the record
+// verdict, then the CRC words extend the carry.
+static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const uint32_t* out, CheckCarry& cur) {
     Work& w = *bt.w;
     const uint32_t nb = bt.nb;
-    const uint32_t* got = w.h_sizes;
-    const uint32_t* status = w.h_sizes + nb;
+    const uint32_t* got = out;
+    const uint32_t* status = out + nb;
+    const ChunkLayout& index = q.index;
     uint64_t L = 0, obj = 0;
     for (uint32_t i = 0; i < nb; i++) {
         const unsigned long long g = cur.chunks + bt.c0 + i;
@@ -1260,12 +1357,26 @@ static int check_drain(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool recor
         if (got[i] != index.size(g))
             return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, the chunk index gives %u", g, got[i], index.size(g));
         L += got[i];
-        obj += tsizes[bt.c0 + i];
+        obj += q.tsizes[bt.c0 + i];
     }
-    if (records) { int rc = records_resolve(c, w, cur.rec); if (rc) return rc; }
-    const uint32_t seg_word = w.h_sizes[2 * nb + 1], obj_word = flags ? w.h_sizes[2 * nb] : seg_word;
+    if (q.records) { int rc = records_resolve(c, w, cur.rec); if (rc) return rc; }
+    const uint32_t seg_word = out[2 * nb + 1], obj_word = q.flags ? out[2 * nb] : seg_word;
     cur.obj_raw = crc_shift(cur.obj_raw, obj, 0) ^ obj_word;
     cur.seg_raw = crc_shift(cur.seg_raw, L, 0) ^ seg_word;
+    return TSGPU_OK;
+}
+
+// After a window's batches: the carry moves past its chunks, and at the object's end the chunk count and the last record entry
+// are checked.
+static int source_finish(const SourceReq& q, CheckCarry& cur, int object_ends_here) {
+    cur.chunks += q.n;
+    cur.obj_len += q.need;
+    for (uint32_t i = 0; i < q.n; i++) cur.seg_len += q.index.size(cur.chunks - q.n + i);
+    if (!object_ends_here) return TSGPU_OK;
+    if (cur.chunks != q.index.count)
+        return fail(TSGPU_E_CORRUPT, "the object has %llu chunks, the chunk index (original chunk size %u, original file size %llu) "
+                    "has %llu", (unsigned long long)cur.chunks, q.index.ocs, (unsigned long long)q.index.ofs, (unsigned long long)q.index.count);
+    if (q.records) { int rc = records_segment_end(cur.rec); if (rc) return rc; }
     return TSGPU_OK;
 }
 
@@ -1274,58 +1385,213 @@ extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* s
                                   const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                                   tsgpu_check_cursor* cursor, int object_ends_here, uint32_t* object_crc32c, uint32_t* segment_crc32c) try {
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
-    if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VALIDATE_RECORDS)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
     if (object_ends_here && (!object_crc32c || !segment_crc32c)) return fail(TSGPU_E_ARG, "object_crc32c/segment_crc32c cannot be null");
-    if (n_chunks && !transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
-    if (original_chunk_size == 0) return fail(TSGPU_E_ARG, "Original chunk size must be positive, 0 given");
-    if (original_chunk_size > c->chunk_cap)
-        return fail(TSGPU_E_ARG, "original chunk size %u exceeds the context's max_chunk_bytes %u", original_chunk_size, c->chunk_cap);
-    if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
-    if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
-    if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
-    const bool records = flags & TSGPU_FLAG_VALIDATE_RECORDS;
-    if (records && (uint64_t)c->max_batch * original_chunk_size > REC_MAX_BATCH)
-        return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch,
-                    original_chunk_size);
-    if ((uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
-        return fail(TSGPU_E_ARG, "object checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
-                    (unsigned long long)c->slot_stride);
-    flags &= ~(ZSTD_MODIFIERS | TSGPU_FLAG_VALIDATE_RECORDS);      // how a frame was compressed does not matter to the reader
-    uint64_t need = 0;
-    for (uint32_t i = 0; i < n_chunks; i++) need += transformed_sizes[i];
-    if (need && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
-    if (need > src_len) return fail(TSGPU_E_SHORT, "Stream has fewer bytes than expected");
-    const ChunkLayout index{original_chunk_size, original_file_size, (original_file_size + original_chunk_size - 1) / original_chunk_size};
     CheckCarry cur;
     memcpy(&cur, cursor, sizeof cur);
-    // The index of an empty segment materialises one chunk of 0 transformed bytes: a caller that walks it passes that chunk.
-    uint32_t n = n_chunks;
-    if (index.count == 0 && cur.chunks == 0 && n == 1 && transformed_sizes[0] == 0) n = 0;
-
-    Aes256RoundKeys rk{};
-    if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
-    if (n) {
+    SourceReq q;
+    int rc = source_args(c, flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, key, aad, aad_len,
+                         cur, q);
+    if (rc) return rc;
+    if (q.n) {
         uint64_t in_off = 0;                                     // batches are issued in order: in_off walks src with them
-        const int rc = run_batches(c, n,
+        rc = run_batches(c, q.n,
             [&](const Batch& bt) {
-                const int r = check_issue(c, bt, flags, records, src + in_off, transformed_sizes, index, cur.chunks, rk, aad, aad_len);
+                Work& w = *bt.w;
+                RT(rt::set_device(w.device));
+                const int r = source_stage(c, w, w.stream, bt, q, src + in_off, cur.chunks, /*to_frames=*/false, w.h_sizes);
+                for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
+                if (r) return r;
+                RT(rt::event_record(w.ev_sizes, w.stream));
+                return TSGPU_OK;
+            },
+            [&](const Batch& bt) { return source_drain(c, bt, q, bt.w->h_sizes, cur); });
+        if (rc) return rc;
+    }
+    if ((rc = source_finish(q, cur, object_ends_here))) return rc;
+    if (object_ends_here) {
+        *object_crc32c = crc_finish(cur.obj_raw, cur.obj_len, 0);
+        *segment_crc32c = crc_finish(cur.seg_raw, cur.seg_len, 0);
+    }
+    memcpy(cursor, &cur, sizeof cur);
+    return TSGPU_OK;
+} catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
+
+// ------------------------------------------------------------------------------------------ object rewrite (host)
+// tsgpu_rewrite_object: the source half of the check, then the target half of the transform (target_stage) from the decoded
+// chunks in d_orig, so the plaintext never leaves the GPU.  When both sides compress, the source frames are kept: they are in
+// d_frames (a zstd-only object is loaded there rather than into d_xf, where each encrypted chunk would overlap its own frame
+// 12 bytes further on; an encrypted one is decrypted there), and the target half only encrypts or packs them.  At the drain, in
+// object order: the source's statuses, sizes and records (source_drain), the verify verdict on the new chunks, then the new
+// chunks' sizes, part prefixes and copy-out.
+
+// The state of a rewrite between calls: the public tsgpu_rewrite_cursor (192 bytes, zero = start of the object).
+struct RewriteCarry {
+    CheckCarry src;        // the old object and the decoded segment
+    PartsCarry out;        // the new object's parts
+    uint64_t reserved[4];
+};
+static_assert(sizeof(RewriteCarry) == sizeof(tsgpu_rewrite_cursor), "the cursor holds the carry");
+
+// The new object's side of a rewrite.
+struct TargetReq {
+    uint32_t flags;                  // ZSTD, modifiers and AES of the new object
+    bool verify, kept;               // kept: the source frames go into the new object as they are
+    Aes256RoundKeys rk;
+    const uint8_t* aad; uint32_t aad_len;
+    const uint8_t* ivs;
+};
+
+// One batch of a rewrite: the target's IVs and AAD, the source half, the target half, the D2H of the new sizes.  h_sizes:
+// [0, nb) new sizes, [nb, 3 nb) the verify stage's verdicts (verify_verdict), [3 nb, 5 nb + 2) the source half's out.
+static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const TargetReq& t, const uint8_t* src, uint64_t g0) {
+    Work& w = *bt.w;
+    const uint32_t nb = bt.nb;
+    RT(rt::set_device(w.device));
+    rt::stream_t st = w.stream;
+    GcmKeys& k = w.keys[1];
+    if (t.flags & TSGPU_FLAG_AES) {
+        memcpy(w.hd.ivs, t.ivs + (size_t)bt.c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
+        if (!k.ctx) {
+            RT(rt::malloc_device((void**)&k.ctx, sizeof(GcmKeyCtx)));
+            RT(rt::malloc_device((void**)&k.d_aad, MAX_AAD));
+            RT(rt::malloc_host((void**)&k.h_aad, MAX_AAD));
+        }
+        if (t.aad_len) {                     // the slot's previous batch has drained: its upload of h_aad is done
+            memcpy(k.h_aad, t.aad, t.aad_len);
+            RT(rt::h2d(k.d_aad, k.h_aad, t.aad_len, st));
+        }
+    }
+    { int rc = source_stage(c, w, st, bt, q, src, g0, /*to_frames=*/q.flags == TSGPU_FLAG_ZSTD, w.h_sizes + 3 * nb); if (rc) return rc; }
+    uint64_t frames_max = 0;                 // the largest kept frame, by the object's sizes
+    for (uint32_t i = 0; i < nb; i++) {
+        const uint32_t ts = q.tsizes[bt.c0 + i];
+        frames_max = std::max<uint64_t>(frames_max, (q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts);
+    }
+    ChunksOut fin;
+    { int rc = target_stage(c, w, k, st, t.flags, t.verify, /*parts=*/true, bt.c0, nb, q.index.ocs, t.rk, t.aad_len,
+                            ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, t.kept, frames_max, fin); if (rc) return rc; }
+    RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
+    RT(rt::event_record(w.ev_sizes, st));
+    return TSGPU_OK;
+}
+
+extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src, uint64_t src_len,
+                                    const uint32_t* transformed_sizes, uint32_t n_chunks, uint32_t original_chunk_size,
+                                    uint64_t original_file_size, const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                                    uint32_t to_flags, const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len,
+                                    const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                                    uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
+                                    tsgpu_rewrite_cursor* cursor, int object_ends_here,
+                                    uint32_t* source_crc32c, uint32_t* object_crc32c, uint32_t* segment_crc32c) try {
+    if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
+    if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
+    if (object_ends_here && (!source_crc32c || !segment_crc32c))
+        return fail(TSGPU_E_ARG, "source_crc32c/object_crc32c/segment_crc32c cannot be null");
+    const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
+    if (to_flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY)) return fail(TSGPU_E_ARG, "unknown to_flags %u", to_flags);
+    if (!(to_flags & xf))
+        return fail(TSGPU_E_ARG, "to_flags needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: the plain object is what tsgpu_detransform gives");
+    if (!(to_flags & TSGPU_FLAG_ZSTD) && (to_flags & ZSTD_MODIFIERS))
+        return fail(TSGPU_E_ARG, "to_flags %u: TSGPU_FLAG_ZSTD_DENSE and TSGPU_FLAG_ZSTD_CHECKSUM need TSGPU_FLAG_ZSTD", to_flags);
+    const bool kept = (from_flags & TSGPU_FLAG_ZSTD) && (to_flags & TSGPU_FLAG_ZSTD);
+    if (kept && (to_flags & ZSTD_MODIFIERS))
+        return fail(TSGPU_E_ARG, "to_flags %u: the source frames are kept as they are, so TSGPU_FLAG_ZSTD_DENSE and "
+                    "TSGPU_FLAG_ZSTD_CHECKSUM have nothing to act on", to_flags);
+    if ((to_flags & TSGPU_FLAG_AES) && (!to_key || (n_chunks && !to_ivs)))
+        return fail(TSGPU_E_ARG, "to_key and to_ivs are required for encryption");
+    if ((to_flags & TSGPU_FLAG_AES) && to_aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "to_aad longer than %u bytes", MAX_AAD);
+    if ((to_flags & TSGPU_FLAG_AES) && to_aad_len && !to_aad) return fail(TSGPU_E_ARG, "to_aad cannot be null");
+    if (n_chunks && !new_transformed_sizes) return fail(TSGPU_E_ARG, "new_transformed_sizes cannot be null");
+    RewriteCarry cur;
+    memcpy(&cur, cursor, sizeof cur);
+    SourceReq q;
+    int rc = source_args(c, from_flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size,
+                         from_key, from_aad, from_aad_len, cur.src, q);
+    if (rc) return rc;
+    if (q.n && !dst) return fail(TSGPU_E_ARG, "dst cannot be null");
+    // GCM breaks when one key encrypts two plaintexts under one IV: no two chunks of the window may share a new IV, nor, under
+    // the old key, a new IV an old chunk of the window has (an old chunk's IV is its first 12 bytes)
+    if ((to_flags & TSGPU_FLAG_AES) && q.n) {
+        struct Iv { std::array<uint8_t, TSGPU_IV_SIZE> b; uint32_t i; bool old; };
+        std::vector<Iv> ivs;
+        for (uint32_t i = 0; i < q.n; i++) {
+            Iv v{{}, i, false};
+            memcpy(v.b.data(), to_ivs + (size_t)i * TSGPU_IV_SIZE, TSGPU_IV_SIZE);
+            ivs.push_back(v);
+        }
+        if ((q.flags & TSGPU_FLAG_AES) && memcmp(from_key, to_key, 32) == 0) {
+            uint64_t at = 0;
+            for (uint32_t i = 0; i < q.n; at += transformed_sizes[i++]) {
+                if (transformed_sizes[i] < TSGPU_IV_SIZE) continue;
+                Iv v{{}, i, true};
+                memcpy(v.b.data(), src + at, TSGPU_IV_SIZE);
+                ivs.push_back(v);
+            }
+        }
+        std::sort(ivs.begin(), ivs.end(), [](const Iv& x, const Iv& y) { return x.b != y.b ? x.b < y.b : x.old < y.old; });
+        for (size_t j = 1; j < ivs.size(); j++) {
+            const Iv &x = ivs[j - 1], &y = ivs[j];
+            if (x.b != y.b || (x.old && y.old)) continue;           // two old chunks sharing an IV is the old object's business
+            if (y.old) return fail(TSGPU_E_ARG, "to_ivs[%u] repeats the IV of chunk %llu under the same key", x.i,
+                                   (unsigned long long)(cur.src.chunks + y.i));
+            return fail(TSGPU_E_ARG, "to_ivs[%u] repeats to_ivs[%u]", std::min(x.i, y.i), std::max(x.i, y.i));
+        }
+    }
+    // part_cap: the transform bound of the window's length by the chunk index, or of its kept frames
+    uint64_t L = 0, frames = 0;
+    for (uint32_t i = 0; i < q.n; i++) {
+        L += q.index.size(cur.src.chunks + i);
+        const uint32_t ts = transformed_sizes[i];
+        frames += ((q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts) + ((to_flags & TSGPU_FLAG_AES) ? 28 : 0);
+    }
+    const uint64_t bound = !q.n ? 0 : kept ? frames : tsgpu_transform_bound(to_flags, L, original_chunk_size);
+    const PartsReq pq{part_size, (tsgpu_parts_cursor*)&cur.out, part_crc32c, part_cap, n_parts, object_crc32c};
+    if ((rc = parts_args_ok(pq, to_flags, bound, object_ends_here))) return rc;
+
+    TargetReq t{};
+    t.flags = to_flags & ~TSGPU_FLAG_VERIFY;
+    t.verify = (to_flags & TSGPU_FLAG_VERIFY) || c->verify_default;
+    t.kept = kept;
+    if (to_flags & TSGPU_FLAG_AES) t.rk = aes256_expand_key(to_key);
+    t.aad = to_aad; t.aad_len = to_aad_len; t.ivs = to_ivs;
+    PartsRun run;
+    run.part_size = part_size; run.obj0 = cur.out.obj_len;
+    if (q.n) {
+        std::vector<uint32_t> len(q.n);                          // the window's original sizes (verify_verdict's messages)
+        for (uint32_t i = 0; i < q.n; i++) len[i] = q.index.size(cur.src.chunks + i);
+        run.batches.assign((q.n + c->max_batch - 1) / c->max_batch, PcrcBatch{});
+        uint64_t in_off = 0, dst_off = 0;                        // batches are issued in order: in_off walks src with them
+        rc = run_batches(c, q.n,
+            [&](const Batch& bt) {
+                const int r = rewrite_issue(c, bt, q, t, src + in_off, cur.src.chunks);
                 for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
                 return r;
             },
-            [&](const Batch& bt) { return check_drain(c, bt, flags, records, transformed_sizes, index, cur); });
+            [&](const Batch& bt) {
+                Work& w = *bt.w;
+                { int r = source_drain(c, bt, q, w.h_sizes + 3 * bt.nb, cur.src); if (r) return r; }
+                if (t.verify) { int r = verify_verdict(bt, len.data(), cur.src.chunks); if (r) return r; }
+                uint64_t total = 0;
+                for (uint32_t i = 0; i < bt.nb; i++) { new_transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
+                if (dst_off + total <= dst_cap) {
+                    int r = parts_drain(c, w, run, bt.c0 / c->max_batch, run.obj0 + dst_off, total);
+                    if (r) return r;
+                }
+                return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);
+            },
+            [&](const std::vector<Work*>& slots, int rcb) {          // the last batches' part prefixes, once all is idle
+                for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, run); w->pcrc.pending = -1; }
+                return rcb;
+            });
         if (rc) return rc;
-        cur.chunks += n;
-        cur.obj_len += need;
-        for (uint32_t i = 0; i < n; i++) cur.seg_len += index.size(cur.chunks - n + i);
     }
+    if ((rc = source_finish(q, cur.src, object_ends_here))) return rc;
+    if (n_chunks && !q.n) new_transformed_sizes[0] = 0;                    // the empty segment's one empty chunk stays one
+    parts_finish(pq, cur.out, q.n ? &run : nullptr, object_ends_here);     // writes cur.out and the part CRCs
     if (object_ends_here) {
-        if (cur.chunks != index.count)
-            return fail(TSGPU_E_CORRUPT, "the object has %llu chunks, the chunk index (original chunk size %u, original file size %llu) "
-                        "has %llu", (unsigned long long)cur.chunks, index.ocs, (unsigned long long)index.ofs, (unsigned long long)index.count);
-        if (records) { int rc = records_segment_end(cur.rec); if (rc) return rc; }
-        *object_crc32c = crc_finish(cur.obj_raw, cur.obj_len, 0);
-        *segment_crc32c = crc_finish(cur.seg_raw, cur.seg_len, 0);
+        *source_crc32c = crc_finish(cur.src.obj_raw, cur.src.obj_len, 0);
+        *segment_crc32c = crc_finish(cur.src.seg_raw, cur.src.seg_len, 0);
     }
     memcpy(cursor, &cur, sizeof cur);
     return TSGPU_OK;
@@ -1395,7 +1661,7 @@ extern "C" int tsgpu_transform_device(tsgpu_ctx* c, int device_index, uint32_t f
     });
     if (rc) return rc;
     Work& w = *claim.slots[0];
-    rc = transform_enqueue(c, w, st, flags, nb, cs, rk, aad_len, ChunksIn{d_src, w.dd.a_off, w.dd.a_len},
+    rc = transform_enqueue(c, w, w.keys[0], st, flags, nb, cs, rk, aad_len, ChunksIn{d_src, w.dd.a_off, w.dd.a_len},
                            ChunksOut{d_slots, w.dd.c_off, d_transformed_sizes});
     if (rc) return rc;
     RT(rt::event_record(w.ev_dev_done, st));
@@ -1433,7 +1699,7 @@ extern "C" int tsgpu_detransform_device(tsgpu_ctx* c, int device_index, uint32_t
     lim.aes_room = (flags & TSGPU_FLAG_ZSTD) ? (uint32_t)std::min<uint64_t>(c->frame_stride - 16, in_room - 28) : chunk_size;
     lim.zstd_in = (flags & TSGPU_FLAG_AES) ? (uint32_t)(c->frame_stride - 16) : in_room;
     lim.zstd_out = chunk_size;
-    rc = detransform_enqueue(c, w, st, flags, n_chunks, rk, aad_len, ChunksIn{d_slots, w.dd.c_off, d_transformed_sizes},
+    rc = detransform_enqueue(c, w, w.keys[0], st, flags, n_chunks, rk, aad_len, ChunksIn{d_slots, w.dd.c_off, d_transformed_sizes},
                              ChunksOut{d_dst, w.dd.a_off, d_original_sizes}, d_status, lim, /*packed=*/false);
     if (rc) return rc;
     RT(rt::event_record(w.ev_dev_done, st));
