@@ -66,3 +66,9 @@ tests/cpp/test_rewrite_mirror_simt: tests/cpp/test_rewrite_mirror.cpp $(PKG)/hos
 # JNI glue's object-rewrite path (RewriteCursor.rewriteObject) in the window flow of an operator tool, same fake JNIEnv
 tests/cpp/test_jni_rewrite_simt: tests/cpp/test_jni_rewrite.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so
 	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_rewrite.c -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'
+# Host mirror with CRC-64/NVME (crc64Parts, check64, RemoteSegmentRewriter::crc64), on the emulator build
+tests/cpp/test_crc64_mirror_simt: tests/cpp/test_crc64_mirror.cpp $(PKG)/host/chunk_transform.hpp $(PKG)/host/segment_upload.hpp $(PKG)/host/segment_check.hpp $(PKG)/host/segment_rewrite.hpp include/tsgpu.h tests/simt/libtsgpu_simt.so
+	g++ -O1 -g -std=c++17 -o $@ tests/cpp/test_crc64_mirror.cpp -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'
+# JNI glue's CRC-64/NVME exports (Crc64.transformParts, checkObject, rewriteObject), same fake JNIEnv
+tests/cpp/test_jni_crc64_simt: tests/cpp/test_jni_crc64.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so
+	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_crc64.c -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'

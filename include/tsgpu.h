@@ -315,6 +315,47 @@ int tsgpu_rewrite_object(tsgpu_ctx* ctx,
                          uint32_t* source_crc32c, uint32_t* object_crc32c, uint32_t* segment_crc32c);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * CRC-64/NVME twins of tsgpu_transform_parts, tsgpu_check_object and tsgpu_rewrite_object.  Each takes the arguments, rules,
+ * errors and part_cap bound of its CRC-32C twin, and writes the same transformed bytes, transformed_sizes and
+ * new_transformed_sizes for the same arguments; only the checksum outputs differ, as uint64_t.  A failed call writes no
+ * checksum, as in the CRC-32C calls.
+ *
+ * CRC-64/NVME: width 64, polynomial 0xAD93D23594C93659 (reflected 0x9A6C9329AC4BC9B5), init and xorout all ones, reflected
+ * input and output; crc64nvme("123456789") = 0xAE8B14860A799888, and 0 for no bytes.  The stores take it as 8 big-endian
+ * bytes, Base64-encoded (wiring: INTEGRATION.md):
+ *   - S3: CRC64NVME as a part checksum (x-amz-checksum-crc64nvme on UploadPart) and as the FULL_OBJECT checksum of a multipart
+ *     upload.  S3 is understood to store a CRC64NVME full-object checksum for objects uploaded without a client checksum, so
+ *     object_crc64 of tsgpu_check_object_crc64 is what such an object is compared with -- unverified here.
+ *   - Azure Blob: x-ms-content-crc64 on Put Block is understood to be this CRC -- unverified here (INTEGRATION.md).
+ *
+ * The cursors keep their sizes and hold the 64-bit words in place of the 32-bit ones.  A cursor carries one width: continuing
+ * a cursor with the twin of the call that started it gives wrong checksums.  The call does not detect this; the object store
+ * then refuses the upload, so the failure is safe.
+ * --------------------------------------------------------------------------------------------------------- */
+int tsgpu_transform_parts_crc64(tsgpu_ctx* ctx, uint32_t flags,
+                                const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
+                                const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                                uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                                tsgpu_records_cursor* records, int segment_ends_here,
+                                uint64_t part_size, tsgpu_parts_cursor* parts,
+                                uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts, uint64_t* object_crc64);
+int tsgpu_check_object_crc64(tsgpu_ctx* ctx, uint32_t flags,
+                             const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes, uint32_t n_chunks,
+                             uint32_t original_chunk_size, uint64_t original_file_size,
+                             const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
+                             tsgpu_check_cursor* cursor, int object_ends_here,
+                             uint64_t* object_crc64, uint64_t* segment_crc64);
+int tsgpu_rewrite_object_crc64(tsgpu_ctx* ctx,
+                               uint32_t from_flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                               uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
+                               const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                               uint32_t to_flags, const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len,
+                               const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                               uint64_t part_size, uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts,
+                               tsgpu_rewrite_cursor* cursor, int object_ends_here,
+                               uint64_t* source_crc64, uint64_t* object_crc64, uint64_t* segment_crc64);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Device-resident variants (inputs and outputs already in HBM of device `device_index` of the context; used by
  * bench.py for the kernel-side throughput and by callers that keep segments on the GPU).  Layouts:
  *   original side     contiguous, chunk i at i * chunk_size

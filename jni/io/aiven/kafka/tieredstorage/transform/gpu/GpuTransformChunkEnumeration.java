@@ -67,6 +67,15 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
                                         final int originalChunkSize, final boolean compression,
                                         final DataKeyAndAAD keyAndAad, final int batchChunks, final boolean validateRecords,
                                         final long partSize) {
+        this(ctx, pool, inputStream, originalChunkSize, compression, keyAndAad, batchChunks, validateRecords, partSize, false);
+    }
+
+    /** crc64Parts: with a partSize, the CRC-64/NVME of every part and of the object ({@link #partCrc64(int)},
+     *  {@link #objectCrc64()}; S3 CRC64NVME, Azure x-ms-content-crc64) instead of CRC-32C. */
+    public GpuTransformChunkEnumeration(final long ctx, final PinnedPool pool, final InputStream inputStream,
+                                        final int originalChunkSize, final boolean compression,
+                                        final DataKeyAndAAD keyAndAad, final int batchChunks, final boolean validateRecords,
+                                        final long partSize, final boolean crc64Parts) {
         if (inputStream == null) {
             throw new NullPointerException("inputStream cannot be null");
         }
@@ -84,7 +93,7 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
         if (partSize < 0 || (partSize > 0 && transforms == 0)) {
             throw new IllegalArgumentException("partSize must be 0, or positive with compression or encryption; " + partSize + " given");
         }
-        this.parts = partSize > 0 ? new PartsCursor(partSize) : null;
+        this.parts = partSize <= 0 ? null : crc64Parts ? new PartsCursor(partSize, true) : new PartsCursor(partSize);
         this.keyAndAad = keyAndAad;
         this.batchChunks = batchChunks;
         if (originalChunkSize > 0) {
@@ -122,6 +131,22 @@ public class GpuTransformChunkEnumeration implements TransformChunkEnumeration, 
             throw new IllegalStateException("part checksums were not requested (partSize 0)");
         }
         return parts.objectCrc32c();
+    }
+
+    /** The CRC-64/NVME of upload part partNumber (1-based) with crc64Parts, valid once the window that ends it is transformed. */
+    public long partCrc64(final int partNumber) {
+        if (parts == null) {
+            throw new IllegalStateException("part checksums were not requested (partSize 0)");
+        }
+        return parts.partCrc64(partNumber);
+    }
+
+    /** The CRC-64/NVME of the whole object (S3 FULL_OBJECT CRC64NVME) with crc64Parts, valid after the last window. */
+    public long objectCrc64() {
+        if (parts == null) {
+            throw new IllegalStateException("part checksums were not requested (partSize 0)");
+        }
+        return parts.objectCrc64();
     }
 
     @Override

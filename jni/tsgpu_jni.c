@@ -3,7 +3,7 @@
  * There is no JDK in this repository's build image: the tests compile this file against a test-only stand-in for
  * <jni.h> and drive it through a fake JNIEnv (tests/cpp/test_jni_shim.c).  Build on the broker host with
  *   gcc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude jni/tsgpu_jni.c -L<pkg> -ltsgpu -o libtsgpu_jni.so
- * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
+ * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,RewriteCursor,Crc64,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
  * (implement TransformChunkEnumeration / DetransformChunkEnumeration of the reference, core/M/transform/TransformChunkEnumeration.java:28-42,
  * DetransformChunkEnumeration.java:28-29) and jni/io/aiven/kafka/tieredstorage/fetch/gpu/GpuChunkManager.java (ChunkManager, fetch/ChunkManager.java).
  *
@@ -60,13 +60,15 @@ JNIEXPORT jlong JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_TsGpu_tr
                                                                                              jlong srcLen, jint chunkSize) {
     return (jlong)tsgpu_transform_bound((uint32_t)flags, (uint64_t)srcLen, (uint32_t)chunkSize);
 }
-/* The part-checksum arguments of tsgpu_transform_parts (PartsCursor.transformParts). */
+/* The part-checksum arguments of tsgpu_transform_parts (PartsCursor.transformParts), or with crcs64 of
+ * tsgpu_transform_parts_crc64 (Crc64.transformParts). */
 typedef struct {
     uint64_t part_size; tsgpu_parts_cursor* cursor;
     uint32_t* crcs; uint32_t cap; uint32_t n; uint32_t object_crc;
+    uint64_t* crcs64; uint64_t object_crc64;
 } parts_args;
-/* tsgpu_transform, tsgpu_transform_cursor when `cursor` is given, or tsgpu_transform_parts when `parts` is; returns the number
- * of chunks, or -1 with an exception pending.  transformedSizes (int[]) receives one entry per chunk. */
+/* tsgpu_transform, tsgpu_transform_cursor when `cursor` is given, or tsgpu_transform_parts[_crc64] when `parts` is; returns the
+ * number of chunks, or -1 with an exception pending.  transformedSizes (int[]) receives one entry per chunk. */
 static jint transform_call(JNIEnv* env, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
                            jbyteArray ivs, jobject dst, jintArray transformedSizes, tsgpu_records_cursor* cursor, int segmentEndsHere,
                            parts_args* parts) {
@@ -91,7 +93,12 @@ static jint transform_call(JNIEnv* env, jlong h, jint flags, jobject src, jlong 
         return -1;
     }
     jint* sizes = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
-    int rc = parts
+    int rc = parts && parts->crcs64
+        ? tsgpu_transform_parts_crc64((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
+                                      (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n,
+                                      cursor, segmentEndsHere, parts->part_size, parts->cursor, parts->crcs64, parts->cap, &parts->n,
+                                      &parts->object_crc64)
+        : parts
         ? tsgpu_transform_parts((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (uint32_t)chunkSize, (const uint8_t*)k,
                                 (const uint8_t*)a, (uint32_t)alen, (const uint8_t*)iv, d, (uint64_t)dcap, (uint32_t*)sizes, &n,
                                 cursor, segmentEndsHere, parts->part_size, parts->cursor, parts->crcs, parts->cap, &parts->n,
@@ -143,7 +150,7 @@ JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_PartsCurs
     if (partSize < 1) { throw_arg(env, "partSize must be positive"); return -1; }
     if (!partCrc32c || !partsOut) { throw_arg(env, "partCrc32c and partsOut cannot be null"); return -1; }
     if ((*env)->GetArrayLength(env, partsOut) < 2) { throw_arg(env, "partsOut must hold 2 ints"); return -1; }
-    parts_args pa = {(uint64_t)partSize, pcur, NULL, (uint32_t)(*env)->GetArrayLength(env, partCrc32c), 0, 0};
+    parts_args pa = {(uint64_t)partSize, pcur, NULL, (uint32_t)(*env)->GetArrayLength(env, partCrc32c), 0, 0, NULL, 0};
     jint* crcs = (*env)->GetIntArrayElements(env, partCrc32c, NULL);
     pa.crcs = (uint32_t*)crcs;
     const jint n = transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, rcur,
@@ -287,4 +294,151 @@ JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RewriteCu
         out[0] = (jint)crcs[0]; out[1] = (jint)crcs[1]; out[2] = (jint)crcs[2];
         (*env)->ReleaseIntArrayElements(env, crcsOut, out, 0);
     }
+}
+
+/* ---------------------------------------------------------------------------------------------------------------------------
+ * CRC-64/NVME twins (Crc64.java).  Each takes the arguments of its CRC-32C twin above; the 64-bit checksums come back in direct
+ * ByteBuffers, one 8-byte word each in the platform's byte order (ByteOrder.nativeOrder() on the Java side). */
+
+/* The cursors of a parts call, checked as PartsCursor.transformParts checks them; NULL with an exception pending. */
+static int parts_cursors(JNIEnv* env, jobject recordsCursor, jobject partsCursor, jlong partSize, tsgpu_records_cursor** rcur,
+                         tsgpu_parts_cursor** pcur) {
+    jlong rcap = 0, pcap = 0;
+    *rcur = (tsgpu_records_cursor*)direct(env, recordsCursor, 0, &rcap, "records cursor must be a direct ByteBuffer of 64 bytes");
+    if (!*rcur) return -1;
+    if (rcap < (jlong)sizeof(tsgpu_records_cursor)) { throw_arg(env, "records cursor must be a direct ByteBuffer of 64 bytes"); return -1; }
+    *pcur = (tsgpu_parts_cursor*)direct(env, partsCursor, 0, &pcap, "parts cursor must be a direct ByteBuffer of 32 bytes");
+    if (!*pcur) return -1;
+    if (pcap < (jlong)sizeof(tsgpu_parts_cursor)) { throw_arg(env, "parts cursor must be a direct ByteBuffer of 32 bytes"); return -1; }
+    if (partSize < 1) { throw_arg(env, "partSize must be positive"); return -1; }
+    return 0;
+}
+
+/* Crc64.transformParts: PartsCursor.transformParts with CRC-64/NVME.  partCrc64 (direct, 8 bytes per part: its capacity / 8 is
+ * part_cap) receives the CRCs of the parts the window completed, nPartsOut[0] their count, and objectCrc64Out (direct, 8 bytes)
+ * on the segment's last window the object's CRC-64/NVME.  Nothing is written on failure. */
+JNIEXPORT jint JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_Crc64_transformParts(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jint chunkSize, jbyteArray key, jbyteArray aad,
+    jbyteArray ivs, jobject dst, jintArray transformedSizes, jobject recordsCursor, jboolean segmentEndsHere, jlong partSize,
+    jobject partsCursor, jobject partCrc64, jintArray nPartsOut, jobject objectCrc64Out) {
+    tsgpu_records_cursor* rcur; tsgpu_parts_cursor* pcur;
+    if (parts_cursors(env, recordsCursor, partsCursor, partSize, &rcur, &pcur)) return -1;
+    jlong ccap = 0;
+    uint64_t* crcs = (uint64_t*)direct(env, partCrc64, 0, &ccap, "partCrc64 must be a direct ByteBuffer");
+    if (!crcs) return -1;
+    jlong ocap = 0;
+    uint64_t* obj = (uint64_t*)direct(env, objectCrc64Out, 0, &ocap, "objectCrc64Out must be a direct ByteBuffer of 8 bytes");
+    if (!obj) return -1;
+    if (ocap < 8) { throw_arg(env, "objectCrc64Out must be a direct ByteBuffer of 8 bytes"); return -1; }
+    if (!nPartsOut || (*env)->GetArrayLength(env, nPartsOut) < 1) { throw_arg(env, "nPartsOut must hold 1 int"); return -1; }
+    parts_args pa = {(uint64_t)partSize, pcur, NULL, (uint32_t)(ccap / 8), 0, 0, crcs, 0};
+    const jint n = transform_call(env, h, flags, src, srcLen, chunkSize, key, aad, ivs, dst, transformedSizes, rcur,
+                                  segmentEndsHere ? 1 : 0, &pa);
+    if (n < 0) return -1;
+    jint* np = (*env)->GetIntArrayElements(env, nPartsOut, NULL);
+    np[0] = (jint)pa.n;
+    (*env)->ReleaseIntArrayElements(env, nPartsOut, np, 0);
+    if (segmentEndsHere) *obj = pa.object_crc64;
+    return n;
+}
+
+/* Crc64.checkObject: CheckCursor.checkObject with CRC-64/NVME.  crcsOut (direct, 16 bytes) receives, on the object's last window,
+ * the CRC-64/NVME of the object and of the decoded segment. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_Crc64_checkObject(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray transformedSizes, jint originalChunkSize,
+    jlong originalFileSize, jbyteArray key, jbyteArray aad, jobject cursor, jboolean objectEndsHere, jobject crcsOut) {
+    jlong ccap = 0;
+    uint8_t* s = srcLen ? direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer") : NULL;
+    if (srcLen && !s) return;
+    tsgpu_check_cursor* cur = (tsgpu_check_cursor*)direct(env, cursor, 0, &ccap, "check cursor must be a direct ByteBuffer of 128 bytes");
+    if (!cur) return;
+    if (ccap < (jlong)sizeof(tsgpu_check_cursor)) { throw_arg(env, "check cursor must be a direct ByteBuffer of 128 bytes"); return; }
+    jlong wcap = 0;
+    uint64_t* out = (uint64_t*)direct(env, crcsOut, 0, &wcap, "crcsOut must be a direct ByteBuffer of 16 bytes");
+    if (!out) return;
+    if (wcap < 16) { throw_arg(env, "crcsOut must be a direct ByteBuffer of 16 bytes"); return; }
+    if (!transformedSizes) { throw_arg(env, "chunks cannot be null"); return; }
+    if (originalChunkSize < 1) { throw_arg(env, "Original chunk size must be positive"); return; }
+    if (originalFileSize < 0) { throw_arg(env, "Original file size must be non-negative"); return; }
+    if ((flags & TSGPU_FLAG_AES) && key && (*env)->GetArrayLength(env, key) != 32) { throw_arg(env, "data key must be 32 bytes"); return; }
+    jbyte* k = key ? (*env)->GetByteArrayElements(env, key, NULL) : NULL;
+    jbyte* a = aad ? (*env)->GetByteArrayElements(env, aad, NULL) : NULL;
+    jint alen = aad ? (*env)->GetArrayLength(env, aad) : 0;
+    uint32_t n = (uint32_t)(*env)->GetArrayLength(env, transformedSizes);
+    jint* ts = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
+    uint64_t crcs[2] = {0, 0};
+    int rc = tsgpu_check_object_crc64((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, s, (uint64_t)srcLen, (const uint32_t*)ts, n,
+                                      (uint32_t)originalChunkSize, (uint64_t)originalFileSize, (const uint8_t*)k, (const uint8_t*)a,
+                                      (uint32_t)alen, cur, objectEndsHere ? 1 : 0, &crcs[0], &crcs[1]);
+    (*env)->ReleaseIntArrayElements(env, transformedSizes, ts, JNI_ABORT);
+    if (k) (*env)->ReleaseByteArrayElements(env, key, k, JNI_ABORT);
+    if (a) (*env)->ReleaseByteArrayElements(env, aad, a, JNI_ABORT);
+    if (rc) { throw_rt(env, rc); return; }
+    if (objectEndsHere) { out[0] = crcs[0]; out[1] = crcs[1]; }
+}
+
+/* Crc64.rewriteObject: RewriteCursor.rewriteObject with CRC-64/NVME.  partCrc64 (direct, 8 bytes per part: its capacity / 8 is
+ * part_cap) receives the CRCs of the upload parts the window completes and nPartsOut[0] their count; crcsOut (direct, 24 bytes)
+ * receives, on the object's last window, the CRC-64/NVME of the old object, of the new object and of the decoded segment. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_Crc64_rewriteObject(
+    JNIEnv* env, jclass c, jlong h, jint fromFlags, jobject src, jlong srcLen, jintArray transformedSizes, jint originalChunkSize,
+    jlong originalFileSize, jbyteArray fromKey, jbyteArray fromAad, jint toFlags, jbyteArray toKey, jbyteArray toAad,
+    jbyteArray toIvs, jobject dst, jlong dstCap, jintArray newTransformedSizes, jlong partSize, jobject partCrc64,
+    jintArray nPartsOut, jobject cursor, jboolean objectEndsHere, jobject crcsOut) {
+    jlong ccap = 0, pcap = 0;
+    uint8_t* s = srcLen ? direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer") : NULL;
+    if (srcLen && !s) return;
+    uint8_t* d = dstCap ? direct(env, dst, dstCap, NULL, "dst must be a direct ByteBuffer") : NULL;
+    if (dstCap && !d) return;
+    tsgpu_rewrite_cursor* cur = (tsgpu_rewrite_cursor*)direct(env, cursor, 0, &ccap, "rewrite cursor must be a direct ByteBuffer of 192 bytes");
+    if (!cur) return;
+    if (ccap < (jlong)sizeof(tsgpu_rewrite_cursor)) { throw_arg(env, "rewrite cursor must be a direct ByteBuffer of 192 bytes"); return; }
+    uint64_t* pc = (uint64_t*)direct(env, partCrc64, 0, &pcap, "partCrc64 must be a direct ByteBuffer");
+    if (!pc) return;
+    jlong wcap = 0;
+    uint64_t* out = (uint64_t*)direct(env, crcsOut, 0, &wcap, "crcsOut must be a direct ByteBuffer of 24 bytes");
+    if (!out) return;
+    if (wcap < 24) { throw_arg(env, "crcsOut must be a direct ByteBuffer of 24 bytes"); return; }
+    if (!transformedSizes) { throw_arg(env, "chunks cannot be null"); return; }
+    const uint32_t n = (uint32_t)(*env)->GetArrayLength(env, transformedSizes);
+    if (!newTransformedSizes || (uint32_t)(*env)->GetArrayLength(env, newTransformedSizes) < n) {
+        throw_arg(env, "newTransformedSizes must hold one int per chunk"); return;
+    }
+    if (!nPartsOut || (*env)->GetArrayLength(env, nPartsOut) < 1) { throw_arg(env, "nPartsOut must hold 1 int"); return; }
+    if (originalChunkSize < 1) { throw_arg(env, "Original chunk size must be positive"); return; }
+    if (originalFileSize < 0) { throw_arg(env, "Original file size must be non-negative"); return; }
+    if (partSize < 1) { throw_arg(env, "partSize must be positive"); return; }
+    if ((fromFlags & TSGPU_FLAG_AES) && fromKey && (*env)->GetArrayLength(env, fromKey) != 32) { throw_arg(env, "data key must be 32 bytes"); return; }
+    if ((toFlags & TSGPU_FLAG_AES) && toKey && (*env)->GetArrayLength(env, toKey) != 32) { throw_arg(env, "data key must be 32 bytes"); return; }
+    if ((toFlags & TSGPU_FLAG_AES) && n && (!toIvs || (uint32_t)(*env)->GetArrayLength(env, toIvs) < 12 * n)) {
+        throw_arg(env, "toIvs must hold 12 bytes per chunk"); return;
+    }
+    jbyte* fk = fromKey ? (*env)->GetByteArrayElements(env, fromKey, NULL) : NULL;
+    jbyte* fa = fromAad ? (*env)->GetByteArrayElements(env, fromAad, NULL) : NULL;
+    jint falen = fromAad ? (*env)->GetArrayLength(env, fromAad) : 0;
+    jbyte* tk = toKey ? (*env)->GetByteArrayElements(env, toKey, NULL) : NULL;
+    jbyte* ta = toAad ? (*env)->GetByteArrayElements(env, toAad, NULL) : NULL;
+    jint talen = toAad ? (*env)->GetArrayLength(env, toAad) : 0;
+    jbyte* iv = toIvs ? (*env)->GetByteArrayElements(env, toIvs, NULL) : NULL;
+    jint* ts = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
+    jint* nts = (*env)->GetIntArrayElements(env, newTransformedSizes, NULL);
+    uint32_t nParts = 0;
+    uint64_t crcs[3] = {0, 0, 0};
+    int rc = tsgpu_rewrite_object_crc64((tsgpu_ctx*)(intptr_t)h, (uint32_t)fromFlags, s, (uint64_t)srcLen, (const uint32_t*)ts, n,
+                                        (uint32_t)originalChunkSize, (uint64_t)originalFileSize, (const uint8_t*)fk, (const uint8_t*)fa,
+                                        (uint32_t)falen, (uint32_t)toFlags, (const uint8_t*)tk, (const uint8_t*)ta, (uint32_t)talen,
+                                        (const uint8_t*)iv, d, (uint64_t)dstCap, (uint32_t*)nts, (uint64_t)partSize, pc,
+                                        (uint32_t)(pcap / 8), &nParts, cur, objectEndsHere ? 1 : 0, &crcs[0], &crcs[1], &crcs[2]);
+    (*env)->ReleaseIntArrayElements(env, transformedSizes, ts, JNI_ABORT);
+    (*env)->ReleaseIntArrayElements(env, newTransformedSizes, nts, rc ? JNI_ABORT : 0);
+    if (fk) (*env)->ReleaseByteArrayElements(env, fromKey, fk, JNI_ABORT);
+    if (fa) (*env)->ReleaseByteArrayElements(env, fromAad, fa, JNI_ABORT);
+    if (tk) (*env)->ReleaseByteArrayElements(env, toKey, tk, JNI_ABORT);
+    if (ta) (*env)->ReleaseByteArrayElements(env, toAad, ta, JNI_ABORT);
+    if (iv) (*env)->ReleaseByteArrayElements(env, toIvs, iv, JNI_ABORT);
+    if (rc) { throw_rt(env, rc); return; }
+    jint* np = (*env)->GetIntArrayElements(env, nPartsOut, NULL);
+    np[0] = (jint)nParts;
+    (*env)->ReleaseIntArrayElements(env, nPartsOut, np, 0);
+    if (objectEndsHere) { out[0] = crcs[0]; out[1] = crcs[1]; out[2] = crcs[2]; }
 }

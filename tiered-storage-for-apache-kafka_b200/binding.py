@@ -36,6 +36,7 @@ SYMBOLS = [
     "tsgpu_transformed_chunks_deserialize", "tsgpu_chunk_index_json", "tsgpu_profile_enable", "tsgpu_profile_report",
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
     "tsgpu_transform_cursor", "tsgpu_transform_parts", "tsgpu_check_object", "tsgpu_rewrite_object",
+    "tsgpu_transform_parts_crc64", "tsgpu_check_object_crc64", "tsgpu_rewrite_object_crc64",
 ]
 
 
@@ -79,6 +80,9 @@ def load(path=None):
     L.tsgpu_check_object.argtypes = [vp, u32, vp, u64, vp, u32, u32, u64, vp, vp, u32, vp, C.c_int, vp, vp]
     L.tsgpu_rewrite_object.argtypes = [vp, u32, vp, u64, vp, u32, u32, u64, vp, vp, u32, u32, vp, vp, u32, vp, vp, u64, vp,
                                        u64, vp, u32, vp, vp, C.c_int, vp, vp, vp]
+    L.tsgpu_transform_parts_crc64.argtypes = L.tsgpu_transform_parts.argtypes
+    L.tsgpu_check_object_crc64.argtypes = L.tsgpu_check_object.argtypes
+    L.tsgpu_rewrite_object_crc64.argtypes = L.tsgpu_rewrite_object.argtypes
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
     L.tsgpu_detransform_device.argtypes = [vp, C.c_int, u32, vp, u64, vp, u32, u32, vp, vp, u32, vp, vp, vp, vp]
     L.tsgpu_launch_count.restype = u64
@@ -108,6 +112,10 @@ def _u8(b):
 
 def _p(a):
     return a.ctypes.data if a is not None and a.size else None
+
+
+def _np_word(word):
+    return np.uint64 if word is C.c_uint64 else np.uint32
 
 
 class Context:
@@ -202,6 +210,18 @@ class Context:
         start of the object), updated in place on success; `records_cursor` a 64-byte one as transform_cursor takes (needed with
         FLAG_VALIDATE_RECORDS).  Returns (transformed bytes, [transformed sizes], [CRC-32C of the parts this call completed],
         CRC-32C of the whole object or None when the segment does not end here)."""
+        return self._transform_parts(self.lib.tsgpu_transform_parts, C.c_uint32, flags, src, chunk_size, part_size, parts_cursor,
+                                     segment_ends_here, records_cursor, key, aad, ivs, part_cap)
+
+    def transform_parts_crc64(self, flags, src, chunk_size, part_size, parts_cursor, segment_ends_here, records_cursor=None,
+                              key=None, aad=b"", ivs=None, part_cap=None):
+        """transform_parts with CRC-64/NVME part and object checksums (tsgpu_transform_parts_crc64): the same bytes and sizes,
+        the checksums as ints below 2**64.  A parts cursor carries one width: start and continue it with the same method."""
+        return self._transform_parts(self.lib.tsgpu_transform_parts_crc64, C.c_uint64, flags, src, chunk_size, part_size,
+                                     parts_cursor, segment_ends_here, records_cursor, key, aad, ivs, part_cap)
+
+    def _transform_parts(self, fn, word, flags, src, chunk_size, part_size, parts_cursor, segment_ends_here, records_cursor,
+                         key, aad, ivs, part_cap):
         s = _u8(src)
         for cur, size in ((parts_cursor, PARTS_CURSOR_SIZE), (records_cursor, CURSOR_SIZE)):
             if cur is not None and not (isinstance(cur, np.ndarray) and cur.dtype == np.uint8 and cur.size == size
@@ -215,10 +235,10 @@ class Context:
         n = C.c_uint32(n_max)
         if part_cap is None:
             part_cap = (bound + part_size) // max(part_size, 1) + 1
-        crcs = np.zeros(max(part_cap, 1), dtype=np.uint32)
-        n_parts, obj = C.c_uint32(0), C.c_uint32(0)
+        crcs = np.zeros(max(part_cap, 1), dtype=_np_word(word))
+        n_parts, obj = C.c_uint32(0), word(0)
         k, a, iv = _u8(key), _u8(aad), _u8(ivs)
-        self._check(self.lib.tsgpu_transform_parts(
+        self._check(fn(
             self._h, flags, _p(s), s.size, chunk_size, _p(k), _p(a), a.size, _p(iv), dst.ctypes.data, dst.size,
             sizes.ctypes.data, C.addressof(n), None if records_cursor is None else records_cursor.ctypes.data,
             1 if segment_ends_here else 0, part_size, None if parts_cursor is None else parts_cursor.ctypes.data,
@@ -258,6 +278,18 @@ class Context:
         """Checks one window of a stored object against its chunk index on the GPU (tsgpu_check_object) without copying its
         plaintext back.  `cursor`: a 128-byte np.uint8 array (zeros at the start of the object), updated in place on success; None
         checks a whole object.  Returns (object CRC-32C, segment CRC-32C) when the object ends here, else None."""
+        return self._check_object(self.lib.tsgpu_check_object, C.c_uint32, flags, src, transformed_sizes, original_chunk_size,
+                                  original_file_size, cursor, object_ends_here, key, aad)
+
+    def check_object_crc64(self, flags, src, transformed_sizes, original_chunk_size, original_file_size, cursor=None,
+                           object_ends_here=True, key=None, aad=b""):
+        """check_object with CRC-64/NVME words (tsgpu_check_object_crc64): (object CRC-64/NVME, segment CRC-64/NVME) when the
+        object ends here, else None.  A cursor carries one width: start and continue it with the same method."""
+        return self._check_object(self.lib.tsgpu_check_object_crc64, C.c_uint64, flags, src, transformed_sizes, original_chunk_size,
+                                  original_file_size, cursor, object_ends_here, key, aad)
+
+    def _check_object(self, fn, word, flags, src, transformed_sizes, original_chunk_size, original_file_size, cursor,
+                      object_ends_here, key, aad):
         s = _u8(src)
         if cursor is None:
             cursor = np.zeros(CHECK_CURSOR_SIZE, np.uint8)
@@ -265,9 +297,9 @@ class Context:
                 and cursor.flags.c_contiguous):
             raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % CHECK_CURSOR_SIZE)
         ts = np.ascontiguousarray(transformed_sizes, dtype=np.uint32)
-        obj, seg = C.c_uint32(0), C.c_uint32(0)
+        obj, seg = word(0), word(0)
         k, a = _u8(key), _u8(aad)
-        self._check(self.lib.tsgpu_check_object(self._h, flags, _p(s), s.size, _p(ts), ts.size, original_chunk_size,
+        self._check(fn(self._h, flags, _p(s), s.size, _p(ts), ts.size, original_chunk_size,
                                                 original_file_size, _p(k), _p(a), a.size, cursor.ctypes.data,
                                                 1 if object_ends_here else 0, C.addressof(obj), C.addressof(seg)))
         return (int(obj.value), int(seg.value)) if object_ends_here else None
@@ -280,6 +312,21 @@ class Context:
         np.uint8 array (zeros at the start of the object), updated in place on success; None rewrites a whole object.  Returns
         (new bytes, [new transformed sizes], [CRC-32C of the parts this call completed], (source, object, segment) CRC-32C or None
         when the object does not end here)."""
+        return self._rewrite_object(self.lib.tsgpu_rewrite_object, C.c_uint32, from_flags, src, transformed_sizes,
+                                    original_chunk_size, original_file_size, to_flags, part_size, cursor, object_ends_here,
+                                    from_key, from_aad, to_key, to_aad, to_ivs, part_cap)
+
+    def rewrite_object_crc64(self, from_flags, src, transformed_sizes, original_chunk_size, original_file_size, to_flags,
+                             part_size, cursor=None, object_ends_here=True, from_key=None, from_aad=b"", to_key=None, to_aad=b"",
+                             to_ivs=None, part_cap=None):
+        """rewrite_object with CRC-64/NVME part, source, object and segment checksums (tsgpu_rewrite_object_crc64): the same new
+        bytes and sizes.  A cursor carries one width: start and continue it with the same method."""
+        return self._rewrite_object(self.lib.tsgpu_rewrite_object_crc64, C.c_uint64, from_flags, src, transformed_sizes,
+                                    original_chunk_size, original_file_size, to_flags, part_size, cursor, object_ends_here,
+                                    from_key, from_aad, to_key, to_aad, to_ivs, part_cap)
+
+    def _rewrite_object(self, fn, word, from_flags, src, transformed_sizes, original_chunk_size, original_file_size, to_flags,
+                        part_size, cursor, object_ends_here, from_key, from_aad, to_key, to_aad, to_ivs, part_cap):
         s = _u8(src)
         if cursor is None:
             cursor = np.zeros(REWRITE_CURSOR_SIZE, np.uint8)
@@ -295,10 +342,10 @@ class Context:
         sizes = np.zeros(max(n, 1), dtype=np.uint32)
         if part_cap is None:
             part_cap = (cap + part_size) // max(part_size, 1) + 1
-        crcs = np.zeros(max(part_cap, 1), dtype=np.uint32)
-        n_parts, src_crc, obj_crc, seg_crc = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        crcs = np.zeros(max(part_cap, 1), dtype=_np_word(word))
+        n_parts, src_crc, obj_crc, seg_crc = C.c_uint32(0), word(0), word(0), word(0)
         fk, fa, tk, ta, iv = _u8(from_key), _u8(from_aad), _u8(to_key), _u8(to_aad), _u8(to_ivs)
-        self._check(self.lib.tsgpu_rewrite_object(
+        self._check(fn(
             self._h, from_flags, _p(s), s.size, _p(ts), n, original_chunk_size, original_file_size, _p(fk), _p(fa), fa.size,
             to_flags, _p(tk), _p(ta), ta.size, _p(iv), dst.ctypes.data, dst.size, sizes.ctypes.data, part_size,
             crcs.ctypes.data, part_cap, C.addressof(n_parts), cursor.ctypes.data, 1 if object_ends_here else 0,

@@ -10,7 +10,8 @@
 //   detransformed on the device and compared with its input before any of its bytes are copied out.  With
 //   TSGPU_FLAG_VALIDATE_RECORDS the Kafka log entries of each batch are checked on the device (records.cuh) and the batch's
 //   verdict is resolved, in batch order, before its bytes are copied out.  tsgpu_transform_parts also hashes each packed batch
-//   (part_crc.cuh) and combines the CRC-32C of the object's upload parts on the host once the call's streams are idle.
+//   (part_crc.cuh) and combines the CRC-32C of the object's upload parts on the host once the call's streams are idle;
+//   tsgpu_transform_parts_crc64 does the same with CRC-64/NVME (one source, instantiated for each CRC word).
 #include <algorithm>
 #include <array>
 #include <condition_variable>
@@ -80,13 +81,14 @@ struct RecScratch {
     RecOut* h_out = nullptr;       // pinned
 };
 
-// Device arrays of the upload-part checksums of one slot (part_crc.cuh), sized for batches of up to `cap` packed bytes.
-struct PcrcScratch {
+// Device arrays of the upload-part checksums of one slot (part_crc.cuh), sized for batches of up to `cap` packed bytes, for one
+// CRC word W (uint32_t: CRC-32C, uint64_t: CRC-64/NVME).
+template <typename W> struct PcrcScratch {
     uint8_t* d = nullptr;
     uint64_t cap = 0;
-    PcrcArgs a{};                  // the batch last enqueued on the slot: pcrc_cuts reads the same arrays at its drain
-    uint32_t* d_cuts = nullptr;    // pcrc_cuts output and its pinned copy, cuts_cap words
-    uint32_t* h_cuts = nullptr;
+    PcrcArgs<W> a{};               // the batch last enqueued on the slot: pcrc_cuts reads the same arrays at its drain
+    W* d_cuts = nullptr;           // pcrc_cuts output and its pinned copy, cuts_cap words
+    W* h_cuts = nullptr;
     uint32_t cuts_cap = 0;
     int32_t pending = -1;          // the call's batch whose prefixes h_cuts receives (collected at the slot's next drain or at the end)
 };
@@ -123,8 +125,13 @@ struct Work {
     ZstdDecScratch zdec{};
     uint32_t* h_sizes = nullptr;   // pinned: sizes/status (and the verify stage's first differing bytes) coming back
     RecScratch rec{};              // TSGPU_FLAG_VALIDATE_RECORDS, allocated on first use
-    PcrcScratch pcrc{};            // tsgpu_transform_parts, allocated on first use
+    PcrcScratch<uint32_t> pcrc{};  // CRC-32C part and object checksums, allocated on first use
+    PcrcScratch<uint64_t> pcrc64{};   // CRC-64/NVME (the _crc64 calls), allocated on first use
 };
+template <typename W> PcrcScratch<W>& pcrc_of(Work& w) {
+    if constexpr (sizeof(W) == 8) return w.pcrc64;
+    else return w.pcrc;
+}
 
 struct Lane { int device = 0; Work w[NSLOT_MAX]; };
 
@@ -206,7 +213,8 @@ static void work_free(Work& w) {
     rt::free_device(w.keys[1].ctx); rt::free_device(w.keys[1].d_aad); rt::free_host(w.keys[1].h_aad);
     zstd_enc_scratch_free(w.zenc); zstd_blk_scratch_free(w.zblk); zstd_dec_scratch_free(w.zdec);
     rt::free_device(w.rec.d); rt::free_device(w.rec.d_out); rt::free_host(w.rec.h_out); w.rec = RecScratch{};
-    rt::free_device(w.pcrc.d); rt::free_device(w.pcrc.d_cuts); rt::free_host(w.pcrc.h_cuts); w.pcrc = PcrcScratch{};
+    rt::free_device(w.pcrc.d); rt::free_device(w.pcrc.d_cuts); rt::free_host(w.pcrc.h_cuts); w.pcrc = PcrcScratch<uint32_t>{};
+    rt::free_device(w.pcrc64.d); rt::free_device(w.pcrc64.d_cuts); rt::free_host(w.pcrc64.h_cuts); w.pcrc64 = PcrcScratch<uint64_t>{};
     for (GcmKeys& k : w.keys) k = GcmKeys{};                // forgets the keys too
     rt::event_destroy(w.ev_sizes); rt::event_destroy(w.ev_done);
     rt::event_destroy(w.ev_dev_desc); rt::event_destroy(w.ev_dev_done);
@@ -643,102 +651,112 @@ static int records_segment_end(const RecCarry& carry) {
 }
 
 // ------------------------------------------------------------------------------------------ upload-part checksums
-// The state of an object between calls: the public tsgpu_parts_cursor (32 bytes, zero = start of the object).
-struct PartsCarry {
+// The state of an object between calls: the public tsgpu_parts_cursor (32 bytes, zero = start of the object).  The two raw CRCs
+// take 8 of the last 16 bytes with CRC-32C (the other 8 are reserved) and all 16 with CRC-64/NVME.
+template <typename W> struct PartsCarry {
     uint64_t obj_len;      // object bytes so far
     uint64_t part_size;    // the segment's part size (checked against every later call)
-    uint32_t part_raw;     // raw CRC-32C of the open part's bytes (obj_len % part_size of them)
-    uint32_t obj_raw;      // raw CRC-32C of the object so far
-    uint64_t reserved;
+    W raw[16 / sizeof(W)]; // [0]: raw CRC of the open part's bytes (obj_len % part_size of them); [1]: of the object so far
 };
-static_assert(sizeof(PartsCarry) == sizeof(tsgpu_parts_cursor), "the cursor holds the carry");
+static_assert(sizeof(PartsCarry<uint32_t>) == sizeof(tsgpu_parts_cursor) && sizeof(PartsCarry<uint64_t>) == sizeof(tsgpu_parts_cursor),
+              "the cursor holds the carry");
+
+// Names of the checksum arguments in messages.
+template <typename W> constexpr const char* crc_arg() { return sizeof(W) == 8 ? "crc64" : "crc32c"; }
 
 // One batch of a tsgpu_transform_parts call, L packed bytes: words[k] is the raw CRC of [0, x_k) of the batch,
 // x_k = first + k * part_size for k < m (the part boundaries strictly inside it), x_m = L.
-struct PcrcBatch { uint32_t L = 0, first = 0, m = 0; std::vector<uint32_t> words; };
-struct PartsRun {
+template <typename W> struct PcrcBatch { uint32_t L = 0, first = 0, m = 0; std::vector<W> words; };
+template <typename W> struct PartsRun {
     uint64_t part_size = 0;
-    uint64_t obj0 = 0;                 // object bytes before the call
-    std::vector<PcrcBatch> batches;    // by batch index
+    uint64_t obj0 = 0;                    // object bytes before the call
+    std::vector<PcrcBatch<W>> batches;    // by batch index
 };
 
-static int parts_alloc(PcrcScratch& r, uint64_t cap, rt::stream_t st) {
+template <typename W>
+static int parts_alloc(PcrcScratch<W>& r, uint64_t cap, rt::stream_t st) {
     if (r.cap >= cap) return TSGPU_OK;
     rt::free_device(r.d); r.d = nullptr; r.cap = 0;
     const uint64_t np = (cap + PCRC_PIECE - 1) / PCRC_PIECE, nt = (cap + PCRC_TILE - 1) / PCRC_TILE;
-    const uint64_t sz[3] = {4 * np, 4 * nt, 4};
+    const uint64_t sz[3] = {sizeof(W) * np, sizeof(W) * nt, 4};
     uint64_t total = 0;
     for (uint64_t b : sz) total += align_up(b, 256);
     RT(rt::malloc_device((void**)&r.d, total));
     uint8_t* p = r.d;
     auto take = [&](uint64_t b) { uint8_t* q = p; p += align_up(b, 256); return q; };
-    r.a.pin = (uint32_t*)take(sz[0]); r.a.ttot = (uint32_t*)take(sz[1]); r.a.done = (uint32_t*)take(sz[2]);
+    r.a.pin = (W*)take(sz[0]); r.a.ttot = (W*)take(sz[1]); r.a.done = (uint32_t*)take(sz[2]);
     RT(rt::memset_async(r.a.done, 0, 4, st));
     r.cap = cap;
     return TSGPU_OK;
 }
 
 // Enqueues pcrc_tiles over the batch's packed chunks (d_pack, sizes `len` on the device, at most `bound` bytes in all).
+template <typename W>
 static int parts_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint32_t* len, uint32_t nb, uint64_t bound) {
-    { int rc = parts_alloc(w.pcrc, (uint64_t)c->max_batch * c->slot_stride, st); if (rc) return rc; }
-    PcrcArgs& a = w.pcrc.a;
+    { int rc = parts_alloc(pcrc_of<W>(w), (uint64_t)c->max_batch * c->slot_stride, st); if (rc) return rc; }
+    PcrcArgs<W>& a = pcrc_of<W>(w).a;
     a.b = w.d_pack; a.len = len; a.nb = nb;
     const uint32_t grid = (uint32_t)std::min<uint64_t>(PCRC_GRID, (bound + PCRC_TILE - 1) / PCRC_TILE);
-    TS_LAUNCH_P(c->prof, "pcrc_tiles", pcrc_tiles_kernel<false>, dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
+    TS_LAUNCH_P(c->prof, sizeof(W) == 8 ? "pcrc64_tiles" : "pcrc_tiles", (pcrc_tiles_kernel<W, false>), dim3(std::max(grid, 1u)),
+                dim3(PCRC_T), 0, st, a);
     CHECK_LAUNCH("pcrc_tiles_kernel");
     return TSGPU_OK;
 }
 
 // The prefixes of the slot's previous batch are on the host once this slot's sizes event has completed: the batch's first
 // kernel that rewrites d_pack waited for the previous copy-out (wait_copies_out), and pcrc_cuts and its D2H precede that copy.
-static void parts_collect(Work& w, PartsRun& pr) {
-    PcrcScratch& p = w.pcrc;
+template <typename W>
+static void parts_collect(Work& w, PartsRun<W>& pr) {
+    PcrcScratch<W>& p = pcrc_of<W>(w);
     if (p.pending < 0) return;
-    PcrcBatch& b = pr.batches[(size_t)p.pending];
+    PcrcBatch<W>& b = pr.batches[(size_t)p.pending];
     b.words.assign(p.h_cuts, p.h_cuts + b.m + 1);
     p.pending = -1;
 }
 
 // At the drain of batch `bi` (L packed bytes at object offset `at`): pcrc_cuts and the D2H of its m + 1 words on out_stream,
 // ahead of the batch's copy-out.
-static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun& pr, uint32_t bi, uint64_t at, uint64_t L) {
+template <typename W>
+static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun<W>& pr, uint32_t bi, uint64_t at, uint64_t L) {
     parts_collect(w, pr);
-    PcrcScratch& p = w.pcrc;
+    PcrcScratch<W>& p = pcrc_of<W>(w);
     const uint64_t P = pr.part_size;
     const uint64_t first = P - at % P;                                   // the first part boundary after the batch's start
     const uint32_t m = first < L ? (uint32_t)((L - 1 - first) / P + 1) : 0;
     if (m + 1 > p.cuts_cap) {                                            // nothing on the slot reads the old arrays any more
         rt::free_device(p.d_cuts); rt::free_host(p.h_cuts); p.d_cuts = nullptr; p.h_cuts = nullptr; p.cuts_cap = 0;
         const uint32_t cap = std::max<uint32_t>(64, m + 1);
-        RT(rt::malloc_device((void**)&p.d_cuts, 4ull * cap));
-        RT(rt::malloc_host((void**)&p.h_cuts, 4ull * cap));
+        RT(rt::malloc_device((void**)&p.d_cuts, sizeof(W) * cap));
+        RT(rt::malloc_host((void**)&p.h_cuts, sizeof(W) * cap));
         p.cuts_cap = cap;
     }
-    TS_LAUNCH_P(c->prof, "pcrc_cuts", pcrc_cuts_kernel<false>, dim3((m + PCRC_CUTS_T) / PCRC_CUTS_T), dim3(PCRC_CUTS_T), 0, w.out_stream,
-                p.a, (uint32_t)L, m ? (uint32_t)first : 0u, P, m, p.d_cuts);
+    TS_LAUNCH_P(c->prof, sizeof(W) == 8 ? "pcrc64_cuts" : "pcrc_cuts", (pcrc_cuts_kernel<W, false>), dim3((m + PCRC_CUTS_T) / PCRC_CUTS_T),
+                dim3(PCRC_CUTS_T), 0, w.out_stream, p.a, (uint32_t)L, m ? (uint32_t)first : 0u, P, m, p.d_cuts);
     CHECK_LAUNCH("pcrc_cuts_kernel");
-    RT(rt::d2h(p.h_cuts, p.d_cuts, 4ull * (m + 1), w.out_stream));
-    PcrcBatch& b = pr.batches[bi];
+    RT(rt::d2h(p.h_cuts, p.d_cuts, sizeof(W) * (m + 1), w.out_stream));
+    PcrcBatch<W>& b = pr.batches[bi];
     b.L = (uint32_t)L; b.first = m ? (uint32_t)first : 0u; b.m = m; b.words.clear();
     p.pending = (int32_t)bi;
     return TSGPU_OK;
 }
 
 // The call's batches in order: their pieces extend the open part and the object; a part whose last byte arrives is emitted.
-static void parts_combine(const PartsRun& pr, PartsCarry& cur, std::vector<uint32_t>& emitted) {
+template <typename W>
+static void parts_combine(const PartsRun<W>& pr, PartsCarry<W>& cur, std::vector<W>& emitted) {
     const uint64_t P = pr.part_size;
-    for (const PcrcBatch& b : pr.batches) {
-        uint32_t prev = 0, prev_x = 0;
+    for (const PcrcBatch<W>& b : pr.batches) {
+        W prev = 0;
+        uint32_t prev_x = 0;
         for (uint32_t k = 0; k <= b.m; k++) {
             const uint32_t x = k < b.m ? (uint32_t)(b.first + k * P) : b.L;
             const uint32_t n = x - prev_x;
-            const uint32_t raw = b.words[k] ^ crc_shift(prev, n, 0);      // raw CRC of [prev_x, x)
-            cur.part_raw = crc_shift(cur.part_raw, n, 0) ^ raw;
+            const W raw = b.words[k] ^ crc_shift(prev, n, 0);             // raw CRC of [prev_x, x)
+            cur.raw[0] = crc_shift(cur.raw[0], n, 0) ^ raw;
             cur.obj_len += n;
-            if (n && cur.obj_len % P == 0) { emitted.push_back(crc_finish(cur.part_raw, P, 0)); cur.part_raw = 0; }
+            if (n && cur.obj_len % P == 0) { emitted.push_back(crc_finish(cur.raw[0], P, 0)); cur.raw[0] = 0; }
             prev = b.words[k]; prev_x = x;
         }
-        cur.obj_raw = crc_shift(cur.obj_raw, b.L, 0) ^ b.words[b.m];
+        cur.raw[1] = crc_shift(cur.raw[1], b.L, 0) ^ b.words[b.m];
     }
 }
 
@@ -760,8 +778,9 @@ static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
 // The target half of a batch whose original chunks are `orig` in d_orig (each at most cs bytes): [zstd ->] [AES-GCM encrypt]
 // with the keys `k`, or with `kept` the batch's frames in the d_frames slots (b_off, b_len; frames_max bytes at most) as they are
 // [-> AES-GCM encrypt]; the transformed chunks packed into d_pack, [pcrc_tiles over them,] [the verify stage and the D2H of its
-// verdicts to h_sizes + nb.]  `fin` receives the transformed chunks in their slots.
-static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, bool verify, bool parts, uint32_t c0,
+// verdicts to h_sizes + nb.]  `fin` receives the transformed chunks in their slots.  `parts`: the bytes of the part checksums'
+// CRC word (4: CRC-32C, 8: CRC-64/NVME), 0 without part checksums.
+static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, bool verify, int parts, uint32_t c0,
                         uint32_t nb, uint32_t cs, const Aes256RoundKeys& rk, uint32_t aad_len, ChunksIn orig, bool kept,
                         uint64_t frames_max, ChunksOut& fin) {
     const bool aes = flags & TSGPU_FLAG_AES;
@@ -793,7 +812,10 @@ static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint
         const uint64_t longest = payload + 28;
         TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
         CHECK_LAUNCH("pack_chunks_kernel");
-        if (parts) { int rc = parts_stage(c, w, st, fin.len, nb, longest * nb); if (rc) return rc; }
+        if (parts) {
+            int rc = parts == 8 ? parts_stage<uint64_t>(c, w, st, fin.len, nb, longest * nb) : parts_stage<uint32_t>(c, w, st, fin.len, nb, longest * nb);
+            if (rc) return rc;
+        }
     }
     if (verify) {
         int rc = verify_stage(c, w, k, st, flags, nb, cs, payload, rk, aad_len, fin);
@@ -806,7 +828,7 @@ static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint
 
 // One batch: copy in, fill the descriptors, the target half, [the record kernels,] D2H of the transformed sizes.
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
-static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, bool parts, const uint8_t* src, const uint64_t* off,
+static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, int parts, const uint8_t* src, const uint64_t* off,
                            const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
                            const uint8_t* ivs) {
     Work& w = *bt.w;
@@ -859,10 +881,11 @@ static int verify_verdict(const Batch& bt, const uint32_t* len, uint64_t first =
     return TSGPU_OK;
 }
 
+template <typename W = uint32_t>
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                             const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
-                            RecCarry* records, PartsRun* parts = nullptr);
+                            RecCarry* records, PartsRun<W>* parts = nullptr);
 
 static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint8_t* key, const uint8_t* aad,
                              uint32_t aad_len, const uint8_t* ivs, uint32_t* transformed_sizes, uint32_t* n_chunks) {
@@ -877,15 +900,16 @@ static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
 }
 
 static_assert(sizeof(tsgpu_records_cursor) == sizeof(RecCarry), "the cursor holds the carry");
-// The part-checksum arguments of tsgpu_transform_parts.
-struct PartsReq {
+// The part-checksum arguments of tsgpu_transform_parts (and its _crc64 twin).
+template <typename W> struct PartsReq {
     uint64_t part_size; tsgpu_parts_cursor* cursor;
-    uint32_t* crcs; uint32_t cap; uint32_t* n; uint32_t* object_crc;
+    W* crcs; uint32_t cap; uint32_t* n; W* object_crc;
 };
+template <typename W = uint32_t>
 static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
                              const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
                              uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
-                             bool env_default, const struct PartsReq* parts = nullptr);
+                             bool env_default, const PartsReq<W>* parts = nullptr);
 
 extern "C" int tsgpu_transform(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
                                const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
@@ -912,49 +936,64 @@ extern "C" int tsgpu_transform_parts(tsgpu_ctx* c, uint32_t flags, const uint8_t
                                      tsgpu_records_cursor* records, int segment_ends_here,
                                      uint64_t part_size, tsgpu_parts_cursor* parts,
                                      uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts, uint32_t* object_crc32c) {
-    const PartsReq req{part_size, parts, part_crc32c, part_cap, n_parts, object_crc32c};
+    const PartsReq<uint32_t> req{part_size, parts, part_crc32c, part_cap, n_parts, object_crc32c};
+    return transform_segment(c, flags, src, src_len, chunk_size, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, n_chunks,
+                             records, segment_ends_here, /*env_default=*/true, &req);
+}
+
+extern "C" int tsgpu_transform_parts_crc64(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
+                                           const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                                           uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
+                                           tsgpu_records_cursor* records, int segment_ends_here,
+                                           uint64_t part_size, tsgpu_parts_cursor* parts,
+                                           uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts, uint64_t* object_crc64) {
+    const PartsReq<uint64_t> req{part_size, parts, part_crc64, part_cap, n_parts, object_crc64};
     return transform_segment(c, flags, src, src_len, chunk_size, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, n_chunks,
                              records, segment_ends_here, /*env_default=*/true, &req);
 }
 
 // The part-checksum arguments, checked before any GPU work.  `bound`: the most bytes the call can add to the object.
-static int parts_args_ok(const PartsReq& q, uint32_t flags, uint64_t bound, int segment_ends_here) {
+template <typename W>
+static int parts_args_ok(const PartsReq<W>& q, uint32_t flags, uint64_t bound, int segment_ends_here) {
     if (!(flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)))
-        return fail(TSGPU_E_ARG, "tsgpu_transform_parts needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU");
+        return fail(TSGPU_E_ARG, "%s needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU",
+                    sizeof(W) == 8 ? "tsgpu_transform_parts_crc64" : "tsgpu_transform_parts");
     if (q.part_size == 0) return fail(TSGPU_E_ARG, "part_size must be at least 1");
-    if (!q.cursor || !q.n || !q.object_crc) return fail(TSGPU_E_ARG, "parts cursor, n_parts and object_crc32c cannot be null");
-    PartsCarry cur;
+    if (!q.cursor || !q.n || !q.object_crc) return fail(TSGPU_E_ARG, "parts cursor, n_parts and object_%s cannot be null", crc_arg<W>());
+    PartsCarry<W> cur;
     memcpy(&cur, q.cursor, sizeof cur);
     if (cur.obj_len && cur.part_size != q.part_size)
         return fail(TSGPU_E_ARG, "part_size %llu differs from the %llu the object started with", (unsigned long long)q.part_size,
                     (unsigned long long)cur.part_size);
     const uint64_t most = (cur.obj_len % q.part_size + bound) / q.part_size + (segment_ends_here ? 1 : 0);
-    if (most > q.cap) return fail(TSGPU_E_SHORT, "part_crc32c too small: the call may complete %llu parts, part_cap is %u",
-                                  (unsigned long long)most, q.cap);
-    if (q.cap && !q.crcs) return fail(TSGPU_E_ARG, "part_crc32c cannot be null");
+    if (most > q.cap) return fail(TSGPU_E_SHORT, "part_%s too small: the call may complete %llu parts, part_cap is %u",
+                                  crc_arg<W>(), (unsigned long long)most, q.cap);
+    if (q.cap && !q.crcs) return fail(TSGPU_E_ARG, "part_%s cannot be null", crc_arg<W>());
     return TSGPU_OK;
 }
 
 // After a successful call: the completed parts (and at the segment's end the open part and the object CRC) go out, and the
-// cursor moves on.  Nothing is written before: a failed call leaves part_crc32c and object_crc32c as they were.
-static void parts_finish(const PartsReq& q, PartsCarry cur, const PartsRun* run, int segment_ends_here) {
-    std::vector<uint32_t> emitted;
+// cursor moves on.  Nothing is written before: a failed call leaves the part and object checksums as they were.
+template <typename W>
+static void parts_finish(const PartsReq<W>& q, PartsCarry<W> cur, const PartsRun<W>* run, int segment_ends_here) {
+    std::vector<W> emitted;
     if (run) parts_combine(*run, cur, emitted);
     cur.part_size = q.part_size;
     if (segment_ends_here) {
         const uint64_t open = cur.obj_len % q.part_size;
-        if (open) { emitted.push_back(crc_finish(cur.part_raw, open, 0)); cur.part_raw = 0; }
-        *q.object_crc = crc_finish(cur.obj_raw, cur.obj_len, 0);
+        if (open) { emitted.push_back(crc_finish(cur.raw[0], open, 0)); cur.raw[0] = 0; }
+        *q.object_crc = crc_finish(cur.raw[1], cur.obj_len, 0);
     }
-    if (!emitted.empty()) memcpy(q.crcs, emitted.data(), 4 * emitted.size());
+    if (!emitted.empty()) memcpy(q.crcs, emitted.data(), sizeof(W) * emitted.size());
     *q.n = (uint32_t)emitted.size();
     memcpy(q.cursor, &cur, sizeof cur);
 }
 
+template <typename W>
 static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
                              const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
                              uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
-                             bool env_default, const PartsReq* parts) try {
+                             bool env_default, const PartsReq<W>* parts) try {
     int rc = transform_args_ok(c, flags, src, src_len, key, aad, aad_len, ivs, transformed_sizes, n_chunks);
     if (rc) return rc;
     const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
@@ -965,7 +1004,7 @@ static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     if (records && !cursor) return fail(TSGPU_E_ARG, "cursor cannot be null when record batches are validated");
     RecCarry carry{};
     if (records) memcpy(&carry, cursor, sizeof carry);
-    PartsCarry pcarry{};
+    PartsCarry<W> pcarry{};
     if (parts) {
         rc = parts_args_ok(*parts, flags, src_len ? tsgpu_transform_bound(flags, src_len, chunk_size) : 0, segment_ends_here);
         if (rc) return rc;
@@ -976,7 +1015,7 @@ static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     if (src_len == 0) {
         if (records && segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
         *n_chunks = 0;
-        if (parts) parts_finish(*parts, pcarry, nullptr, segment_ends_here);
+        if (parts) parts_finish<W>(*parts, pcarry, nullptr, segment_ends_here);
         return TSGPU_OK;
     }
     if (cs64 > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk size %llu exceeds the context's max_chunk_bytes %u", (unsigned long long)cs64, c->chunk_cap);
@@ -991,7 +1030,7 @@ static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     std::vector<uint64_t> off(n64);
     std::vector<uint32_t> len(n64);
     for (uint64_t i = 0; i < n64; i++) { off[i] = i * cs; len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - i * cs); }
-    PartsRun run;
+    PartsRun<W> run;
     if (parts) { run.part_size = parts->part_size; run.obj0 = pcarry.obj_len; }
     rc = transform_common(c, flags & ~TSGPU_FLAG_VALIDATE_RECORDS, src, src_len, off, len, cs, key, aad, aad_len, ivs, dst, dst_cap,
                           transformed_sizes, n_chunks, records ? &carry : nullptr, parts ? &run : nullptr);
@@ -1029,10 +1068,11 @@ extern "C" int tsgpu_transform_chunks(tsgpu_ctx* c, uint32_t flags, const uint8_
     return transform_common(c, flags, src, total, off, len, mx, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, &cap, nullptr);
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
+template <typename W>
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                             const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
-                            RecCarry* records, PartsRun* parts) {
+                            RecCarry* records, PartsRun<W>* parts) {
     const uint32_t n = (uint32_t)len.size();
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
     if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~ZSTD_MODIFIERS;         // modifiers of ZSTD: meaningless (and harmless) without it
@@ -1050,9 +1090,10 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
 
     uint64_t dst_off = 0;
-    if (parts) parts->batches.assign((n + c->max_batch - 1) / c->max_batch, PcrcBatch{});
+    if (parts) parts->batches.assign((n + c->max_batch - 1) / c->max_batch, PcrcBatch<W>{});
+    const int parts_word = parts ? (int)sizeof(W) : 0;
     const int rc = run_batches(c, n,
-        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, records != nullptr, parts != nullptr, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
+        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, records != nullptr, parts_word, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
         [&](const Batch& bt) {
             Work& w = *bt.w;
             if (records) { int rcr = records_resolve(c, w, *records); if (rcr) return rcr; }   // the input first: none of the batch's bytes leave
@@ -1066,7 +1107,7 @@ static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, ui
             return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);     // one copy per batch: packed on the device
         },
         [&](const std::vector<Work*>& slots, int rcb) {                     // the last batches' part prefixes, once all is idle
-            if (parts) for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, *parts); w->pcrc.pending = -1; }
+            if (parts) for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, *parts); pcrc_of<W>(*w).pending = -1; }
             return rcb;
         });
     if (rc) return rc;
@@ -1189,17 +1230,19 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
 // drain (source_drain), in object order: tag and frame statuses, decoded sizes against the chunk index, the record verdict, then
 // the words extend the cursor's CRCs.
 
-// The state of an object between calls: the public tsgpu_check_cursor (128 bytes, zero = start of the object).
-struct CheckCarry {
+// The state of an object between calls: the public tsgpu_check_cursor (128 bytes, zero = start of the object).  CRC-64/NVME's
+// wider words take 8 of the 32 bytes CRC-32C leaves reserved.
+template <typename W> struct CheckCarry {
     uint64_t chunks;       // chunks checked so far
     uint64_t obj_len;      // object bytes so far
     uint64_t seg_len;      // decoded segment bytes so far
-    uint32_t obj_raw;      // raw CRC-32C of the object so far
-    uint32_t seg_raw;      //   ... and of the decoded segment so far
+    W obj_raw;             // raw CRC of the object so far
+    W seg_raw;             //   ... and of the decoded segment so far
     RecCarry rec;          // TSGPU_FLAG_VALIDATE_RECORDS
-    uint64_t reserved[4];
+    uint64_t reserved[sizeof(W) == 8 ? 3 : 4];
 };
-static_assert(sizeof(CheckCarry) == sizeof(tsgpu_check_cursor), "the cursor holds the carry");
+static_assert(sizeof(CheckCarry<uint32_t>) == sizeof(tsgpu_check_cursor) && sizeof(CheckCarry<uint64_t>) == sizeof(tsgpu_check_cursor),
+              "the cursor holds the carry");
 
 // The chunk index of the manifest (AbstractChunkIndex.materializeChunks): ceil(ofs / ocs) chunks of ocs original bytes, the
 // last one holding the remainder; an empty segment has none.
@@ -1222,7 +1265,7 @@ struct SourceReq {
 
 static int source_args(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
                        uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size, const uint8_t* key,
-                       const uint8_t* aad, uint32_t aad_len, const CheckCarry& cur, SourceReq& q) {
+                       const uint8_t* aad, uint32_t aad_len, uint64_t chunks_before, SourceReq& q) {
     if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VALIDATE_RECORDS)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
     if (n_chunks && !transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
     if (original_chunk_size == 0) return fail(TSGPU_E_ARG, "Original chunk size must be positive, 0 given");
@@ -1247,33 +1290,35 @@ static int source_args(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_
     q.index = ChunkLayout{original_chunk_size, original_file_size, (original_file_size + original_chunk_size - 1) / original_chunk_size};
     // The index of an empty segment materialises one chunk of 0 transformed bytes: a caller that walks it passes that chunk.
     q.n = n_chunks;
-    if (q.index.count == 0 && cur.chunks == 0 && q.n == 1 && transformed_sizes[0] == 0) q.n = 0;
+    if (q.index.count == 0 && chunks_before == 0 && q.n == 1 && transformed_sizes[0] == 0) q.n = 0;
     q.rk = Aes256RoundKeys{};
     if (q.flags & TSGPU_FLAG_AES) q.rk = aes256_expand_key(key);
     q.aad = aad; q.aad_len = aad_len;
     return TSGPU_OK;
 }
 
-// The raw CRC-32C of a batch's L bytes into pcrc.d_cuts[k]: pcrc_tiles, then pcrc_cuts without part boundaries.
-template <bool SLOTS>
+// The raw CRC of a batch's L bytes into pcrc.d_cuts[k]: pcrc_tiles, then pcrc_cuts without part boundaries.
+template <typename W, bool SLOTS>
 static int check_crc_word(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint8_t* b, const uint64_t* off, const uint32_t* len,
                           uint32_t nb, uint64_t L, uint32_t k) {
-    PcrcScratch& p = w.pcrc;
+    PcrcScratch<W>& p = pcrc_of<W>(w);
     { int rc = parts_alloc(p, (uint64_t)c->max_batch * c->slot_stride, st); if (rc) return rc; }
     if (!p.d_cuts) {
-        RT(rt::malloc_device((void**)&p.d_cuts, 4ull * 64));
-        RT(rt::malloc_host((void**)&p.h_cuts, 4ull * 64));
+        RT(rt::malloc_device((void**)&p.d_cuts, sizeof(W) * 64));
+        RT(rt::malloc_host((void**)&p.h_cuts, sizeof(W) * 64));
         p.cuts_cap = 64;
     }
     p.a.b = b; p.a.len = len; p.a.nb = nb;
-    PcrcIn<SLOTS> a{};
-    static_cast<PcrcArgs&>(a) = p.a;
+    PcrcIn<W, SLOTS> a{};
+    static_cast<PcrcArgs<W>&>(a) = p.a;
     if constexpr (SLOTS) a.off = off;
     const uint32_t grid = (uint32_t)std::min<uint64_t>(PCRC_GRID, (L + PCRC_TILE - 1) / PCRC_TILE);
-    TS_LAUNCH_P(c->prof, SLOTS ? "pcrc_tiles_slots" : "pcrc_tiles", pcrc_tiles_kernel<SLOTS>, dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
+    const bool w64 = sizeof(W) == 8;
+    TS_LAUNCH_P(c->prof, SLOTS ? (w64 ? "pcrc64_tiles_slots" : "pcrc_tiles_slots") : (w64 ? "pcrc64_tiles" : "pcrc_tiles"),
+                (pcrc_tiles_kernel<W, SLOTS>), dim3(std::max(grid, 1u)), dim3(PCRC_T), 0, st, a);
     CHECK_LAUNCH("pcrc_tiles_kernel");
-    TS_LAUNCH_P(c->prof, SLOTS ? "pcrc_cuts_slots" : "pcrc_cuts", pcrc_cuts_kernel<SLOTS>, dim3(1), dim3(PCRC_CUTS_T), 0, st,
-                a, (uint32_t)L, 0u, (uint64_t)1, 0u, p.d_cuts + k);
+    TS_LAUNCH_P(c->prof, SLOTS ? (w64 ? "pcrc64_cuts_slots" : "pcrc_cuts_slots") : (w64 ? "pcrc64_cuts" : "pcrc_cuts"),
+                (pcrc_cuts_kernel<W, SLOTS>), dim3(1), dim3(PCRC_CUTS_T), 0, st, a, (uint32_t)L, 0u, (uint64_t)1, 0u, p.d_cuts + k);
     CHECK_LAUNCH("pcrc_cuts_kernel");
     return TSGPU_OK;
 }
@@ -1282,8 +1327,9 @@ static int check_crc_word(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint8_t*
 // chunk.  A zstd-only object's frames go to the d_frames slots with to_frames, else in place in d_xf.  Chunk i decodes to
 // d_orig + a_off[i], the offset the chunk index gives it, and v_len[i] holds its size by the index: what later stages read, so a
 // damaged chunk cannot steer them (its batch fails at the drain).  The descriptor block is uploaded here: a caller fills its
-// other fields first.  out[0, nb) receives the decoded sizes, out[nb, 2 nb) the statuses, out[2 nb, 2 nb + 2) the object and
-// segment words.
+// other fields first.  out[0, nb) receives the decoded sizes, out[nb, 2 nb) the statuses, and the 2 sizeof(W) bytes from
+// out + 2 nb the object and segment words.
+template <typename W>
 static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, const SourceReq& q, const uint8_t* src, uint64_t g0,
                         bool to_frames, uint32_t* out) {
     const uint32_t nb = bt.nb, flags = q.flags;
@@ -1317,14 +1363,14 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
     { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
     if (flags) {
         const ChunksIn in = to_frames ? ChunksIn{w.d_frames, w.dd.b_off, w.dd.b_len} : ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len};
-        { int rc = check_crc_word<true>(c, w, st, in.base, in.off, in.len, nb, obj, 0); if (rc) return rc; }
+        { int rc = check_crc_word<W, true>(c, w, st, in.base, in.off, in.len, nb, obj, 0); if (rc) return rc; }
         RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
         int rc = detransform_enqueue(c, w, w.keys[0], st, flags, nb, q.rk, q.aad_len, in, ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len},
                                      w.dd.status, lim, /*packed=*/false);
         if (rc) return rc;
     }
     // The segment word and the records over the L bytes the index gives: a batch that decodes to another length fails first.
-    { int rc = check_crc_word<false>(c, w, st, w.d_orig, nullptr, w.dd.v_len, nb, L, 1); if (rc) return rc; }
+    { int rc = check_crc_word<W, false>(c, w, st, w.d_orig, nullptr, w.dd.v_len, nb, L, 1); if (rc) return rc; }
     if (q.records && L) {
         int rc = records_alloc(w.rec, (uint64_t)c->max_batch * q.index.ocs);
         if (!rc) rc = records_stage(c, w, st, L);
@@ -1334,13 +1380,14 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
         RT(rt::d2h(out, w.dd.a_len, 4ull * nb, st));
         RT(rt::d2h(out + nb, w.dd.status, 4ull * nb, st));
     }
-    RT(rt::d2h(out + 2 * nb, w.pcrc.d_cuts, 8, st));
+    RT(rt::d2h(out + 2 * nb, pcrc_of<W>(w).d_cuts, 2 * sizeof(W), st));
     return TSGPU_OK;
 }
 
 // A drained batch in object order (`out` as source_stage filled it): every chunk's tag, frame and decoded size, then the record
 // verdict, then the CRC words extend the carry.
-static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const uint32_t* out, CheckCarry& cur) {
+template <typename W>
+static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const uint32_t* out, CheckCarry<W>& cur) {
     Work& w = *bt.w;
     const uint32_t nb = bt.nb;
     const uint32_t* got = out;
@@ -1360,7 +1407,9 @@ static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const
         obj += q.tsizes[bt.c0 + i];
     }
     if (q.records) { int rc = records_resolve(c, w, cur.rec); if (rc) return rc; }
-    const uint32_t seg_word = out[2 * nb + 1], obj_word = q.flags ? out[2 * nb] : seg_word;
+    W words[2];                                                        // 4-byte aligned only
+    memcpy(words, out + 2 * nb, sizeof words);
+    const W seg_word = words[1], obj_word = q.flags ? words[0] : seg_word;
     cur.obj_raw = crc_shift(cur.obj_raw, obj, 0) ^ obj_word;
     cur.seg_raw = crc_shift(cur.seg_raw, L, 0) ^ seg_word;
     return TSGPU_OK;
@@ -1368,7 +1417,8 @@ static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const
 
 // After a window's batches: the carry moves past its chunks, and at the object's end the chunk count and the last record entry
 // are checked.
-static int source_finish(const SourceReq& q, CheckCarry& cur, int object_ends_here) {
+template <typename W>
+static int source_finish(const SourceReq& q, CheckCarry<W>& cur, int object_ends_here) {
     cur.chunks += q.n;
     cur.obj_len += q.need;
     for (uint32_t i = 0; i < q.n; i++) cur.seg_len += q.index.size(cur.chunks - q.n + i);
@@ -1380,18 +1430,20 @@ static int source_finish(const SourceReq& q, CheckCarry& cur, int object_ends_he
     return TSGPU_OK;
 }
 
-extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
-                                  uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
-                                  const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
-                                  tsgpu_check_cursor* cursor, int object_ends_here, uint32_t* object_crc32c, uint32_t* segment_crc32c) try {
+template <typename W>
+static int check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                        uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size, const uint8_t key[32],
+                        const uint8_t* aad, uint32_t aad_len, tsgpu_check_cursor* cursor, int object_ends_here, W* object_crc,
+                        W* segment_crc) try {
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
     if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
-    if (object_ends_here && (!object_crc32c || !segment_crc32c)) return fail(TSGPU_E_ARG, "object_crc32c/segment_crc32c cannot be null");
-    CheckCarry cur;
+    if (object_ends_here && (!object_crc || !segment_crc))
+        return fail(TSGPU_E_ARG, "object_%s/segment_%s cannot be null", crc_arg<W>(), crc_arg<W>());
+    CheckCarry<W> cur;
     memcpy(&cur, cursor, sizeof cur);
     SourceReq q;
     int rc = source_args(c, flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, key, aad, aad_len,
-                         cur, q);
+                         cur.chunks, q);
     if (rc) return rc;
     if (q.n) {
         uint64_t in_off = 0;                                     // batches are issued in order: in_off walks src with them
@@ -1399,7 +1451,7 @@ extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* s
             [&](const Batch& bt) {
                 Work& w = *bt.w;
                 RT(rt::set_device(w.device));
-                const int r = source_stage(c, w, w.stream, bt, q, src + in_off, cur.chunks, /*to_frames=*/false, w.h_sizes);
+                const int r = source_stage<W>(c, w, w.stream, bt, q, src + in_off, cur.chunks, /*to_frames=*/false, w.h_sizes);
                 for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
                 if (r) return r;
                 RT(rt::event_record(w.ev_sizes, w.stream));
@@ -1410,12 +1462,28 @@ extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* s
     }
     if ((rc = source_finish(q, cur, object_ends_here))) return rc;
     if (object_ends_here) {
-        *object_crc32c = crc_finish(cur.obj_raw, cur.obj_len, 0);
-        *segment_crc32c = crc_finish(cur.seg_raw, cur.seg_len, 0);
+        *object_crc = crc_finish(cur.obj_raw, cur.obj_len, 0);
+        *segment_crc = crc_finish(cur.seg_raw, cur.seg_len, 0);
     }
     memcpy(cursor, &cur, sizeof cur);
     return TSGPU_OK;
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
+
+extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                                  uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
+                                  const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
+                                  tsgpu_check_cursor* cursor, int object_ends_here, uint32_t* object_crc32c, uint32_t* segment_crc32c) {
+    return check_object(c, flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, key, aad, aad_len,
+                        cursor, object_ends_here, object_crc32c, segment_crc32c);
+}
+
+extern "C" int tsgpu_check_object_crc64(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                                        uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
+                                        const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
+                                        tsgpu_check_cursor* cursor, int object_ends_here, uint64_t* object_crc64, uint64_t* segment_crc64) {
+    return check_object(c, flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, key, aad, aad_len,
+                        cursor, object_ends_here, object_crc64, segment_crc64);
+}
 
 // ------------------------------------------------------------------------------------------ object rewrite (host)
 // tsgpu_rewrite_object: the source half of the check, then the target half of the transform (target_stage) from the decoded
@@ -1426,12 +1494,13 @@ extern "C" int tsgpu_check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* s
 // chunks' sizes, part prefixes and copy-out.
 
 // The state of a rewrite between calls: the public tsgpu_rewrite_cursor (192 bytes, zero = start of the object).
-struct RewriteCarry {
-    CheckCarry src;        // the old object and the decoded segment
-    PartsCarry out;        // the new object's parts
+template <typename W> struct RewriteCarry {
+    CheckCarry<W> src;         // the old object and the decoded segment
+    tsgpu_parts_cursor out;    // the new object's parts (a PartsCarry<W>)
     uint64_t reserved[4];
 };
-static_assert(sizeof(RewriteCarry) == sizeof(tsgpu_rewrite_cursor), "the cursor holds the carry");
+static_assert(sizeof(RewriteCarry<uint32_t>) == sizeof(tsgpu_rewrite_cursor) && sizeof(RewriteCarry<uint64_t>) == sizeof(tsgpu_rewrite_cursor),
+              "the cursor holds the carry");
 
 // The new object's side of a rewrite.
 struct TargetReq {
@@ -1443,7 +1512,9 @@ struct TargetReq {
 };
 
 // One batch of a rewrite: the target's IVs and AAD, the source half, the target half, the D2H of the new sizes.  h_sizes:
-// [0, nb) new sizes, [nb, 3 nb) the verify stage's verdicts (verify_verdict), [3 nb, 5 nb + 2) the source half's out.
+// [0, nb) new sizes, [nb, 3 nb) the verify stage's verdicts (verify_verdict), [3 nb, 5 nb + 2 sizeof(W) / 4) the source half's
+// out (its two CRC words take 2 or 4 of the 16 words h_sizes has beyond 5 nb).
+template <typename W>
 static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const TargetReq& t, const uint8_t* src, uint64_t g0) {
     Work& w = *bt.w;
     const uint32_t nb = bt.nb;
@@ -1462,32 +1533,31 @@ static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, cons
             RT(rt::h2d(k.d_aad, k.h_aad, t.aad_len, st));
         }
     }
-    { int rc = source_stage(c, w, st, bt, q, src, g0, /*to_frames=*/q.flags == TSGPU_FLAG_ZSTD, w.h_sizes + 3 * nb); if (rc) return rc; }
+    { int rc = source_stage<W>(c, w, st, bt, q, src, g0, /*to_frames=*/q.flags == TSGPU_FLAG_ZSTD, w.h_sizes + 3 * nb); if (rc) return rc; }
     uint64_t frames_max = 0;                 // the largest kept frame, by the object's sizes
     for (uint32_t i = 0; i < nb; i++) {
         const uint32_t ts = q.tsizes[bt.c0 + i];
         frames_max = std::max<uint64_t>(frames_max, (q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts);
     }
     ChunksOut fin;
-    { int rc = target_stage(c, w, k, st, t.flags, t.verify, /*parts=*/true, bt.c0, nb, q.index.ocs, t.rk, t.aad_len,
+    { int rc = target_stage(c, w, k, st, t.flags, t.verify, /*parts=*/(int)sizeof(W), bt.c0, nb, q.index.ocs, t.rk, t.aad_len,
                             ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, t.kept, frames_max, fin); if (rc) return rc; }
     RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
     return TSGPU_OK;
 }
 
-extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src, uint64_t src_len,
-                                    const uint32_t* transformed_sizes, uint32_t n_chunks, uint32_t original_chunk_size,
-                                    uint64_t original_file_size, const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
-                                    uint32_t to_flags, const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len,
-                                    const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
-                                    uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
-                                    tsgpu_rewrite_cursor* cursor, int object_ends_here,
-                                    uint32_t* source_crc32c, uint32_t* object_crc32c, uint32_t* segment_crc32c) try {
+template <typename W>
+static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                          uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size, const uint8_t from_key[32],
+                          const uint8_t* from_aad, uint32_t from_aad_len, uint32_t to_flags, const uint8_t to_key[32],
+                          const uint8_t* to_aad, uint32_t to_aad_len, const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap,
+                          uint32_t* new_transformed_sizes, uint64_t part_size, W* part_crc, uint32_t part_cap, uint32_t* n_parts,
+                          tsgpu_rewrite_cursor* cursor, int object_ends_here, W* source_crc, W* object_crc, W* segment_crc) try {
     if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
     if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
-    if (object_ends_here && (!source_crc32c || !segment_crc32c))
-        return fail(TSGPU_E_ARG, "source_crc32c/object_crc32c/segment_crc32c cannot be null");
+    if (object_ends_here && (!source_crc || !segment_crc))
+        return fail(TSGPU_E_ARG, "source_%s/object_%s/segment_%s cannot be null", crc_arg<W>(), crc_arg<W>(), crc_arg<W>());
     const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
     if (to_flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY)) return fail(TSGPU_E_ARG, "unknown to_flags %u", to_flags);
     if (!(to_flags & xf))
@@ -1503,11 +1573,11 @@ extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uin
     if ((to_flags & TSGPU_FLAG_AES) && to_aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "to_aad longer than %u bytes", MAX_AAD);
     if ((to_flags & TSGPU_FLAG_AES) && to_aad_len && !to_aad) return fail(TSGPU_E_ARG, "to_aad cannot be null");
     if (n_chunks && !new_transformed_sizes) return fail(TSGPU_E_ARG, "new_transformed_sizes cannot be null");
-    RewriteCarry cur;
+    RewriteCarry<W> cur;
     memcpy(&cur, cursor, sizeof cur);
     SourceReq q;
     int rc = source_args(c, from_flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size,
-                         from_key, from_aad, from_aad_len, cur.src, q);
+                         from_key, from_aad, from_aad_len, cur.src.chunks, q);
     if (rc) return rc;
     if (q.n && !dst) return fail(TSGPU_E_ARG, "dst cannot be null");
     // GCM breaks when one key encrypts two plaintexts under one IV: no two chunks of the window may share a new IV, nor, under
@@ -1546,7 +1616,7 @@ extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uin
         frames += ((q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts) + ((to_flags & TSGPU_FLAG_AES) ? 28 : 0);
     }
     const uint64_t bound = !q.n ? 0 : kept ? frames : tsgpu_transform_bound(to_flags, L, original_chunk_size);
-    const PartsReq pq{part_size, (tsgpu_parts_cursor*)&cur.out, part_crc32c, part_cap, n_parts, object_crc32c};
+    const PartsReq<W> pq{part_size, &cur.out, part_crc, part_cap, n_parts, object_crc};
     if ((rc = parts_args_ok(pq, to_flags, bound, object_ends_here))) return rc;
 
     TargetReq t{};
@@ -1555,16 +1625,18 @@ extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uin
     t.kept = kept;
     if (to_flags & TSGPU_FLAG_AES) t.rk = aes256_expand_key(to_key);
     t.aad = to_aad; t.aad_len = to_aad_len; t.ivs = to_ivs;
-    PartsRun run;
-    run.part_size = part_size; run.obj0 = cur.out.obj_len;
+    PartsRun<W> run;
+    PartsCarry<W> out0;
+    memcpy(&out0, &cur.out, sizeof out0);
+    run.part_size = part_size; run.obj0 = out0.obj_len;
     if (q.n) {
         std::vector<uint32_t> len(q.n);                          // the window's original sizes (verify_verdict's messages)
         for (uint32_t i = 0; i < q.n; i++) len[i] = q.index.size(cur.src.chunks + i);
-        run.batches.assign((q.n + c->max_batch - 1) / c->max_batch, PcrcBatch{});
+        run.batches.assign((q.n + c->max_batch - 1) / c->max_batch, PcrcBatch<W>{});
         uint64_t in_off = 0, dst_off = 0;                        // batches are issued in order: in_off walks src with them
         rc = run_batches(c, q.n,
             [&](const Batch& bt) {
-                const int r = rewrite_issue(c, bt, q, t, src + in_off, cur.src.chunks);
+                const int r = rewrite_issue<W>(c, bt, q, t, src + in_off, cur.src.chunks);
                 for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
                 return r;
             },
@@ -1581,21 +1653,47 @@ extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uin
                 return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);
             },
             [&](const std::vector<Work*>& slots, int rcb) {          // the last batches' part prefixes, once all is idle
-                for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, run); w->pcrc.pending = -1; }
+                for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, run); pcrc_of<W>(*w).pending = -1; }
                 return rcb;
             });
         if (rc) return rc;
     }
     if ((rc = source_finish(q, cur.src, object_ends_here))) return rc;
     if (n_chunks && !q.n) new_transformed_sizes[0] = 0;                    // the empty segment's one empty chunk stays one
-    parts_finish(pq, cur.out, q.n ? &run : nullptr, object_ends_here);     // writes cur.out and the part CRCs
+    parts_finish(pq, out0, q.n ? &run : nullptr, object_ends_here);       // writes cur.out and the part CRCs
     if (object_ends_here) {
-        *source_crc32c = crc_finish(cur.src.obj_raw, cur.src.obj_len, 0);
-        *segment_crc32c = crc_finish(cur.src.seg_raw, cur.src.seg_len, 0);
+        *source_crc = crc_finish(cur.src.obj_raw, cur.src.obj_len, 0);
+        *segment_crc = crc_finish(cur.src.seg_raw, cur.src.seg_len, 0);
     }
     memcpy(cursor, &cur, sizeof cur);
     return TSGPU_OK;
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
+
+extern "C" int tsgpu_rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src, uint64_t src_len,
+                                    const uint32_t* transformed_sizes, uint32_t n_chunks, uint32_t original_chunk_size,
+                                    uint64_t original_file_size, const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                                    uint32_t to_flags, const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len,
+                                    const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                                    uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
+                                    tsgpu_rewrite_cursor* cursor, int object_ends_here,
+                                    uint32_t* source_crc32c, uint32_t* object_crc32c, uint32_t* segment_crc32c) {
+    return rewrite_object(c, from_flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, from_key,
+                          from_aad, from_aad_len, to_flags, to_key, to_aad, to_aad_len, to_ivs, dst, dst_cap, new_transformed_sizes,
+                          part_size, part_crc32c, part_cap, n_parts, cursor, object_ends_here, source_crc32c, object_crc32c, segment_crc32c);
+}
+
+extern "C" int tsgpu_rewrite_object_crc64(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src, uint64_t src_len,
+                                          const uint32_t* transformed_sizes, uint32_t n_chunks, uint32_t original_chunk_size,
+                                          uint64_t original_file_size, const uint8_t from_key[32], const uint8_t* from_aad,
+                                          uint32_t from_aad_len, uint32_t to_flags, const uint8_t to_key[32], const uint8_t* to_aad,
+                                          uint32_t to_aad_len, const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap,
+                                          uint32_t* new_transformed_sizes, uint64_t part_size, uint64_t* part_crc64, uint32_t part_cap,
+                                          uint32_t* n_parts, tsgpu_rewrite_cursor* cursor, int object_ends_here,
+                                          uint64_t* source_crc64, uint64_t* object_crc64, uint64_t* segment_crc64) {
+    return rewrite_object(c, from_flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, from_key,
+                          from_aad, from_aad_len, to_flags, to_key, to_aad, to_aad_len, to_ivs, dst, dst_cap, new_transformed_sizes,
+                          part_size, part_crc64, part_cap, n_parts, cursor, object_ends_here, source_crc64, object_crc64, segment_crc64);
+}
 
 // ------------------------------------------------------------------------------------------ device-resident API
 // The device API reuses slot 0's pinned descriptor block and scratch arenas.  Two events make back-to-back calls safe on

@@ -16,6 +16,7 @@
 namespace tieredstorage {
 
 struct ObjectCheck { uint32_t objectCrc32c, segmentCrc32c; };
+struct ObjectCheck64 { uint64_t objectCrc64nvme, segmentCrc64nvme; };     // check64: CRC-64/NVME (S3 CRC64NVME)
 
 class RemoteSegmentChecker {
 public:
@@ -30,6 +31,21 @@ public:
     // std::runtime_error (RuntimeException in the reference) for a failed tag, a bad frame, a size that disagrees with the index
     // or a short fetch; the message is the library's.
     ObjectCheck check(const SegmentManifestV1& manifest, const RangeFetcher& fetcher, const DataKeyAndAAD* key) const {
+        ObjectCheck out{0, 0};
+        run(manifest, fetcher, key, tsgpu_check_object, &out.objectCrc32c, &out.segmentCrc32c);
+        return out;
+    }
+    // check with the CRC-64/NVME of the object and of the decoded segment (tsgpu_check_object_crc64).
+    ObjectCheck64 check64(const SegmentManifestV1& manifest, const RangeFetcher& fetcher, const DataKeyAndAAD* key) const {
+        ObjectCheck64 out{0, 0};
+        run(manifest, fetcher, key, tsgpu_check_object_crc64, &out.objectCrc64nvme, &out.segmentCrc64nvme);
+        return out;
+    }
+
+private:
+    template <typename W, typename Call>
+    void run(const SegmentManifestV1& manifest, const RangeFetcher& fetcher, const DataKeyAndAAD* key, Call call, W* objectCrc,
+             W* segmentCrc) const {
         if (!fetcher) throw NullPointerException("objectKey cannot be null");
         if (!manifest.chunkIndex) throw NullPointerException("chunkIndex cannot be null");
         const bool encrypted = manifest.aad.has_value();
@@ -40,7 +56,6 @@ public:
         const ChunkIndex& index = *manifest.chunkIndex;
         const std::vector<Chunk>& chunks = index.chunks();
         tsgpu_check_cursor cursor{};
-        ObjectCheck out{0, 0};
         for (size_t k = 0;; k += window) {
             const size_t e = std::min(chunks.size(), k + window);
             const bool end = e == chunks.size();
@@ -52,19 +67,18 @@ public:
                 const BytesRange range = transformedRange(part);
                 if (!range.isEmpty()) bytes = fetcher(range);
             }
-            const int rc = tsgpu_check_object(ctx, flags, bytes.data(), bytes.size(), sizes.data(), (uint32_t)sizes.size(),
+            const int rc = call(ctx, flags, bytes.data(), bytes.size(), sizes.data(), (uint32_t)sizes.size(),
                                               (uint32_t)index.originalChunkSize, (uint64_t)index.originalFileSize,
                                               encrypted ? key->dataKey.data() : nullptr, encrypted ? key->aad.data() : nullptr,
                                               encrypted ? (uint32_t)key->aad.size() : 0u, &cursor, end ? 1 : 0,
-                                              &out.objectCrc32c, &out.segmentCrc32c);
+                                              objectCrc, segmentCrc);
             if (rc == TSGPU_E_RECORDS) throw InvalidRecordBatchException(tsgpu_last_error());
             if (rc == TSGPU_E_ARG) throw IllegalArgumentException(tsgpu_last_error());
             if (rc) throw std::runtime_error(tsgpu_last_error());
-            if (end) return out;
+            if (end) return;
         }
     }
 
-private:
     tsgpu_ctx* ctx;
     uint32_t window;
 };

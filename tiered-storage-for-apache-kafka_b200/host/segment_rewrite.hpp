@@ -27,6 +27,8 @@ struct SegmentRewrite {
     uint32_t sourceCrc32c = 0;                   // CRC-32C of the old `.log` object (compare with the store's checksum of it)
     uint32_t objectCrc32c = 0;                   // CRC-32C of the new `.log` object (S3 FULL_OBJECT, GCS crc32c)
     uint32_t segmentCrc32c = 0;                  // CRC-32C of the decoded segment (the same for both objects)
+    // With RemoteSegmentRewriter::crc64 the three words are CRC-64/NVME (S3 CRC64NVME) here instead, and the 32-bit ones stay 0.
+    uint64_t sourceCrc64nvme = 0, objectCrc64nvme = 0, segmentCrc64nvme = 0;
 };
 
 class RemoteSegmentRewriter {
@@ -43,6 +45,9 @@ public:
     }
     bool validateRecords = false;        // also check every record batch of the decoded segment (TSGPU_FLAG_VALIDATE_RECORDS)
     bool verify = false;                 // read every new batch back on the GPU before it leaves (TSGPU_FLAG_VERIFY)
+    // CRC-64/NVME instead of CRC-32C (tsgpu_rewrite_object_crc64): every part reaches the sink with crc64nvme, and the result
+    // carries the 64-bit words.  The new object's bytes are the same.
+    bool crc64 = false;
 
     // `oldKey`: the old manifest's unwrapped data key and AAD, or null when it has no encryption.  `newKey`: the new data key
     // (DataKeyAndAAD) when encryptionEnabled; `ivs`: 12 random bytes per chunk of the segment and `indexIvs` 12 per non-empty
@@ -72,11 +77,13 @@ public:
         r.compressed = compressionEnabled;
         std::vector<int32_t> sizes;                  // the new object's chunk sizes
         Bytes pending;                               // bytes of the open part
-        std::vector<uint32_t> crcs;                  // CRCs of the parts not yet handed to the sink
+        std::vector<uint64_t> crcs;                  // CRCs of the parts not yet handed to the sink
         int partNumber = 0;
         uint64_t sent = 0;
-        auto emit = [&](uint64_t n, uint32_t crc) {
-            const UploadPart p{++partNumber, sent, n, crc};
+        auto emit = [&](uint64_t n, uint64_t crc) {
+            UploadPart p{++partNumber, sent, n};
+            if (crc64) p.crc64nvme = crc;
+            else p.crc32c = (uint32_t)crc;
             sink(p, pending.data());
             pending.erase(pending.begin(), pending.begin() + (ptrdiff_t)n);
             sent += n;
@@ -98,9 +105,22 @@ public:
                                                     (uint64_t)bytes.size() + 28 * tsz.size()) + 28 * tsz.size() + 64;
             Bytes out(cap);
             std::vector<uint32_t> nsz(std::max<size_t>(tsz.size(), 1));
-            std::vector<uint32_t> windowCrcs((pending.size() + cap) / partSize + 2);
+            const size_t partCap = (pending.size() + cap) / partSize + 2;
+            std::vector<uint32_t> windowCrcs(crc64 ? 0 : partCap);
+            std::vector<uint64_t> windowCrcs64(crc64 ? partCap : 0);
             uint32_t nParts = 0, src = 0, obj = 0, seg = 0;
-            const int rc = tsgpu_rewrite_object(ctx, from, bytes.data(), bytes.size(), tsz.data(), (uint32_t)tsz.size(), ocs,
+            uint64_t src64 = 0, obj64 = 0, seg64 = 0;
+            const int rc = crc64
+                ? tsgpu_rewrite_object_crc64(ctx, from, bytes.data(), bytes.size(), tsz.data(), (uint32_t)tsz.size(), ocs,
+                                             (uint64_t)index.originalFileSize, encrypted ? oldKey->dataKey.data() : nullptr,
+                                             encrypted ? oldKey->aad.data() : nullptr, encrypted ? (uint32_t)oldKey->aad.size() : 0u,
+                                             to, encryptionEnabled ? newKey->dataKey.data() : nullptr,
+                                             encryptionEnabled ? newKey->aad.data() : nullptr,
+                                             encryptionEnabled ? (uint32_t)newKey->aad.size() : 0u,
+                                             encryptionEnabled ? ivs + 12 * k : nullptr, out.data(), out.size(), nsz.data(),
+                                             partSize, windowCrcs64.data(), (uint32_t)partCap, &nParts, &cursor,
+                                             end ? 1 : 0, &src64, &obj64, &seg64)
+                : tsgpu_rewrite_object(ctx, from, bytes.data(), bytes.size(), tsz.data(), (uint32_t)tsz.size(), ocs,
                                                 (uint64_t)index.originalFileSize, encrypted ? oldKey->dataKey.data() : nullptr,
                                                 encrypted ? oldKey->aad.data() : nullptr, encrypted ? (uint32_t)oldKey->aad.size() : 0u,
                                                 to, encryptionEnabled ? newKey->dataKey.data() : nullptr,
@@ -116,7 +136,8 @@ public:
             for (size_t i = 0; i < tsz.size(); i++) { sizes.push_back((int32_t)nsz[i]); produced += nsz[i]; }
             pending.insert(pending.end(), out.begin(), out.begin() + (ptrdiff_t)produced);
             r.objectBytes += produced;
-            crcs.insert(crcs.end(), windowCrcs.begin(), windowCrcs.begin() + nParts);
+            if (crc64) crcs.insert(crcs.end(), windowCrcs64.begin(), windowCrcs64.begin() + nParts);
+            else crcs.insert(crcs.end(), windowCrcs.begin(), windowCrcs.begin() + nParts);
             size_t c = 0;
             for (; c < crcs.size() && pending.size() >= partSize; c++) emit(partSize, crcs[c]);
             if (end && !pending.empty() && c < crcs.size()) emit(pending.size(), crcs[c++]);
@@ -124,6 +145,7 @@ public:
             if (end) {
                 if (!pending.empty() || !crcs.empty()) throw std::runtime_error("part checksums do not match the new object");
                 r.sourceCrc32c = src; r.objectCrc32c = obj; r.segmentCrc32c = seg;
+                r.sourceCrc64nvme = src64; r.objectCrc64nvme = obj64; r.segmentCrc64nvme = seg64;
                 break;
             }
         }

@@ -147,7 +147,12 @@ private:
 
 // S3MultiPartOutputStream: the object goes out in parts of exactly partSize bytes, the last one may be shorter.  With
 // SegmentLogUploader::partChecksums a part carries the CRC-32C of its bytes, computed on the GPU (tsgpu_transform_parts).
-struct UploadPart { int partNumber; uint64_t offset; uint64_t size; std::optional<uint32_t> crc32c = std::nullopt; };
+// With SegmentLogUploader::crc64Parts the part carries the CRC-64/NVME of its bytes instead (tsgpu_transform_parts_crc64).
+struct UploadPart {
+    int partNumber; uint64_t offset; uint64_t size;
+    std::optional<uint32_t> crc32c = std::nullopt;
+    std::optional<uint64_t> crc64nvme = std::nullopt;
+};
 inline std::vector<UploadPart> multipartPlan(uint64_t objectBytes, uint64_t partSize) {
     if (partSize == 0) throw IllegalArgumentException("partSize must be positive");
     std::vector<UploadPart> parts;
@@ -166,6 +171,7 @@ struct SegmentLogUpload {
     bool compressed = false;
     std::vector<int32_t> transformedSizes;
     std::optional<uint32_t> objectCrc32c;                // with partChecksums: CRC-32C of the whole object (S3 FULL_OBJECT, GCS crc32c)
+    std::optional<uint64_t> objectCrc64nvme;             // with partChecksums and crc64Parts: CRC-64/NVME of the whole object (S3 CRC64NVME)
 };
 class SegmentLogUploader {
 public:
@@ -186,6 +192,9 @@ public:
     // part (S3 x-amz-checksum-crc32c, GCS crc32c; INTEGRATION.md), so damage on any later hop is refused by the object store.
     // Like validateRecords it applies when the segment is compressed or encrypted; otherwise no byte reaches the GPU.
     bool partChecksums = false;
+    // With partChecksums: CRC-64/NVME instead of CRC-32C (tsgpu_transform_parts_crc64), for S3's CRC64NVME and, unverified,
+    // Azure's x-ms-content-crc64: the parts carry crc64nvme and the result objectCrc64nvme.  The object's bytes are the same.
+    bool crc64Parts = false;
     // `log`/`n`: the segment file (ideally in memory from tsgpu_host_alloc); `ivs`: 12 bytes per chunk when encrypting.
     SegmentLogUpload upload(const uint8_t* log, uint64_t n, const DataKeyAndAAD* key, const uint8_t* ivs, const PartSink& sink) {
         if (n > 0x7fffffffull) throw IllegalArgumentException("originalFileSize must fit an int");
@@ -208,18 +217,29 @@ public:
         uint32_t got = (uint32_t)sizes.size();
         const bool checksums = partChecksums && flags;
         std::vector<uint32_t> partCrcs;
+        std::vector<uint64_t> partCrcs64;
         uint32_t objectCrc = 0;
+        uint64_t objectCrc64 = 0;
         int rc;
         if (checksums) {
             if (partSize == 0) throw IllegalArgumentException("partSize must be positive");
             tsgpu_records_cursor records{};
             tsgpu_parts_cursor parts{};
-            partCrcs.resize(bound / partSize + 2);
             uint32_t nParts = 0;
-            rc = tsgpu_transform_parts(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
-                                       key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got, &records, 1,
-                                       partSize, &parts, partCrcs.data(), (uint32_t)partCrcs.size(), &nParts, &objectCrc);
-            partCrcs.resize(rc ? 0 : nParts);
+            if (crc64Parts) {
+                partCrcs64.resize(bound / partSize + 2);
+                rc = tsgpu_transform_parts_crc64(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr,
+                                                 key ? key->aad.data() : nullptr, key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound,
+                                                 sizes.data(), &got, &records, 1, partSize, &parts, partCrcs64.data(),
+                                                 (uint32_t)partCrcs64.size(), &nParts, &objectCrc64);
+                partCrcs64.resize(rc ? 0 : nParts);
+            } else {
+                partCrcs.resize(bound / partSize + 2);
+                rc = tsgpu_transform_parts(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
+                                           key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got, &records, 1,
+                                           partSize, &parts, partCrcs.data(), (uint32_t)partCrcs.size(), &nParts, &objectCrc);
+                partCrcs.resize(rc ? 0 : nParts);
+            }
         } else {
             rc = tsgpu_transform(ctx, callFlags, log, n, cs, key ? key->dataKey.data() : nullptr, key ? key->aad.data() : nullptr,
                                  key ? (uint32_t)key->aad.size() : 0u, ivs, dst, bound, sizes.data(), &got);
@@ -243,7 +263,11 @@ public:
             r.chunkIndex = b.finish((int)sizes[got - 1]);
         }
         std::vector<UploadPart> plan = multipartPlan(r.objectBytes, partSize);
-        if (checksums) {
+        if (checksums && crc64Parts) {
+            if (partCrcs64.size() != plan.size()) throw std::runtime_error("part checksums do not match the multipart plan");
+            for (size_t i = 0; i < plan.size(); i++) plan[i].crc64nvme = partCrcs64[i];
+            r.objectCrc64nvme = objectCrc64;
+        } else if (checksums) {
             if (partCrcs.size() != plan.size()) throw std::runtime_error("part checksums do not match the multipart plan");
             for (size_t i = 0; i < plan.size(); i++) plan[i].crc32c = partCrcs[i];
             r.objectCrc32c = objectCrc;
