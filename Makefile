@@ -72,3 +72,9 @@ tests/cpp/test_crc64_mirror_simt: tests/cpp/test_crc64_mirror.cpp $(PKG)/host/ch
 # JNI glue's CRC-64/NVME exports (Crc64.transformParts, checkObject, rewriteObject), same fake JNIEnv
 tests/cpp/test_jni_crc64_simt: tests/cpp/test_jni_crc64.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so
 	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_crc64.c -Ltests/simt -ltsgpu_simt -Wl,-rpath,'$$ORIGIN/../simt'
+# Host mirror of TSGPU_FLAG_REFRAME (RemoteSegmentRewriter::addChecksums, ::denseFrames) on an oracle-written object, on the emulator build
+tests/cpp/test_reframe_mirror_simt: tests/cpp/test_reframe_mirror.cpp $(PKG)/host/chunk_transform.hpp $(PKG)/host/segment_upload.hpp $(PKG)/host/segment_check.hpp $(PKG)/host/segment_rewrite.hpp include/tsgpu.h tests/simt/libtsgpu_simt.so oracle
+	g++ -O1 -g -std=c++17 -o $@ tests/cpp/test_reframe_mirror.cpp -Ltests/simt -ltsgpu_simt -Loracle -ltsoracle -Wl,-rpath,'$$ORIGIN/../simt' -Wl,-rpath,'$$ORIGIN/../../oracle'
+# JNI glue's REFRAME path (RewriteCursor.rewriteObject with TsGpu.FLAG_REFRAME) on an oracle-written object, same fake JNIEnv
+tests/cpp/test_jni_reframe_simt: tests/cpp/test_jni_reframe.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so oracle
+	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_reframe.c -Ltests/simt -ltsgpu_simt -Loracle -ltsoracle -Wl,-rpath,'$$ORIGIN/../simt' -Wl,-rpath,'$$ORIGIN/../../oracle'

@@ -69,6 +69,26 @@ extern "C" {
  * window of a segment (a window checked as a whole segment would fail where an entry crosses its end).  Cost and memory:
  * DESIGN.md §3 and §8. */
 #define TSGPU_FLAG_VALIDATE_RECORDS 32u
+/* to_flags of tsgpu_rewrite_object and tsgpu_rewrite_object_crc64 only (every other call refuses it as an unknown bit): when
+ * from_flags and to_flags both have TSGPU_FLAG_ZSTD, the ZSTD_CHECKSUM and ZSTD_DENSE bits of to_flags act on the source frames
+ * instead of being refused.  It needs ZSTD on both sides and one of the two bits, else TSGPU_E_ARG.
+ *   REFRAME | ZSTD_CHECKSUM (seal): every source frame is kept byte for byte, except that Frame_Header_Descriptor bit 2 is set
+ *     and the 4-byte Content_Checksum of the chunk is inserted after its last block; skippable frames that followed it in the
+ *     chunk move 4 bytes on.  That is the frame libzstd writes for the same blocks with its checksum flag, so objects the Java
+ *     plugin wrote keep their level-3 density.  A frame that already has a checksum (verified by the source decode) is kept as
+ *     it is.  Clearing the bit and dropping the 4 bytes gives back the old frame.
+ *   REFRAME | ZSTD_DENSE [| ZSTD_CHECKSUM] (re-encode): every chunk is also compressed anew by the dense compressor, with a
+ *     checksum if asked, and the new frame replaces the old one only when it is strictly smaller than what the old frame
+ *     becomes (sealed with CHECKSUM, else unchanged).  No chunk grows by more than the 4 checksum bytes.  Without
+ *     ZSTD_CHECKSUM a dense frame carries no checksum, so it can replace a frame that had one: add ZSTD_CHECKSUM when the source
+ *     may hold checksummed frames.
+ * Only the bits given count: the context's TSGPU_ZSTD_MODE=dense and TSGPU_ZSTD_CHECKSUM=1 do not add to them.  REFRAME turns
+ * TSGPU_FLAG_VERIFY on, so every new chunk is decoded again, and its new checksum checked, before its batch leaves: a chunk the
+ * first decode misread by chance fails the call with TSGPU_E_VERIFY instead of being sealed with the checksum of wrong bytes.
+ * A misread that repeats is caught by TSGPU_FLAG_VALIDATE_RECORDS on the source, which a caller sealing objects should set.
+ * The part_cap bound and dst grow by 4 bytes per chunk with ZSTD_CHECKSUM, and a chunk whose sealed frame would not fit the
+ * context's frame slot (tsgpu_transform_bound of max_chunk_bytes) fails with TSGPU_E_ARG before any GPU work.  Cost: DESIGN.md §8. */
+#define TSGPU_FLAG_REFRAME 64u
 
 #define TSGPU_IV_SIZE   12     /* SegmentEncryptionMetadataV1.java:30 */
 #define TSGPU_TAG_SIZE  16     /* AesEncryptionProvider.java:38 (128-bit tag) */
@@ -270,13 +290,13 @@ int tsgpu_check_object(tsgpu_ctx* ctx, uint32_t flags,
  *   the cursor walk and the empty-segment rule are those of tsgpu_check_object (flags 0 is a plain object; VALIDATE_RECORDS
  *   checks every record batch).  Every source chunk passes all of that call's checks before any byte of its batch is released.
  * Target side:
- *   to_flags       TSGPU_FLAG_ZSTD, ZSTD_DENSE, ZSTD_CHECKSUM, AES and VERIFY; it must contain ZSTD or AES (the plain object is
+ *   to_flags       TSGPU_FLAG_ZSTD, ZSTD_DENSE, ZSTD_CHECKSUM, AES, VERIFY and REFRAME; it must contain ZSTD or AES (the plain object is
  *                  what tsgpu_detransform gives).  Any other bit fails with TSGPU_E_ARG.  New chunk i holds the same original
  *                  bytes as old chunk i: the chunk size and the file size do not change.
  *                  When both from_flags and to_flags have ZSTD, every source frame goes into the new object byte for byte (it
  *                  is still decoded, for the size, record and segment-CRC checks, but not re-encoded: objects the Java plugin
  *                  wrote are libzstd level 3, denser than this library's speed mode).  ZSTD_DENSE or ZSTD_CHECKSUM then fail with
- *                  TSGPU_E_ARG, having nothing to act on.  Only a source without ZSTD is compressed, by the selected compressor.
+ *                  TSGPU_E_ARG, having nothing to act on, unless TSGPU_FLAG_REFRAME is set: it seals or re-encodes the frames.  Only a source without ZSTD is compressed, by the selected compressor.
  *                  The context's TSGPU_ZSTD_MODE=dense and TSGPU_ZSTD_CHECKSUM=1 act where a chunk is compressed, and
  *                  TSGPU_VERIFY=1 turns on VERIFY, as for tsgpu_transform_parts.
  *   to_key, to_aad, to_ivs   with AES: the new data key, AAD and one 12-byte IV per chunk of the window.  One GCM key must never
@@ -290,7 +310,7 @@ int tsgpu_check_object(tsgpu_ctx* ctx, uint32_t flags,
  *                  part_cap >= floor((carried + B) / part_size) + (object_ends_here ? 1 : 0), B = tsgpu_transform_bound(to_flags,
  *                  L, original_chunk_size) with L the window's original bytes by the index -- or, when the frames are kept, the
  *                  window's exact new length (its frames, plus 28 bytes each with AES), which is no more for frames within the
- *                  zstd bound.  A smaller part_cap fails with TSGPU_E_SHORT before any GPU work.  A caller that uploads in one
+ *                  zstd bound; 4 bytes more per frame that TSGPU_FLAG_REFRAME seals.  A smaller part_cap fails with TSGPU_E_SHORT before any GPU work.  A caller that uploads in one
  *                  PUT passes a part_size no smaller than the object's bound.
  *   cursor         192 bytes, zeroed at the start of the object, passed to every window in order; updated on success, without a
  *                  defined value after a failure.

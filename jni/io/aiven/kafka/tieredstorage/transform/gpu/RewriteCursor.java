@@ -36,6 +36,9 @@ public final class RewriteCursor {
     /**
      * One window: old transformed chunks transformedSizes back to back in src.  fromFlags are the old manifest's (TsGpu.FLAG_ZSTD,
      * TsGpu.FLAG_AES), plus TsGpu.FLAG_VALIDATE_RECORDS; toFlags the new object's (FLAG_ZSTD and/or FLAG_AES, plus FLAG_VERIFY).
+     * When both have FLAG_ZSTD, TsGpu.FLAG_REFRAME with 16 (checksum) and/or 4 (dense) in toFlags seals the old frames with their
+     * Content_Checksum or re-encodes them when that makes them smaller: each new chunk is then up to 4 bytes longer than its old
+     * frame, so dst needs 4 more bytes per chunk.  Set FLAG_VALIDATE_RECORDS in fromFlags when sealing.
      * toIvs holds 12 bytes per chunk of the window when toFlags has FLAG_AES.  newTransformedSizes receives one size per chunk,
      * partCrcs the CRC-32C of the parts the window completes; returns their count.
      */

@@ -12,6 +12,10 @@ public final class TsGpu {
      *  FLAG_AES.  A damaged batch fails the call with a RuntimeException, so Kafka keeps the local segment and retries the
      *  copy.  Segments that arrive in windows carry the state from one window to the next in a {@link RecordsCursor}. */
     public static final int FLAG_VALIDATE_RECORDS = 32;
+    /** RewriteCursor only, with FLAG_ZSTD on both sides: seal the kept frames with their Content_Checksum (with 16,
+     *  TSGPU_FLAG_ZSTD_CHECKSUM) or re-encode them in dense mode when that is smaller (with 4, TSGPU_FLAG_ZSTD_DENSE); every new
+     *  chunk is then read back on the GPU before it leaves.  Every other call refuses it. */
+    public static final int FLAG_REFRAME = 64;
     public static final int IV_SIZE = 12;
 
     static {

@@ -6,5 +6,5 @@ surface and of the caller side of the copy path) and corpus.py (synthetic segmen
 The directory name has a hyphen, so import it through the `tsgpu` shim at the repo root or importlib.
 """
 from . import binding  # noqa: F401
-from .binding import (FLAG_AES, FLAG_VALIDATE_RECORDS, FLAG_VERIFY, FLAG_ZSTD, FLAG_ZSTD_CHECKSUM, FLAG_ZSTD_DENSE, IV_SIZE,  # noqa: F401
+from .binding import (FLAG_AES, FLAG_REFRAME, FLAG_VALIDATE_RECORDS, FLAG_VERIFY, FLAG_ZSTD, FLAG_ZSTD_CHECKSUM, FLAG_ZSTD_DENSE, IV_SIZE,  # noqa: F401
                       TAG_SIZE, Context, TsgpuError)

@@ -17,6 +17,7 @@ FLAG_ZSTD_DENSE = 4
 FLAG_VERIFY = 8          # host-buffer transforms: read each batch back on the device before releasing it
 FLAG_ZSTD_CHECKSUM = 16  # with FLAG_ZSTD: every frame ends with its Content_Checksum (XXH64 of the chunk, checked by every reader)
 FLAG_VALIDATE_RECORDS = 32  # segment transforms with ZSTD or AES: check every Kafka record batch's length, magic and CRC first
+FLAG_REFRAME = 64        # rewrite_object to_flags: seal (ZSTD_CHECKSUM) or re-encode (ZSTD_DENSE) the kept source frames
 IV_SIZE = 12
 TAG_SIZE = 16
 SLOT_HEAD = 4
@@ -337,7 +338,8 @@ class Context:
         n = ts.size
         # every chunk of the window at most a frame bound (or its source frame, when frames are kept) plus IV and tag
         per = int(self.lib.tsgpu_transform_bound(to_flags | FLAG_ZSTD, original_chunk_size, original_chunk_size)) + 28
-        cap = max(n * per, int(ts.sum(dtype=np.uint64)) + 28 * n) + 64
+        # (a frame TSGPU_FLAG_REFRAME seals is 4 bytes longer than its source frame)
+        cap = max(n * per, int(ts.sum(dtype=np.uint64)) + 32 * n) + 64
         dst = np.empty(cap, dtype=np.uint8)
         sizes = np.zeros(max(n, 1), dtype=np.uint32)
         if part_cap is None:

@@ -35,6 +35,7 @@
 #include "zstd_enc.cuh"
 #include "zstd_enc_blk.cuh"
 #include "zstd_dec.cuh"
+#include "reframe.cuh"
 #include "host_index.hpp"
 
 using namespace ts;
@@ -313,9 +314,8 @@ struct DxBounds {
 // zstd compress.  Two kernels, one contract (zstd_enc_blk.cuh: independent 8 KiB blocks, fastest; zstd_enc.cuh: 64 KiB
 // regions with shared tables and history, densest).  Their scratch is allocated the first time a slot runs the mode.
 // With the checksum either kernel also hashes every chunk, in extra CTAs of the same launch, and ends its frame with it.
-static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, ChunksIn in, uint32_t nb, uint32_t cs, ChunksOut out) {
-    const bool dense = (flags & TSGPU_FLAG_ZSTD_DENSE) || c->dense_default;
-    const bool checksum = (flags & TSGPU_FLAG_ZSTD_CHECKSUM) || c->checksum_default;
+static int zstd_stage_modes(tsgpu_ctx* c, Work& w, rt::stream_t st, bool dense, bool checksum, ChunksIn in, uint32_t nb, uint32_t cs,
+                            ChunksOut out) {
     int rc;
     if (dense) {
         if (!w.zenc.seqs) {
@@ -332,6 +332,11 @@ static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, Ch
     }
     if (rc) return fail(rc, "zstd compress: %s", zstd_last_error());
     return TSGPU_OK;
+}
+// The modifiers of `flags`, or the context's defaults.
+static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, ChunksIn in, uint32_t nb, uint32_t cs, ChunksOut out) {
+    return zstd_stage_modes(c, w, st, (flags & TSGPU_FLAG_ZSTD_DENSE) || c->dense_default,
+                            (flags & TSGPU_FLAG_ZSTD_CHECKSUM) || c->checksum_default, in, nb, cs, out);
 }
 
 // AES-GCM: key set-up, the main kernel over (ranges x chunks) and the finalize kernel.  IVs (ENC) come from the slot's
@@ -773,22 +778,61 @@ static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
     if (at < 0) at += n;
     if (at >= 0 && at < (long)n) fin.base[fin.off[i] + at] ^= 1;
 }
+// TEST-ONLY, as above: TSGPU_SIMT_FLIP_DECODED=<chunk>:<offset> flips the low bit of one byte of that chunk's decoded bytes in
+// d_orig right after the source decode of tsgpu_check_object / tsgpu_rewrite_object -- a decoder that misread the chunk.
+// tests/test_simt_reframe.py drives it: TSGPU_FLAG_REFRAME must not stamp the checksum of such a chunk.
+static void simt_flip_decoded(ChunksIn orig, uint32_t c0, uint32_t nb) {
+    const char* e = getenv("TSGPU_SIMT_FLIP_DECODED");
+    long k = 0, at = 0;
+    if (!e || sscanf(e, "%ld:%ld", &k, &at) != 2 || k < (long)c0 || k >= (long)c0 + (long)nb) return;
+    const uint32_t i = (uint32_t)(k - c0), n = orig.len[i];
+    if (at < 0) at += n;
+    if (at >= 0 && at < (long)n) const_cast<uint8_t*>(orig.base)[orig.off[i] + at] ^= 1;
+}
 #endif
+
+// TSGPU_FLAG_REFRAME (`reframe`: its ZSTD_DENSE and ZSTD_CHECKSUM bits) on the batch's kept frames in the d_frames slots (b_off,
+// b_len): with CHECKSUM each frame is sealed with the checksum of its decoded chunk in `orig`; with DENSE the dense compressor
+// writes every chunk anew into d_xf at the same slot offsets, and the smaller of the two frames stays in the slot.  d_xf is free
+// here: the source half read its encrypted chunks before, and the target half encrypts into it after.  b_len ends with each
+// slot's frame size.  XXH64 is a serial chain per chunk: the seal kernel takes one warp per chunk, and the other slots' batches
+// run beside it on their own streams.
+static int reframe_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t reframe, uint32_t nb, uint32_t cs, ChunksIn orig) {
+    ReframeArgs R;
+    R.frames = w.d_frames; R.f_off = w.dd.b_off; R.f_len = w.dd.b_len;
+    R.orig = orig.base; R.o_off = orig.off; R.o_len = orig.len;
+    R.cand = w.d_xf; R.cand_len = w.dd.c_len;
+    R.n = nb; R.room = (uint32_t)(c->frame_stride - 16);
+    const bool checksum = reframe & TSGPU_FLAG_ZSTD_CHECKSUM;
+    if (checksum) {
+        TS_LAUNCH_P(c->prof, "reframe_seal", reframe_seal_kernel, dim3((nb + RF_WPB - 1) / RF_WPB), dim3(RF_WPB * 32), 0, st, R);
+        CHECK_LAUNCH("reframe_seal_kernel");
+    }
+    if (reframe & TSGPU_FLAG_ZSTD_DENSE) {
+        int rc = zstd_stage_modes(c, w, st, /*dense=*/true, checksum, orig, nb, cs, ChunksOut{w.d_xf, w.dd.b_off, w.dd.c_len});
+        if (rc) return rc;
+        TS_LAUNCH_P(c->prof, "reframe_pick", reframe_pick_kernel, dim3(nb), dim3(RF_PICK_T), 0, st, R);
+        CHECK_LAUNCH("reframe_pick_kernel");
+    }
+    return TSGPU_OK;
+}
 
 // The target half of a batch whose original chunks are `orig` in d_orig (each at most cs bytes): [zstd ->] [AES-GCM encrypt]
 // with the keys `k`, or with `kept` the batch's frames in the d_frames slots (b_off, b_len; frames_max bytes at most) as they are
 // [-> AES-GCM encrypt]; the transformed chunks packed into d_pack, [pcrc_tiles over them,] [the verify stage and the D2H of its
 // verdicts to h_sizes + nb.]  `fin` receives the transformed chunks in their slots.  `parts`: the bytes of the part checksums'
-// CRC word (4: CRC-32C, 8: CRC-64/NVME), 0 without part checksums.
+// CRC word (4: CRC-32C, 8: CRC-64/NVME), 0 without part checksums.  `reframe`: with `kept`, the ZSTD_DENSE and ZSTD_CHECKSUM
+// bits TSGPU_FLAG_REFRAME applies to the kept frames first (reframe_stage); a sealed frame is 4 bytes longer than frames_max.
 static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, bool verify, int parts, uint32_t c0,
                         uint32_t nb, uint32_t cs, const Aes256RoundKeys& rk, uint32_t aad_len, ChunksIn orig, bool kept,
-                        uint64_t frames_max, ChunksOut& fin) {
+                        uint64_t frames_max, ChunksOut& fin, uint32_t reframe = 0) {
     const bool aes = flags & TSGPU_FLAG_AES;
     // encrypted chunks land in the transformed slots; zstd alone leaves its frames in the frame slots
     fin = aes ? ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len} : ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len};
     uint64_t payload;                        // the largest transformed chunk without IV and tag
     if (kept) {
-        payload = frames_max;
+        payload = frames_max + ((reframe & TSGPU_FLAG_ZSTD_CHECKSUM) ? 4 : 0);
+        if (reframe) { int rc = reframe_stage(c, w, st, reframe, nb, cs, orig); if (rc) return rc; }
         if (aes) {
             int rc = gcm_stage<true>(c, w, k, st, rk, ChunksIn{w.d_frames, w.dd.b_off, w.dd.b_len}, fin, aad_len, w.dd.status, nb,
                                      (uint32_t)payload, 0xffffffffu);
@@ -1368,6 +1412,9 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
         int rc = detransform_enqueue(c, w, w.keys[0], st, flags, nb, q.rk, q.aad_len, in, ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len},
                                      w.dd.status, lim, /*packed=*/false);
         if (rc) return rc;
+#ifdef TSGPU_SIMT
+        simt_flip_decoded(ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, bt.c0, nb);
+#endif
     }
     // The segment word and the records over the L bytes the index gives: a batch that decodes to another length fails first.
     { int rc = check_crc_word<W, false>(c, w, st, w.d_orig, nullptr, w.dd.v_len, nb, L, 1); if (rc) return rc; }
@@ -1506,6 +1553,7 @@ static_assert(sizeof(RewriteCarry<uint32_t>) == sizeof(tsgpu_rewrite_cursor) && 
 struct TargetReq {
     uint32_t flags;                  // ZSTD, modifiers and AES of the new object
     bool verify, kept;               // kept: the source frames go into the new object as they are
+    uint32_t reframe;                // TSGPU_FLAG_REFRAME: the ZSTD_DENSE and ZSTD_CHECKSUM bits that act on the kept frames, else 0
     Aes256RoundKeys rk;
     const uint8_t* aad; uint32_t aad_len;
     const uint8_t* ivs;
@@ -1541,7 +1589,7 @@ static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, cons
     }
     ChunksOut fin;
     { int rc = target_stage(c, w, k, st, t.flags, t.verify, /*parts=*/(int)sizeof(W), bt.c0, nb, q.index.ocs, t.rk, t.aad_len,
-                            ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, t.kept, frames_max, fin); if (rc) return rc; }
+                            ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, t.kept, frames_max, fin, t.reframe); if (rc) return rc; }
     RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
     return TSGPU_OK;
@@ -1559,13 +1607,19 @@ static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src,
     if (object_ends_here && (!source_crc || !segment_crc))
         return fail(TSGPU_E_ARG, "source_%s/object_%s/segment_%s cannot be null", crc_arg<W>(), crc_arg<W>(), crc_arg<W>());
     const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
-    if (to_flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY)) return fail(TSGPU_E_ARG, "unknown to_flags %u", to_flags);
+    if (to_flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY | TSGPU_FLAG_REFRAME)) return fail(TSGPU_E_ARG, "unknown to_flags %u", to_flags);
+    const bool kept = (from_flags & TSGPU_FLAG_ZSTD) && (to_flags & TSGPU_FLAG_ZSTD);
+    const bool reframe = to_flags & TSGPU_FLAG_REFRAME;
+    if (reframe && !kept)
+        return fail(TSGPU_E_ARG, "to_flags %u: TSGPU_FLAG_REFRAME acts on kept frames and needs TSGPU_FLAG_ZSTD in from_flags and "
+                    "to_flags", to_flags);
+    if (reframe && !(to_flags & ZSTD_MODIFIERS))
+        return fail(TSGPU_E_ARG, "to_flags %u: TSGPU_FLAG_REFRAME needs TSGPU_FLAG_ZSTD_DENSE or TSGPU_FLAG_ZSTD_CHECKSUM", to_flags);
     if (!(to_flags & xf))
         return fail(TSGPU_E_ARG, "to_flags needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: the plain object is what tsgpu_detransform gives");
     if (!(to_flags & TSGPU_FLAG_ZSTD) && (to_flags & ZSTD_MODIFIERS))
         return fail(TSGPU_E_ARG, "to_flags %u: TSGPU_FLAG_ZSTD_DENSE and TSGPU_FLAG_ZSTD_CHECKSUM need TSGPU_FLAG_ZSTD", to_flags);
-    const bool kept = (from_flags & TSGPU_FLAG_ZSTD) && (to_flags & TSGPU_FLAG_ZSTD);
-    if (kept && (to_flags & ZSTD_MODIFIERS))
+    if (kept && !reframe && (to_flags & ZSTD_MODIFIERS))
         return fail(TSGPU_E_ARG, "to_flags %u: the source frames are kept as they are, so TSGPU_FLAG_ZSTD_DENSE and "
                     "TSGPU_FLAG_ZSTD_CHECKSUM have nothing to act on", to_flags);
     if ((to_flags & TSGPU_FLAG_AES) && (!to_key || (n_chunks && !to_ivs)))
@@ -1608,21 +1662,30 @@ static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src,
             return fail(TSGPU_E_ARG, "to_ivs[%u] repeats to_ivs[%u]", std::min(x.i, y.i), std::max(x.i, y.i));
         }
     }
-    // part_cap: the transform bound of the window's length by the chunk index, or of its kept frames
+    // part_cap: the transform bound of the window's length by the chunk index, or of its kept frames (4 bytes more each when
+    // TSGPU_FLAG_REFRAME seals them: a dense frame replaces one only when it is smaller)
+    const uint32_t seal = (reframe && (to_flags & TSGPU_FLAG_ZSTD_CHECKSUM)) ? 4 : 0;
     uint64_t L = 0, frames = 0;
     for (uint32_t i = 0; i < q.n; i++) {
         L += q.index.size(cur.src.chunks + i);
         const uint32_t ts = transformed_sizes[i];
-        frames += ((q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts) + ((to_flags & TSGPU_FLAG_AES) ? 28 : 0);
+        const uint64_t frame = (q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts;
+        if (seal && frame + seal > c->frame_stride - 16)
+            return fail(TSGPU_E_ARG, "chunk %llu: its sealed frame of %llu bytes would not fit the context's frame slot of %llu bytes",
+                        (unsigned long long)(cur.src.chunks + i), (unsigned long long)(frame + seal),
+                        (unsigned long long)(c->frame_stride - 16));
+        frames += frame + seal + ((to_flags & TSGPU_FLAG_AES) ? 28 : 0);
     }
     const uint64_t bound = !q.n ? 0 : kept ? frames : tsgpu_transform_bound(to_flags, L, original_chunk_size);
     const PartsReq<W> pq{part_size, &cur.out, part_crc, part_cap, n_parts, object_crc};
     if ((rc = parts_args_ok(pq, to_flags, bound, object_ends_here))) return rc;
 
     TargetReq t{};
-    t.flags = to_flags & ~TSGPU_FLAG_VERIFY;
-    t.verify = (to_flags & TSGPU_FLAG_VERIFY) || c->verify_default;
+    t.flags = to_flags & ~(TSGPU_FLAG_VERIFY | TSGPU_FLAG_REFRAME);
+    // a reframed chunk is read back, and its new checksum checked, before its batch leaves: no checksum of a misread chunk leaves
+    t.verify = (to_flags & TSGPU_FLAG_VERIFY) || c->verify_default || reframe;
     t.kept = kept;
+    t.reframe = reframe ? to_flags & ZSTD_MODIFIERS : 0;
     if (to_flags & TSGPU_FLAG_AES) t.rk = aes256_expand_key(to_key);
     t.aad = to_aad; t.aad_len = to_aad_len; t.ivs = to_ivs;
     PartsRun<W> run;

@@ -45,6 +45,11 @@ public:
     }
     bool validateRecords = false;        // also check every record batch of the decoded segment (TSGPU_FLAG_VALIDATE_RECORDS)
     bool verify = false;                 // read every new batch back on the GPU before it leaves (TSGPU_FLAG_VERIFY)
+    // With compressionEnabled: every new frame carries its Content_Checksum (addChecksums), or comes from the dense compressor
+    // when that makes it smaller (denseFrames).  A compressed source's frames are sealed or re-encoded (TSGPU_FLAG_REFRAME, which
+    // also reads every new chunk back); a plain source is compressed with the ZSTD_CHECKSUM and ZSTD_DENSE modifiers.
+    bool addChecksums = false;
+    bool denseFrames = false;
     // CRC-64/NVME instead of CRC-32C (tsgpu_rewrite_object_crc64): every part reaches the sink with crc64nvme, and the result
     // carries the 64-bit words.  The new object's bytes are the same.
     bool crc64 = false;
@@ -67,8 +72,11 @@ public:
         if (encryptionEnabled && newKey->dataKey.size() != 32) throw IllegalArgumentException("dataKey must be 32 bytes");
         const uint32_t from = (manifest.compression ? TSGPU_FLAG_ZSTD : 0u) | (encrypted ? TSGPU_FLAG_AES : 0u) |
                               (validateRecords ? TSGPU_FLAG_VALIDATE_RECORDS : 0u);
+        const uint32_t modifiers = compressionEnabled ? (addChecksums ? TSGPU_FLAG_ZSTD_CHECKSUM : 0u) |
+                                                        (denseFrames ? TSGPU_FLAG_ZSTD_DENSE : 0u) : 0u;
         const uint32_t to = (compressionEnabled ? TSGPU_FLAG_ZSTD : 0u) | (encryptionEnabled ? TSGPU_FLAG_AES : 0u) |
-                            (verify ? TSGPU_FLAG_VERIFY : 0u);
+                            (verify ? TSGPU_FLAG_VERIFY : 0u) | modifiers |
+                            (modifiers && manifest.compression ? TSGPU_FLAG_REFRAME : 0u);
         const ChunkIndex& index = *manifest.chunkIndex;
         const std::vector<Chunk>& chunks = index.chunks();
         const uint32_t ocs = (uint32_t)index.originalChunkSize;
@@ -100,7 +108,7 @@ public:
                 const BytesRange range = transformedRange(part);
                 if (!range.isEmpty()) bytes = fetcher(range);
             }
-            // room for every new chunk, kept frames included (a frame plus IV and tag per chunk)
+            // room for every new chunk, kept frames included (a frame plus IV and tag per chunk, and 4 bytes for a sealed frame)
             const uint64_t cap = std::max<uint64_t>(tsgpu_transform_bound(to | TSGPU_FLAG_ZSTD, oneWindow, ocs),
                                                     (uint64_t)bytes.size() + 28 * tsz.size()) + 28 * tsz.size() + 64;
             Bytes out(cap);
