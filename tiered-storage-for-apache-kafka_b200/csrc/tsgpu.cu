@@ -73,6 +73,16 @@ struct Desc {            // device-side descriptor block of one work slot (all a
     uint8_t* ivs; uint8_t* aad;
 };
 
+// Pinned read-back block of one work slot (arrays sized for max_batch): what a drained batch reads on the host.
+struct Back {
+    uint32_t* sizes;         // sizes of what the batch copies out
+    uint32_t* status;        // per chunk: the verify stage's status, or the detransform's tag / frame status
+    uint32_t* diff;          // TSGPU_FLAG_VERIFY: first differing byte per chunk
+    uint32_t* src_sizes;     // the source half (source_stage): decoded sizes
+    uint32_t* src_status;    //   ... their tag / frame statuses
+    uint64_t* words;         //   ... the object and segment CRC words, as W[2] for either CRC word W
+};
+
 // Device arrays of the record validation of one slot (records.cuh), sized for batches of up to `cap` bytes.
 struct RecScratch {
     uint8_t* d = nullptr;
@@ -124,7 +134,8 @@ struct Work {
     ZstdEncScratch zenc{};         // region kernel (TSGPU_FLAG_ZSTD_DENSE), allocated on first use
     ZstdBlkScratch zblk{};         // block kernel (default), allocated on first use
     ZstdDecScratch zdec{};
-    uint32_t* h_sizes = nullptr;   // pinned: sizes/status (and the verify stage's first differing bytes) coming back
+    uint8_t* h_back = nullptr;  size_t back_bytes = 0;
+    Back back{};                   // views of h_back
     RecScratch rec{};              // TSGPU_FLAG_VALIDATE_RECORDS, allocated on first use
     PcrcScratch<uint32_t> pcrc{};  // CRC-32C part and object checksums, allocated on first use
     PcrcScratch<uint64_t> pcrc64{};   // CRC-64/NVME (the _crc64 calls), allocated on first use
@@ -153,15 +164,30 @@ struct tsgpu_ctx {
     uint32_t nslot = 16;           // work slots per device (TSGPU_SLOTS overrides); one call takes at most 8 of them
 };
 
-static void carve_desc(uint8_t* base, uint32_t nb, Desc& d, size_t* total) {
-    size_t p = 0;
-    auto take = [&](size_t bytes) { uint8_t* r = base ? base + p : nullptr; p += align_up(bytes, 256); return r; };
-    d.a_off = (uint64_t*)take(8ull * nb); d.b_off = (uint64_t*)take(8ull * nb); d.c_off = (uint64_t*)take(8ull * (nb + 1));
-    d.a_len = (uint32_t*)take(4ull * nb); d.b_len = (uint32_t*)take(4ull * nb); d.c_len = (uint32_t*)take(4ull * nb);
-    d.status = (uint32_t*)take(4ull * nb);
-    d.v_len = (uint32_t*)take(4ull * nb); d.v_diff = (uint32_t*)take(4ull * nb);
-    d.ivs = take(12ull * nb); d.aad = take(MAX_AAD);
-    if (total) *total = p;
+struct Carver {                 // consecutive 256-byte aligned pieces of a block at `base` (nullptr: only adds up its size, p)
+    uint8_t* base; size_t p = 0;
+    template <typename T> T* take(size_t n) { T* r = base ? (T*)(base + p) : nullptr; p += align_up(sizeof(T) * n, 256); return r; }
+};
+
+static size_t carve_desc(uint8_t* base, uint32_t nb, Desc& d) {
+    Carver k{base};
+    d.a_off = k.take<uint64_t>(nb); d.b_off = k.take<uint64_t>(nb); d.c_off = k.take<uint64_t>(nb + 1);
+    d.a_len = k.take<uint32_t>(nb); d.b_len = k.take<uint32_t>(nb); d.c_len = k.take<uint32_t>(nb);
+    d.status = k.take<uint32_t>(nb); d.v_len = k.take<uint32_t>(nb); d.v_diff = k.take<uint32_t>(nb);
+    d.ivs = k.take<uint8_t>(12ull * nb); d.aad = k.take<uint8_t>(MAX_AAD);
+    return k.p;
+}
+
+static size_t carve_back(uint8_t* base, uint32_t nb, Back& b) {
+    Carver k{base};
+    b.sizes = k.take<uint32_t>(nb); b.status = k.take<uint32_t>(nb); b.diff = k.take<uint32_t>(nb);
+    b.src_sizes = k.take<uint32_t>(nb); b.src_status = k.take<uint32_t>(nb); b.words = k.take<uint64_t>(2);
+    return k.p;
+}
+
+// The frame and transformed slots of nb chunks in a descriptor block (the device calls pass their caller's slot_stride).
+static void slot_layout(const tsgpu_ctx* c, Desc& d, uint32_t nb, uint64_t slot_stride) {
+    for (uint32_t i = 0; i < nb; i++) { d.b_off[i] = (uint64_t)i * c->frame_stride; d.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD; }
 }
 
 static void work_free(Work& w);
@@ -188,16 +214,18 @@ static int work_init_impl(tsgpu_ctx* c, Work& w, int device) {
     RT(rt::malloc_device((void**)&w.d_frames, nb * c->frame_stride + 256));
     RT(rt::malloc_device((void**)&w.d_xf, nb * c->slot_stride + 256));
     RT(rt::malloc_device((void**)&w.d_pack, nb * c->slot_stride + 256));
-    carve_desc(nullptr, c->max_batch, w.dd, &w.desc_bytes);
+    w.desc_bytes = carve_desc(nullptr, c->max_batch, w.dd);
     RT(rt::malloc_device((void**)&w.d_desc, w.desc_bytes));
     RT(rt::malloc_host((void**)&w.h_desc, w.desc_bytes));
-    carve_desc(w.d_desc, c->max_batch, w.dd, nullptr);
-    carve_desc(w.h_desc, c->max_batch, w.hd, nullptr);
+    carve_desc(w.d_desc, c->max_batch, w.dd);
+    carve_desc(w.h_desc, c->max_batch, w.hd);
+    w.back_bytes = carve_back(nullptr, c->max_batch, w.back);
+    RT(rt::malloc_host((void**)&w.h_back, w.back_bytes));
+    carve_back(w.h_back, c->max_batch, w.back);
     w.max_ranges = (uint32_t)((frame_bound(c->chunk_cap) / 16 + GH_RANGE_BLOCKS) / GH_RANGE_BLOCKS) + 1;
     RT(rt::malloc_device((void**)&w.d_partials, sizeof(uint4) * (size_t)w.max_ranges * nb));
     RT(rt::malloc_device((void**)&w.keys[0].ctx, sizeof(GcmKeyCtx)));
     w.keys[0].d_aad = w.dd.aad;
-    RT(rt::malloc_host((void**)&w.h_sizes, 4ull * nb * 5 + 64));
     const char* e = zstd_dec_scratch_alloc(w.zdec, c->chunk_cap, c->max_batch);
     if (e) return fail(TSGPU_E_CUDA, "zstd dec scratch: %s", e);
     return TSGPU_OK;
@@ -210,7 +238,7 @@ static void work_free(Work& w) {
     if (w.out_stream) rt::stream_sync(w.out_stream);
     rt::free_device(w.d_orig); rt::free_device(w.d_frames); rt::free_device(w.d_xf); rt::free_device(w.d_pack);
     rt::free_device(w.d_desc); rt::free_host(w.h_desc);
-    rt::free_device(w.d_partials); rt::free_device(w.keys[0].ctx); rt::free_host(w.h_sizes);
+    rt::free_device(w.d_partials); rt::free_device(w.keys[0].ctx); rt::free_host(w.h_back);
     rt::free_device(w.keys[1].ctx); rt::free_device(w.keys[1].d_aad); rt::free_host(w.keys[1].h_aad);
     zstd_enc_scratch_free(w.zenc); zstd_blk_scratch_free(w.zblk); zstd_dec_scratch_free(w.zdec);
     rt::free_device(w.rec.d); rt::free_device(w.rec.d_out); rt::free_host(w.rec.h_out); w.rec = RecScratch{};
@@ -490,16 +518,18 @@ static int claim_slots(tsgpu_ctx* c, uint32_t want, SlotClaim& claim, int only_d
 
 // ------------------------------------------------------------------------------------------ batches (host-buffer calls)
 namespace {
-struct Batch { Work* w; uint32_t c0, nb; };      // chunks [c0, c0 + nb) of a call, in flight on slot w
+// Chunks [c0, c0 + nb) of a call, in flight on slot w; in_off: chunk c0's byte offset in the call's transformed input.
+struct Batch { Work* w; uint32_t c0, nb; uint64_t in_off; };
 }
 
 // Cuts n chunks into batches of max_batch and deals them round-robin over the slots it claims.  issue(batch) enqueues a
 // batch on its slot's stream and ends with the D2H of its sizes (ev_sizes); drain(batch) runs once those sizes are on the
 // host, in batch order, and sends the batch's bytes home (copy_out).  idle(slots, rc) runs once every claimed slot is idle,
-// before the slots are given back.  Returns with every claimed slot idle.
+// before the slots are given back.  Returns with every claimed slot idle.  `tsizes`: the transformed sizes of the n chunks of
+// a call that reads transformed chunks (Batch::in_off), else nullptr.
 namespace { struct NoIdle { int operator()(const std::vector<Work*>&, int rc) const { return rc; } }; }
 template <class Issue, class Drain, class Idle = NoIdle>
-static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain, Idle idle = Idle()) {
+static int run_batches(tsgpu_ctx* c, uint32_t n, const uint32_t* tsizes, Issue issue, Drain drain, Idle idle = Idle()) {
     const uint32_t nbatches = (n + c->max_batch - 1) / c->max_batch;
     SlotClaim claim;
     { int rcc = claim_slots(c, nbatches, claim); if (rcc) return rcc; }
@@ -513,6 +543,7 @@ static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain, Idle 
         return drain(bt);
     };
     int rc = TSGPU_OK;
+    uint64_t in_off = 0;
     for (uint32_t b = 0; b < nbatches && rc == TSGPU_OK; b++) {
         // From b = nwork on a slot is reused: its previous batch is drained first (sizes read on the host, copies-out
         // enqueued on the slot's out_stream); the new batch's copy-in and first kernels start right away and only the
@@ -520,7 +551,8 @@ static int run_batches(tsgpu_ctx* c, uint32_t n, Issue issue, Drain drain, Idle 
         // waits here, which keeps all slots' queues full.
         if (b >= nwork) { rc = drain_next(); if (rc) break; }
         const uint32_t c0 = b * c->max_batch;
-        inflight[b] = Batch{claim.slots[b % nwork], c0, std::min(c->max_batch, n - c0)};
+        inflight[b] = Batch{claim.slots[b % nwork], c0, std::min(c->max_batch, n - c0), in_off};
+        if (tsizes) for (uint32_t i = 0; i < inflight[b].nb; i++) in_off += tsizes[c0 + i];
         rc = issue(inflight[b]);
     }
     while (rc == TSGPU_OK && drained < nbatches) rc = drain_next();
@@ -672,11 +704,39 @@ template <typename W> constexpr const char* crc_arg() { return sizeof(W) == 8 ? 
 // One batch of a tsgpu_transform_parts call, L packed bytes: words[k] is the raw CRC of [0, x_k) of the batch,
 // x_k = first + k * part_size for k < m (the part boundaries strictly inside it), x_m = L.
 template <typename W> struct PcrcBatch { uint32_t L = 0, first = 0, m = 0; std::vector<W> words; };
-template <typename W> struct PartsRun {
-    uint64_t part_size = 0;
-    uint64_t obj0 = 0;                    // object bytes before the call
-    std::vector<PcrcBatch<W>> batches;    // by batch index
+// The part-checksum arguments of tsgpu_transform_parts, tsgpu_rewrite_object and their _crc64 twins.
+template <typename W> struct PartsReq {
+    uint64_t part_size; tsgpu_parts_cursor* cursor;
+    W* crcs; uint32_t cap; uint32_t* n; W* object_crc;
 };
+// The part checksums of one call.  Its entry point takes it through parts_begin, then parts_drain at each batch's drain
+// (target_drain), parts_idle once the call's slots are idle, and parts_finish after a successful call.
+template <typename W> struct PartsRun {
+    PartsReq<W> q{};
+    PartsCarry<W> cur{};                  // the cursor as the call found it
+    std::vector<PcrcBatch<W>> batches;    // by batch index, as they drain
+};
+
+// The part-checksum arguments, checked before any GPU work, and the cursor.  `bound`: the most bytes the call can add to the object.
+template <typename W>
+static int parts_begin(PartsRun<W>& run, const PartsReq<W>& q, uint32_t flags, uint64_t bound, int segment_ends_here) {
+    if (!(flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)))
+        return fail(TSGPU_E_ARG, "%s needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU",
+                    sizeof(W) == 8 ? "tsgpu_transform_parts_crc64" : "tsgpu_transform_parts");
+    if (q.part_size == 0) return fail(TSGPU_E_ARG, "part_size must be at least 1");
+    if (!q.cursor || !q.n || !q.object_crc) return fail(TSGPU_E_ARG, "parts cursor, n_parts and object_%s cannot be null", crc_arg<W>());
+    PartsCarry<W>& cur = run.cur;
+    memcpy(&cur, q.cursor, sizeof cur);
+    if (cur.obj_len && cur.part_size != q.part_size)
+        return fail(TSGPU_E_ARG, "part_size %llu differs from the %llu the object started with", (unsigned long long)q.part_size,
+                    (unsigned long long)cur.part_size);
+    const uint64_t most = (cur.obj_len % q.part_size + bound) / q.part_size + (segment_ends_here ? 1 : 0);
+    if (most > q.cap) return fail(TSGPU_E_SHORT, "part_%s too small: the call may complete %llu parts, part_cap is %u",
+                                  crc_arg<W>(), (unsigned long long)most, q.cap);
+    if (q.cap && !q.crcs) return fail(TSGPU_E_ARG, "part_%s cannot be null", crc_arg<W>());
+    run.q = q;
+    return TSGPU_OK;
+}
 
 template <typename W>
 static int parts_alloc(PcrcScratch<W>& r, uint64_t cap, rt::stream_t st) {
@@ -719,13 +779,14 @@ static void parts_collect(Work& w, PartsRun<W>& pr) {
     p.pending = -1;
 }
 
-// At the drain of batch `bi` (L packed bytes at object offset `at`): pcrc_cuts and the D2H of its m + 1 words on out_stream,
-// ahead of the batch's copy-out.
+// At the drain of batch `bi` (L packed bytes at `dst_off` in the call's output): pcrc_cuts and the D2H of its m + 1 words on
+// out_stream, ahead of the batch's copy-out.
 template <typename W>
-static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun<W>& pr, uint32_t bi, uint64_t at, uint64_t L) {
+static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun<W>& pr, uint32_t bi, uint64_t dst_off, uint64_t L) {
     parts_collect(w, pr);
     PcrcScratch<W>& p = pcrc_of<W>(w);
-    const uint64_t P = pr.part_size;
+    const uint64_t P = pr.q.part_size;
+    const uint64_t at = pr.cur.obj_len + dst_off;                        // the batch's offset in the object
     const uint64_t first = P - at % P;                                   // the first part boundary after the batch's start
     const uint32_t m = first < L ? (uint32_t)((L - 1 - first) / P + 1) : 0;
     if (m + 1 > p.cuts_cap) {                                            // nothing on the slot reads the old arrays any more
@@ -739,6 +800,7 @@ static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun<W>& pr, uint32_t bi, uint
                 dim3(PCRC_CUTS_T), 0, w.out_stream, p.a, (uint32_t)L, m ? (uint32_t)first : 0u, P, m, p.d_cuts);
     CHECK_LAUNCH("pcrc_cuts_kernel");
     RT(rt::d2h(p.h_cuts, p.d_cuts, sizeof(W) * (m + 1), w.out_stream));
+    if (pr.batches.size() <= bi) pr.batches.resize(bi + 1);
     PcrcBatch<W>& b = pr.batches[bi];
     b.L = (uint32_t)L; b.first = m ? (uint32_t)first : 0u; b.m = m; b.words.clear();
     p.pending = (int32_t)bi;
@@ -748,7 +810,7 @@ static int parts_drain(tsgpu_ctx* c, Work& w, PartsRun<W>& pr, uint32_t bi, uint
 // The call's batches in order: their pieces extend the open part and the object; a part whose last byte arrives is emitted.
 template <typename W>
 static void parts_combine(const PartsRun<W>& pr, PartsCarry<W>& cur, std::vector<W>& emitted) {
-    const uint64_t P = pr.part_size;
+    const uint64_t P = pr.q.part_size;
     for (const PcrcBatch<W>& b : pr.batches) {
         W prev = 0;
         uint32_t prev_x = 0;
@@ -765,29 +827,49 @@ static void parts_combine(const PartsRun<W>& pr, PartsCarry<W>& cur, std::vector
     }
 }
 
+// The idle step of a call with a target half (pr: nullptr without part checksums): the last batches' part prefixes, once every
+// slot of the call is idle.
+template <typename W>
+static int parts_idle(PartsRun<W>* pr, const std::vector<Work*>& slots, int rc) {
+    if (pr) for (Work* w : slots) { if (rc == TSGPU_OK) parts_collect(*w, *pr); pcrc_of<W>(*w).pending = -1; }
+    return rc;
+}
+
+// After a successful call: the completed parts (and at the segment's end the open part and the object CRC) go out, and the
+// cursor moves on.  Nothing is written before: a failed call leaves the part and object checksums as they were.
+template <typename W>
+static void parts_finish(const PartsRun<W>& pr, int segment_ends_here) {
+    const PartsReq<W>& q = pr.q;
+    PartsCarry<W> cur = pr.cur;
+    std::vector<W> emitted;
+    parts_combine(pr, cur, emitted);
+    cur.part_size = q.part_size;
+    if (segment_ends_here) {
+        const uint64_t open = cur.obj_len % q.part_size;
+        if (open) { emitted.push_back(crc_finish(cur.raw[0], open, 0)); cur.raw[0] = 0; }
+        *q.object_crc = crc_finish(cur.raw[1], cur.obj_len, 0);
+    }
+    if (!emitted.empty()) memcpy(q.crcs, emitted.data(), sizeof(W) * emitted.size());
+    *q.n = (uint32_t)emitted.size();
+    memcpy(q.cursor, &cur, sizeof cur);
+}
+
 #ifdef TSGPU_SIMT
 // TEST-ONLY fault injection, compiled into the emulator build alone (device memory is host memory there and every kernel
-// has finished when its launch returns).  TSGPU_SIMT_FLIP=<chunk>:<offset> flips the low bit of one byte of that chunk's
-// transformed bytes -- frame, or IV || ciphertext || tag -- before they are packed and verified.  A negative offset counts
-// from the chunk's end (-1: last tag byte).  tests/test_simt_verify.py drives it.
-static void simt_inject_fault(ChunksOut fin, uint32_t c0, uint32_t nb) {
-    const char* e = getenv("TSGPU_SIMT_FLIP");
+// has finished when its launch returns).  The variable `var` = <chunk>:<offset> flips the low bit of one byte of that chunk of
+// the batch's chunks [c0, c0 + nb) in `chunks`.  A negative offset counts from the chunk's end.
+//   TSGPU_SIMT_FLIP: the chunk's transformed bytes -- frame, or IV || ciphertext || tag -- before they are packed and verified
+//     (-1: last tag byte).  tests/test_simt_verify.py drives it.
+//   TSGPU_SIMT_FLIP_DECODED: the chunk's decoded bytes in d_orig right after the source decode of tsgpu_check_object /
+//     tsgpu_rewrite_object -- a decoder that misread the chunk.  tests/test_simt_reframe.py drives it: TSGPU_FLAG_REFRAME must
+//     not stamp the checksum of such a chunk.
+static void simt_flip(const char* var, ChunksOut chunks, uint32_t c0, uint32_t nb) {
+    const char* e = getenv(var);
     long k = 0, at = 0;
     if (!e || sscanf(e, "%ld:%ld", &k, &at) != 2 || k < (long)c0 || k >= (long)c0 + (long)nb) return;
-    const uint32_t i = (uint32_t)(k - c0), n = fin.len[i];
+    const uint32_t i = (uint32_t)(k - c0), n = chunks.len[i];
     if (at < 0) at += n;
-    if (at >= 0 && at < (long)n) fin.base[fin.off[i] + at] ^= 1;
-}
-// TEST-ONLY, as above: TSGPU_SIMT_FLIP_DECODED=<chunk>:<offset> flips the low bit of one byte of that chunk's decoded bytes in
-// d_orig right after the source decode of tsgpu_check_object / tsgpu_rewrite_object -- a decoder that misread the chunk.
-// tests/test_simt_reframe.py drives it: TSGPU_FLAG_REFRAME must not stamp the checksum of such a chunk.
-static void simt_flip_decoded(ChunksIn orig, uint32_t c0, uint32_t nb) {
-    const char* e = getenv("TSGPU_SIMT_FLIP_DECODED");
-    long k = 0, at = 0;
-    if (!e || sscanf(e, "%ld:%ld", &k, &at) != 2 || k < (long)c0 || k >= (long)c0 + (long)nb) return;
-    const uint32_t i = (uint32_t)(k - c0), n = orig.len[i];
-    if (at < 0) at += n;
-    if (at >= 0 && at < (long)n) const_cast<uint8_t*>(orig.base)[orig.off[i] + at] ^= 1;
+    if (at >= 0 && at < (long)n) chunks.base[chunks.off[i] + at] ^= 1;
 }
 #endif
 
@@ -817,34 +899,44 @@ static int reframe_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t refram
     return TSGPU_OK;
 }
 
+// The new object's side of a transform or a rewrite.
+struct TargetReq {
+    uint32_t flags;                  // ZSTD, modifiers and AES of the new object
+    bool verify, kept;               // kept (rewrite): the source frames go into the new object as they are
+    uint32_t reframe;                // TSGPU_FLAG_REFRAME: the ZSTD_DENSE and ZSTD_CHECKSUM bits that act on the kept frames, else 0
+    Aes256RoundKeys rk;
+    const uint8_t* aad; uint32_t aad_len;
+    const uint8_t* ivs;
+};
+
 // The target half of a batch whose original chunks are `orig` in d_orig (each at most cs bytes): [zstd ->] [AES-GCM encrypt]
-// with the keys `k`, or with `kept` the batch's frames in the d_frames slots (b_off, b_len; frames_max bytes at most) as they are
-// [-> AES-GCM encrypt]; the transformed chunks packed into d_pack, [pcrc_tiles over them,] [the verify stage and the D2H of its
-// verdicts to h_sizes + nb.]  `fin` receives the transformed chunks in their slots.  `parts`: the bytes of the part checksums'
-// CRC word (4: CRC-32C, 8: CRC-64/NVME), 0 without part checksums.  `reframe`: with `kept`, the ZSTD_DENSE and ZSTD_CHECKSUM
-// bits TSGPU_FLAG_REFRAME applies to the kept frames first (reframe_stage); a sealed frame is 4 bytes longer than frames_max.
-static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint32_t flags, bool verify, int parts, uint32_t c0,
-                        uint32_t nb, uint32_t cs, const Aes256RoundKeys& rk, uint32_t aad_len, ChunksIn orig, bool kept,
-                        uint64_t frames_max, ChunksOut& fin, uint32_t reframe = 0) {
-    const bool aes = flags & TSGPU_FLAG_AES;
+// with the keys `k`, or with t.kept the batch's frames in the d_frames slots (b_off, b_len; frames_max bytes at most) as they are
+// [-> AES-GCM encrypt]; the transformed chunks packed into d_pack, [pcrc_tiles over them for part checksums of CRC word W,] [the
+// verify stage and the D2H of its verdicts to the read-back block.]  `fin` receives the transformed chunks in their slots.
+// t.reframe: with t.kept, the bits TSGPU_FLAG_REFRAME applies to the kept frames first (reframe_stage); a sealed frame is 4
+// bytes longer than frames_max.
+template <typename W>
+static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, const TargetReq& t, bool parts, uint32_t c0, uint32_t nb,
+                        uint32_t cs, ChunksIn orig, uint64_t frames_max, ChunksOut& fin) {
+    const bool aes = t.flags & TSGPU_FLAG_AES;
     // encrypted chunks land in the transformed slots; zstd alone leaves its frames in the frame slots
     fin = aes ? ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len} : ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len};
     uint64_t payload;                        // the largest transformed chunk without IV and tag
-    if (kept) {
-        payload = frames_max + ((reframe & TSGPU_FLAG_ZSTD_CHECKSUM) ? 4 : 0);
-        if (reframe) { int rc = reframe_stage(c, w, st, reframe, nb, cs, orig); if (rc) return rc; }
+    if (t.kept) {
+        payload = frames_max + ((t.reframe & TSGPU_FLAG_ZSTD_CHECKSUM) ? 4 : 0);
+        if (t.reframe) { int rc = reframe_stage(c, w, st, t.reframe, nb, cs, orig); if (rc) return rc; }
         if (aes) {
-            int rc = gcm_stage<true>(c, w, k, st, rk, ChunksIn{w.d_frames, w.dd.b_off, w.dd.b_len}, fin, aad_len, w.dd.status, nb,
+            int rc = gcm_stage<true>(c, w, k, st, t.rk, ChunksIn{w.d_frames, w.dd.b_off, w.dd.b_len}, fin, t.aad_len, w.dd.status, nb,
                                      (uint32_t)payload, 0xffffffffu);
             if (rc) return rc;
         }
     } else {
-        payload = (flags & TSGPU_FLAG_ZSTD) ? frame_bound(cs) : cs;
-        int rc = transform_enqueue(c, w, k, st, flags, nb, cs, rk, aad_len, orig, fin);
+        payload = (t.flags & TSGPU_FLAG_ZSTD) ? frame_bound(cs) : cs;
+        int rc = transform_enqueue(c, w, k, st, t.flags, nb, cs, t.rk, t.aad_len, orig, fin);
         if (rc) return rc;
     }
 #ifdef TSGPU_SIMT
-    simt_inject_fault(fin, c0, nb);
+    simt_flip("TSGPU_SIMT_FLIP", fin, c0, nb);
 #endif
     // the transformed chunks, back to back, so the batch leaves in one copy (the previous batch's copy-out may still be
     // reading d_pack: this is the first kernel of the batch that has to wait for it)
@@ -856,25 +948,22 @@ static int target_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, uint
         const uint64_t longest = payload + 28;
         TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((uint32_t)((longest + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T), 0, st, P);
         CHECK_LAUNCH("pack_chunks_kernel");
-        if (parts) {
-            int rc = parts == 8 ? parts_stage<uint64_t>(c, w, st, fin.len, nb, longest * nb) : parts_stage<uint32_t>(c, w, st, fin.len, nb, longest * nb);
-            if (rc) return rc;
-        }
+        if (parts) { int rc = parts_stage<W>(c, w, st, fin.len, nb, longest * nb); if (rc) return rc; }
     }
-    if (verify) {
-        int rc = verify_stage(c, w, k, st, flags, nb, cs, payload, rk, aad_len, fin);
+    if (t.verify) {
+        int rc = verify_stage(c, w, k, st, t.flags, nb, cs, payload, t.rk, t.aad_len, fin);
         if (rc) return rc;
-        RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
-        RT(rt::d2h(w.h_sizes + 2 * nb, w.dd.v_diff, 4ull * nb, st));
+        RT(rt::d2h(w.back.status, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.back.diff, w.dd.v_diff, 4ull * nb, st));
     }
     return TSGPU_OK;
 }
 
 // One batch: copy in, fill the descriptors, the target half, [the record kernels,] D2H of the transformed sizes.
 // `off`/`len`: position and size of every chunk inside src (chunks are contiguous); `cs` = largest chunk of the call.
-static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool verify, bool records, int parts, const uint8_t* src, const uint64_t* off,
-                           const uint32_t* len, uint32_t cs, const Aes256RoundKeys& rk, const uint8_t* aad, uint32_t aad_len,
-                           const uint8_t* ivs) {
+template <typename W>
+static int transform_issue(tsgpu_ctx* c, const Batch& bt, const TargetReq& t, bool records, bool parts, const uint8_t* src,
+                           const uint64_t* off, const uint32_t* len, uint32_t cs) {
     Work& w = *bt.w;
     const uint32_t c0 = bt.c0, nb = bt.nb;
     RT(rt::set_device(w.device));
@@ -886,32 +975,30 @@ static int transform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, bool v
     for (uint32_t i = 0; i < nb; i++) {
         w.hd.a_off[i] = off[c0 + i] - byte0;
         w.hd.a_len[i] = len[c0 + i];
-        w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
-        w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
     }
-    if (flags & TSGPU_FLAG_AES) {
-        memcpy(w.hd.ivs, ivs + (size_t)c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
-        if (aad_len) memcpy(w.hd.aad, aad, aad_len);
+    slot_layout(c, w.hd, nb, c->slot_stride);
+    if (t.flags & TSGPU_FLAG_AES) {
+        memcpy(w.hd.ivs, t.ivs + (size_t)c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
+        if (t.aad_len) memcpy(w.hd.aad, t.aad, t.aad_len);
     }
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
     ChunksOut fin;
-    { int rc = target_stage(c, w, w.keys[0], st, flags, verify, parts, c0, nb, cs, rk, aad_len, ChunksIn{w.d_orig, w.dd.a_off, w.dd.a_len},
-                            /*kept=*/false, 0, fin); if (rc) return rc; }
+    { int rc = target_stage<W>(c, w, w.keys[0], st, t, parts, c0, nb, cs, ChunksIn{w.d_orig, w.dd.a_off, w.dd.a_len}, 0, fin); if (rc) return rc; }
     if (records) {
         int rc = records_alloc(w.rec, (uint64_t)c->max_batch * cs);
         if (!rc) rc = records_stage(c, w, st, byte1 - byte0);
         if (rc) return rc;
     }
-    RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
+    RT(rt::d2h(w.back.sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
     return TSGPU_OK;
 }
 
-// The verify stage's verdict on a drained batch (h_sizes: sizes, status, first differing bytes); TSGPU_OK if every chunk
-// read back.  `len`: the original chunk sizes of the call; `first`: the number the call's first chunk has in the messages.
+// The verify stage's verdict on a drained batch; TSGPU_OK if every chunk read back.  `len`: the original chunk sizes of the
+// call; `first`: the number the call's first chunk has in the messages.
 static int verify_verdict(const Batch& bt, const uint32_t* len, uint64_t first = 0) {
-    const uint32_t* status = bt.w->h_sizes + bt.nb;
-    const uint32_t* diff = bt.w->h_sizes + 2 * bt.nb;
+    const uint32_t* status = bt.w->back.status;
+    const uint32_t* diff = bt.w->back.diff;
     for (uint32_t i = 0; i < bt.nb; i++) {
         const uint32_t k = bt.c0 + i;
         const unsigned long long g = first + k;
@@ -925,11 +1012,71 @@ static int verify_verdict(const Batch& bt, const uint32_t* len, uint64_t first =
     return TSGPU_OK;
 }
 
+// The drain of a batch whose target half ran (transform, rewrite), once its verdicts have passed: its new sizes go to the
+// caller's `sizes`, [its part prefixes are cut,] and its bytes leave.
+template <typename W>
+static int target_drain(tsgpu_ctx* c, const Batch& bt, uint32_t* sizes, PartsRun<W>* parts, uint8_t* dst, uint64_t dst_cap,
+                        uint64_t& dst_off) {
+    Work& w = *bt.w;
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < bt.nb; i++) { sizes[bt.c0 + i] = w.back.sizes[i]; total += w.back.sizes[i]; }
+    if (parts && dst_off + total <= dst_cap) {
+        int rc = parts_drain(c, w, *parts, bt.c0 / c->max_batch, dst_off, total);
+        if (rc) return rc;
+    }
+    return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);     // one copy per batch: packed on the device
+}
+
 template <typename W = uint32_t>
 static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
                             const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
                             const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
-                            RecCarry* records, PartsRun<W>* parts = nullptr);
+                            RecCarry* records, PartsRun<W>* parts = nullptr) {
+    const uint32_t n = (uint32_t)len.size();
+    if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
+    if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~ZSTD_MODIFIERS;         // modifiers of ZSTD: meaningless (and harmless) without it
+    const bool verify = (flags & TSGPU_FLAG_VERIFY) || c->verify_default;
+    flags &= ~TSGPU_FLAG_VERIFY;
+
+    if (flags == 0) {       // TransformFinisher no-transform fast path (TransformFinisher.java:135-140): bytes unchanged, nothing to verify
+        if (dst_cap < src_len) return fail(TSGPU_E_SHORT, "dst too small");
+        memcpy(dst, src, src_len);
+        for (uint32_t i = 0; i < n; i++) transformed_sizes[i] = len[i];
+        *n_chunks = n;
+        return TSGPU_OK;
+    }
+    TargetReq t{};
+    t.flags = flags; t.verify = verify; t.kept = false; t.reframe = 0;
+    if (flags & TSGPU_FLAG_AES) t.rk = aes256_expand_key(key);
+    t.aad = aad; t.aad_len = aad_len; t.ivs = ivs;
+
+    uint64_t dst_off = 0;
+    const int rc = run_batches(c, n, nullptr,
+        [&](const Batch& bt) { return transform_issue<W>(c, bt, t, records != nullptr, parts != nullptr, src, off.data(), len.data(), cs); },
+        [&](const Batch& bt) {
+            if (records) { int rcr = records_resolve(c, *bt.w, *records); if (rcr) return rcr; }   // the input first: none of the batch's bytes leave
+            if (verify) { int rcv = verify_verdict(bt, len.data()); if (rcv) return rcv; }   // none of the batch's bytes leave
+            return target_drain(c, bt, transformed_sizes, parts, dst, dst_cap, dst_off);
+        },
+        [&](const std::vector<Work*>& slots, int rcb) { return parts_idle(parts, slots, rcb); });
+    if (rc) return rc;
+    *n_chunks = n;
+    return TSGPU_OK;
+}
+
+// The key, IV and AAD arguments of a call with TSGPU_FLAG_AES in `flags`.  `side`: what the call does with the key, which names
+// the arguments in the messages (AES_TO: the new key of tsgpu_rewrite_object, its arguments named to_*).  `ivs`: the IVs the
+// call needs are there (each call has its own rule; decryption reads them from the chunks).
+enum AesSide { AES_ENC, AES_DEC, AES_TO };
+static int aes_args_ok(uint32_t flags, AesSide side, const uint8_t* key, bool ivs, const uint8_t* aad, uint32_t aad_len) {
+    if (!(flags & TSGPU_FLAG_AES)) return TSGPU_OK;
+    if (!key || !ivs)
+        return fail(TSGPU_E_ARG, side == AES_ENC ? "key and ivs are required for encryption"
+                                 : side == AES_TO ? "to_key and to_ivs are required for encryption" : "key is required for decryption");
+    if (aad_len > MAX_AAD) return fail(TSGPU_E_ARG, side == AES_TO ? "to_aad longer than %u bytes" : "aad longer than %u bytes", MAX_AAD);
+    if (aad_len && !aad) return fail(TSGPU_E_ARG, side == AES_TO ? "to_aad cannot be null" : "aad cannot be null");
+    return TSGPU_OK;
+}
 
 static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint8_t* key, const uint8_t* aad,
                              uint32_t aad_len, const uint8_t* ivs, uint32_t* transformed_sizes, uint32_t* n_chunks) {
@@ -937,23 +1084,60 @@ static int transform_args_ok(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, u
     if (!n_chunks || !transformed_sizes) return fail(TSGPU_E_ARG, "transformed_sizes/n_chunks cannot be null");
     if (src_len && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
     if (flags & ~(KNOWN_FLAGS | TSGPU_FLAG_VERIFY | TSGPU_FLAG_VALIDATE_RECORDS)) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
-    if ((flags & TSGPU_FLAG_AES) && (!key || !ivs)) return fail(TSGPU_E_ARG, "key and ivs are required for encryption");
-    if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
-    if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
-    return TSGPU_OK;
+    return aes_args_ok(flags, AES_ENC, key, ivs != nullptr, aad, aad_len);
 }
 
 static_assert(sizeof(tsgpu_records_cursor) == sizeof(RecCarry), "the cursor holds the carry");
-// The part-checksum arguments of tsgpu_transform_parts (and its _crc64 twin).
-template <typename W> struct PartsReq {
-    uint64_t part_size; tsgpu_parts_cursor* cursor;
-    W* crcs; uint32_t cap; uint32_t* n; W* object_crc;
-};
 template <typename W = uint32_t>
 static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
                              const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
                              uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
-                             bool env_default, const PartsReq<W>* parts = nullptr);
+                             bool env_default, const PartsReq<W>* parts = nullptr) try {
+    int rc = transform_args_ok(c, flags, src, src_len, key, aad, aad_len, ivs, transformed_sizes, n_chunks);
+    if (rc) return rc;
+    const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
+    if ((flags & TSGPU_FLAG_VALIDATE_RECORDS) && !(flags & xf))
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_VALIDATE_RECORDS (%u) needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU",
+                    TSGPU_FLAG_VALIDATE_RECORDS);
+    const bool records = (flags & TSGPU_FLAG_VALIDATE_RECORDS) || (env_default && c->records_default && (flags & xf));
+    if (records && !cursor) return fail(TSGPU_E_ARG, "cursor cannot be null when record batches are validated");
+    RecCarry carry{};
+    if (records) memcpy(&carry, cursor, sizeof carry);
+    PartsRun<W> run;
+    if (parts) {
+        rc = parts_begin(run, *parts, flags, src_len ? tsgpu_transform_bound(flags, src_len, chunk_size) : 0, segment_ends_here);
+        if (rc) return rc;
+    }
+    // BaseTransformChunkEnumeration: originalChunkSize 0 disables chunking (one chunk = whole stream)
+    uint64_t cs64 = chunk_size ? chunk_size : src_len;
+    if (src_len == 0) {
+        if (records && segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
+        *n_chunks = 0;
+        if (parts) parts_finish(run, segment_ends_here);
+        return TSGPU_OK;
+    }
+    if (cs64 > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk size %llu exceeds the context's max_chunk_bytes %u", (unsigned long long)cs64, c->chunk_cap);
+    const uint32_t cs = (uint32_t)cs64;
+    if (records && (uint64_t)c->max_batch * cs > REC_MAX_BATCH)
+        return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch, cs);
+    if (parts && (uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
+        return fail(TSGPU_E_ARG, "part checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
+                    (unsigned long long)c->slot_stride);
+    const uint64_t n64 = (src_len + cs - 1) / cs;
+    if (n64 > *n_chunks) return fail(TSGPU_E_SHORT, "transformed_sizes too small: %llu chunks", (unsigned long long)n64);
+    std::vector<uint64_t> off(n64);
+    std::vector<uint32_t> len(n64);
+    for (uint64_t i = 0; i < n64; i++) { off[i] = i * cs; len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - i * cs); }
+    rc = transform_common(c, flags & ~TSGPU_FLAG_VALIDATE_RECORDS, src, src_len, off, len, cs, key, aad, aad_len, ivs, dst, dst_cap,
+                          transformed_sizes, n_chunks, records ? &carry : nullptr, parts ? &run : nullptr);
+    if (rc) return rc;
+    if (records) {
+        if (segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
+        memcpy(cursor, &carry, sizeof carry);
+    }
+    if (parts) parts_finish(run, segment_ends_here);
+    return TSGPU_OK;
+} catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
 extern "C" int tsgpu_transform(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size,
                                const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
@@ -996,97 +1180,6 @@ extern "C" int tsgpu_transform_parts_crc64(tsgpu_ctx* c, uint32_t flags, const u
                              records, segment_ends_here, /*env_default=*/true, &req);
 }
 
-// The part-checksum arguments, checked before any GPU work.  `bound`: the most bytes the call can add to the object.
-template <typename W>
-static int parts_args_ok(const PartsReq<W>& q, uint32_t flags, uint64_t bound, int segment_ends_here) {
-    if (!(flags & (TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES)))
-        return fail(TSGPU_E_ARG, "%s needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU",
-                    sizeof(W) == 8 ? "tsgpu_transform_parts_crc64" : "tsgpu_transform_parts");
-    if (q.part_size == 0) return fail(TSGPU_E_ARG, "part_size must be at least 1");
-    if (!q.cursor || !q.n || !q.object_crc) return fail(TSGPU_E_ARG, "parts cursor, n_parts and object_%s cannot be null", crc_arg<W>());
-    PartsCarry<W> cur;
-    memcpy(&cur, q.cursor, sizeof cur);
-    if (cur.obj_len && cur.part_size != q.part_size)
-        return fail(TSGPU_E_ARG, "part_size %llu differs from the %llu the object started with", (unsigned long long)q.part_size,
-                    (unsigned long long)cur.part_size);
-    const uint64_t most = (cur.obj_len % q.part_size + bound) / q.part_size + (segment_ends_here ? 1 : 0);
-    if (most > q.cap) return fail(TSGPU_E_SHORT, "part_%s too small: the call may complete %llu parts, part_cap is %u",
-                                  crc_arg<W>(), (unsigned long long)most, q.cap);
-    if (q.cap && !q.crcs) return fail(TSGPU_E_ARG, "part_%s cannot be null", crc_arg<W>());
-    return TSGPU_OK;
-}
-
-// After a successful call: the completed parts (and at the segment's end the open part and the object CRC) go out, and the
-// cursor moves on.  Nothing is written before: a failed call leaves the part and object checksums as they were.
-template <typename W>
-static void parts_finish(const PartsReq<W>& q, PartsCarry<W> cur, const PartsRun<W>* run, int segment_ends_here) {
-    std::vector<W> emitted;
-    if (run) parts_combine(*run, cur, emitted);
-    cur.part_size = q.part_size;
-    if (segment_ends_here) {
-        const uint64_t open = cur.obj_len % q.part_size;
-        if (open) { emitted.push_back(crc_finish(cur.raw[0], open, 0)); cur.raw[0] = 0; }
-        *q.object_crc = crc_finish(cur.raw[1], cur.obj_len, 0);
-    }
-    if (!emitted.empty()) memcpy(q.crcs, emitted.data(), sizeof(W) * emitted.size());
-    *q.n = (uint32_t)emitted.size();
-    memcpy(q.cursor, &cur, sizeof cur);
-}
-
-template <typename W>
-static int transform_segment(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, uint32_t chunk_size, const uint8_t key[32],
-                             const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
-                             uint32_t* transformed_sizes, uint32_t* n_chunks, tsgpu_records_cursor* cursor, int segment_ends_here,
-                             bool env_default, const PartsReq<W>* parts) try {
-    int rc = transform_args_ok(c, flags, src, src_len, key, aad, aad_len, ivs, transformed_sizes, n_chunks);
-    if (rc) return rc;
-    const uint32_t xf = TSGPU_FLAG_ZSTD | TSGPU_FLAG_AES;
-    if ((flags & TSGPU_FLAG_VALIDATE_RECORDS) && !(flags & xf))
-        return fail(TSGPU_E_ARG, "TSGPU_FLAG_VALIDATE_RECORDS (%u) needs TSGPU_FLAG_ZSTD or TSGPU_FLAG_AES: without them no byte reaches the GPU",
-                    TSGPU_FLAG_VALIDATE_RECORDS);
-    const bool records = (flags & TSGPU_FLAG_VALIDATE_RECORDS) || (env_default && c->records_default && (flags & xf));
-    if (records && !cursor) return fail(TSGPU_E_ARG, "cursor cannot be null when record batches are validated");
-    RecCarry carry{};
-    if (records) memcpy(&carry, cursor, sizeof carry);
-    PartsCarry<W> pcarry{};
-    if (parts) {
-        rc = parts_args_ok(*parts, flags, src_len ? tsgpu_transform_bound(flags, src_len, chunk_size) : 0, segment_ends_here);
-        if (rc) return rc;
-        memcpy(&pcarry, parts->cursor, sizeof pcarry);
-    }
-    // BaseTransformChunkEnumeration: originalChunkSize 0 disables chunking (one chunk = whole stream)
-    uint64_t cs64 = chunk_size ? chunk_size : src_len;
-    if (src_len == 0) {
-        if (records && segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
-        *n_chunks = 0;
-        if (parts) parts_finish<W>(*parts, pcarry, nullptr, segment_ends_here);
-        return TSGPU_OK;
-    }
-    if (cs64 > c->chunk_cap) return fail(TSGPU_E_ARG, "chunk size %llu exceeds the context's max_chunk_bytes %u", (unsigned long long)cs64, c->chunk_cap);
-    const uint32_t cs = (uint32_t)cs64;
-    if (records && (uint64_t)c->max_batch * cs > REC_MAX_BATCH)
-        return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch, cs);
-    if (parts && (uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
-        return fail(TSGPU_E_ARG, "part checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
-                    (unsigned long long)c->slot_stride);
-    const uint64_t n64 = (src_len + cs - 1) / cs;
-    if (n64 > *n_chunks) return fail(TSGPU_E_SHORT, "transformed_sizes too small: %llu chunks", (unsigned long long)n64);
-    std::vector<uint64_t> off(n64);
-    std::vector<uint32_t> len(n64);
-    for (uint64_t i = 0; i < n64; i++) { off[i] = i * cs; len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - i * cs); }
-    PartsRun<W> run;
-    if (parts) { run.part_size = parts->part_size; run.obj0 = pcarry.obj_len; }
-    rc = transform_common(c, flags & ~TSGPU_FLAG_VALIDATE_RECORDS, src, src_len, off, len, cs, key, aad, aad_len, ivs, dst, dst_cap,
-                          transformed_sizes, n_chunks, records ? &carry : nullptr, parts ? &run : nullptr);
-    if (rc) return rc;
-    if (records) {
-        if (segment_ends_here) { rc = records_segment_end(carry); if (rc) return rc; }
-        memcpy(cursor, &carry, sizeof carry);
-    }
-    if (parts) parts_finish(*parts, pcarry, &run, segment_ends_here);
-    return TSGPU_OK;
-} catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
-
 // Ragged variant: chunk i is the next chunk_lens[i] bytes of src.  This is what RemoteStorageManager.transformIndex
 // (RemoteStorageManager.java:455-490) needs: every Kafka index file is ONE chunk (chunking disabled), AES only, and the
 // five of them ride in a single batch (SURVEY.md §8f.3).
@@ -1112,57 +1205,10 @@ extern "C" int tsgpu_transform_chunks(tsgpu_ctx* c, uint32_t flags, const uint8_
     return transform_common(c, flags, src, total, off, len, mx, key, aad, aad_len, ivs, dst, dst_cap, transformed_sizes, &cap, nullptr);
 } catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
 
-template <typename W>
-static int transform_common(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const std::vector<uint64_t>& off,
-                            const std::vector<uint32_t>& len, uint32_t cs, const uint8_t key[32], const uint8_t* aad, uint32_t aad_len,
-                            const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap, uint32_t* transformed_sizes, uint32_t* n_chunks,
-                            RecCarry* records, PartsRun<W>* parts) {
-    const uint32_t n = (uint32_t)len.size();
-    if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
-    if (!(flags & TSGPU_FLAG_ZSTD)) flags &= ~ZSTD_MODIFIERS;         // modifiers of ZSTD: meaningless (and harmless) without it
-    const bool verify = (flags & TSGPU_FLAG_VERIFY) || c->verify_default;
-    flags &= ~TSGPU_FLAG_VERIFY;
-
-    if (flags == 0) {       // TransformFinisher no-transform fast path (TransformFinisher.java:135-140): bytes unchanged, nothing to verify
-        if (dst_cap < src_len) return fail(TSGPU_E_SHORT, "dst too small");
-        memcpy(dst, src, src_len);
-        for (uint32_t i = 0; i < n; i++) transformed_sizes[i] = len[i];
-        *n_chunks = n;
-        return TSGPU_OK;
-    }
-    Aes256RoundKeys rk{};
-    if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
-
-    uint64_t dst_off = 0;
-    if (parts) parts->batches.assign((n + c->max_batch - 1) / c->max_batch, PcrcBatch<W>{});
-    const int parts_word = parts ? (int)sizeof(W) : 0;
-    const int rc = run_batches(c, n,
-        [&](const Batch& bt) { return transform_issue(c, bt, flags, verify, records != nullptr, parts_word, src, off.data(), len.data(), cs, rk, aad, aad_len, ivs); },
-        [&](const Batch& bt) {
-            Work& w = *bt.w;
-            if (records) { int rcr = records_resolve(c, w, *records); if (rcr) return rcr; }   // the input first: none of the batch's bytes leave
-            if (verify) { int rcv = verify_verdict(bt, len.data()); if (rcv) return rcv; }   // none of the batch's bytes leave
-            uint64_t total = 0;
-            for (uint32_t i = 0; i < bt.nb; i++) { transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
-            if (parts && dst_off + total <= dst_cap) {
-                int rcp = parts_drain(c, w, *parts, bt.c0 / c->max_batch, parts->obj0 + dst_off, total);
-                if (rcp) return rcp;
-            }
-            return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);     // one copy per batch: packed on the device
-        },
-        [&](const std::vector<Work*>& slots, int rcb) {                     // the last batches' part prefixes, once all is idle
-            if (parts) for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, *parts); pcrc_of<W>(*w).pending = -1; }
-            return rcb;
-        });
-    if (rc) return rc;
-    *n_chunks = n;
-    return TSGPU_OK;
-}
-
 // ------------------------------------------------------------------------------------------ detransform (host)
 // A batch's transformed chunks into the slot's d_xf, one per slot at i * slot_stride + TSGPU_SLOT_HEAD (16-byte aligned ciphertext
 // for the GCM kernel), and the descriptor block filled for detransform_enqueue (not yet uploaded).  Returns the bounds of the stages.
-// `src`: the batch's first transformed chunk.  to_frames (zstd only): the frames go to the d_frames slots (b_off, b_len) instead.
+// `src`: the call's transformed chunks.  to_frames (zstd only): the frames go to the d_frames slots (b_off, b_len) instead.
 static int dx_load(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, uint32_t flags, const uint8_t* src, const uint32_t* tsizes,
                    const uint8_t* aad, uint32_t aad_len, DxBounds& lim, bool to_frames = false) {
     const uint32_t c0 = bt.c0, nb = bt.nb;
@@ -1170,16 +1216,15 @@ static int dx_load(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, uint
     // releases plaintext into the next buffer before the tag is checked).  AES only: plaintext lands in d_orig
     // (chunk_cap per chunk); AES+zstd: in a d_frames slot; zstd only: the frame is read in place from d_xf.
     const uint32_t room = (flags & TSGPU_FLAG_ZSTD) ? (uint32_t)(c->frame_stride - 16) : c->chunk_cap;
-    uint64_t ip = 0, op = 0;
+    uint64_t ip = bt.in_off, op = 0;
     uint32_t max_t = 0;
+    slot_layout(c, w.hd, nb, c->slot_stride);
     for (uint32_t i = 0; i < nb; i++) {
         const uint32_t t = tsizes[c0 + i];
         const uint64_t payload = (flags & TSGPU_FLAG_AES) ? (t >= 28 ? t - 28 : 0) : t;
         if (payload > room || t > c->slot_stride - TSGPU_SLOT_HEAD - 16)
             return fail(TSGPU_E_ARG, "transformed chunk of %u bytes exceeds the context's capacity", t);
-        w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
         w.hd.c_len[i] = t;
-        w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
         w.hd.b_len[i] = (uint32_t)payload;               // what the GCM stage writes there (AES), or the frame (to_frames)
         w.hd.a_off[i] = op;                              // used when there is no zstd stage (sizes are known)
         if (t) RT(rt::h2d((to_frames ? w.d_frames + w.hd.b_off[i] : w.d_xf + w.hd.c_off[i]), src + ip, t, st));
@@ -1205,8 +1250,8 @@ static int detransform_issue(tsgpu_ctx* c, const Batch& bt, uint32_t flags, cons
     RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
     { int rc = detransform_enqueue(c, w, w.keys[0], st, flags, nb, rk, aad_len, ChunksIn{w.d_xf, w.dd.c_off, w.dd.c_len},
                                    ChunksOut{w.d_orig, w.dd.a_off, w.dd.a_len}, w.dd.status, lim, /*packed=*/true); if (rc) return rc; }
-    RT(rt::d2h(w.h_sizes, w.dd.a_len, 4ull * nb, st));
-    RT(rt::d2h(w.h_sizes + nb, w.dd.status, 4ull * nb, st));
+    RT(rt::d2h(w.back.sizes, w.dd.a_len, 4ull * nb, st));
+    RT(rt::d2h(w.back.status, w.dd.status, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
     return TSGPU_OK;
 }
@@ -1222,8 +1267,7 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
     if (!transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
     if (!dst) return fail(TSGPU_E_ARG, "dst cannot be null");
     if (flags & ~KNOWN_FLAGS) return fail(TSGPU_E_ARG, "unknown flags %u", flags);
-    if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
-    if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
+    if (int rc = aes_args_ok(flags, AES_DEC, key, true, aad, aad_len)) return rc;
     flags &= ~ZSTD_MODIFIERS;                                // how a frame was compressed does not matter to the reader
     uint64_t need = 0;
     for (uint32_t i = 0; i < n_chunks; i++) need += transformed_sizes[i];
@@ -1238,23 +1282,19 @@ extern "C" int tsgpu_detransform(tsgpu_ctx* c, uint32_t flags, const uint8_t* sr
     Aes256RoundKeys rk{};
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
 
-    uint64_t in_off = 0, dst_off = 0;                        // batches are issued in order: in_off walks src with them
+    uint64_t dst_off = 0;
     int soft = TSGPU_OK;
-    const int rc = run_batches(c, n_chunks,
-        [&](const Batch& bt) {
-            const int r = detransform_issue(c, bt, flags, src + in_off, transformed_sizes, rk, aad, aad_len);
-            for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
-            return r;
-        },
+    const int rc = run_batches(c, n_chunks, transformed_sizes,
+        [&](const Batch& bt) { return detransform_issue(c, bt, flags, src, transformed_sizes, rk, aad, aad_len); },
         [&](const Batch& bt) {
             Work& w = *bt.w;
             uint64_t total = 0;
             for (uint32_t i = 0; i < bt.nb; i++) {
-                uint32_t stt = w.h_sizes[bt.nb + i];
+                uint32_t stt = w.back.status[i];
                 if (stt == 1 && soft == TSGPU_OK) soft = fail(TSGPU_E_AUTH, "Tag mismatch in chunk %u", bt.c0 + i);
                 else if (stt > 1 && soft == TSGPU_OK) soft = fail(TSGPU_E_CORRUPT, "Invalid zstd frame in chunk %u (code %u)", bt.c0 + i, stt);
-                if (original_sizes) original_sizes[bt.c0 + i] = w.h_sizes[i];
-                total += w.h_sizes[i];
+                if (original_sizes) original_sizes[bt.c0 + i] = w.back.sizes[i];
+                total += w.back.sizes[i];
             }
             if (soft != TSGPU_OK) return soft;
             return copy_out(w, w.d_orig, total, dst, dst_cap, dst_off);
@@ -1315,9 +1355,7 @@ static int source_args(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_
     if (original_chunk_size == 0) return fail(TSGPU_E_ARG, "Original chunk size must be positive, 0 given");
     if (original_chunk_size > c->chunk_cap)
         return fail(TSGPU_E_ARG, "original chunk size %u exceeds the context's max_chunk_bytes %u", original_chunk_size, c->chunk_cap);
-    if ((flags & TSGPU_FLAG_AES) && !key) return fail(TSGPU_E_ARG, "key is required for decryption");
-    if ((flags & TSGPU_FLAG_AES) && aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "aad longer than %u bytes", MAX_AAD);
-    if ((flags & TSGPU_FLAG_AES) && aad_len && !aad) return fail(TSGPU_E_ARG, "aad cannot be null");
+    if (int rc = aes_args_ok(flags, AES_DEC, key, true, aad, aad_len)) return rc;
     q.records = flags & TSGPU_FLAG_VALIDATE_RECORDS;
     if (q.records && (uint64_t)c->max_batch * original_chunk_size > REC_MAX_BATCH)
         return fail(TSGPU_E_ARG, "record validation needs batches below 2 GiB: max_batch %u x chunk size %u is more", c->max_batch,
@@ -1367,15 +1405,13 @@ static int check_crc_word(tsgpu_ctx* c, Work& w, rt::stream_t st, const uint8_t*
     return TSGPU_OK;
 }
 
-// The source half of one batch.  `src`: the batch's first transformed chunk; `g0`: the object's chunk number of the call's first
-// chunk.  A zstd-only object's frames go to the d_frames slots with to_frames, else in place in d_xf.  Chunk i decodes to
-// d_orig + a_off[i], the offset the chunk index gives it, and v_len[i] holds its size by the index: what later stages read, so a
-// damaged chunk cannot steer them (its batch fails at the drain).  The descriptor block is uploaded here: a caller fills its
-// other fields first.  out[0, nb) receives the decoded sizes, out[nb, 2 nb) the statuses, and the 2 sizeof(W) bytes from
-// out + 2 nb the object and segment words.
+// The source half of one batch.  `g0`: the object's chunk number of the call's first chunk.  A zstd-only object's frames go to
+// the d_frames slots with to_frames, else in place in d_xf.  Chunk i decodes to d_orig + a_off[i], the offset the chunk index
+// gives it, and v_len[i] holds its size by the index: what later stages read, so a damaged chunk cannot steer them (its batch
+// fails at the drain).  The descriptor block is uploaded here: a caller fills its other fields first.  The read-back block
+// receives the decoded sizes, the statuses and the object and segment words.
 template <typename W>
-static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, const SourceReq& q, const uint8_t* src, uint64_t g0,
-                        bool to_frames, uint32_t* out) {
+static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt, const SourceReq& q, uint64_t g0, bool to_frames) {
     const uint32_t nb = bt.nb, flags = q.flags;
     uint64_t L = 0, obj = 0;                 // the batch's length by the chunk index (what it decodes to when it is sound)
     for (uint32_t i = 0; i < nb; i++) {
@@ -1385,7 +1421,7 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
     }
     DxBounds lim{};
     if (flags) {
-        int rc = dx_load(c, w, st, bt, flags, src, q.tsizes, q.aad, q.aad_len, lim, to_frames);
+        int rc = dx_load(c, w, st, bt, flags, q.src, q.tsizes, q.aad, q.aad_len, lim, to_frames);
         if (rc) return rc;
         // Chunk i decodes to a_off[i] = i * ocs: a frame may not write past ocs bytes, or it would overwrite the next chunk's
         // region while that one decodes (and reads its own output back).  A larger frame is refused as an invalid frame.
@@ -1394,12 +1430,11 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
         for (uint32_t i = 0; i < nb; i++) {
             if (q.tsizes[bt.c0 + i] > c->chunk_cap)
                 return fail(TSGPU_E_ARG, "transformed chunk of %u bytes exceeds the context's capacity", q.tsizes[bt.c0 + i]);
-            out[i] = w.hd.a_len[i] = q.tsizes[bt.c0 + i];         // a_len: the decoded sizes, as the stages write them
-            out[nb + i] = 0;
-            w.hd.b_off[i] = (uint64_t)i * c->frame_stride;      // the slots a target half writes
-            w.hd.c_off[i] = (uint64_t)i * c->slot_stride + TSGPU_SLOT_HEAD;
+            w.back.src_sizes[i] = w.hd.a_len[i] = q.tsizes[bt.c0 + i];     // a_len: the decoded sizes, as the stages write them
+            w.back.src_status[i] = 0;
         }
-        if (obj) RT(rt::h2d(w.d_orig, src, obj, st));
+        slot_layout(c, w.hd, nb, c->slot_stride);              // the slots a target half writes
+        if (obj) RT(rt::h2d(w.d_orig, q.src + bt.in_off, obj, st));
     }
     for (uint64_t i = 0, a = 0; i < nb; a += w.hd.v_len[i++]) w.hd.a_off[i] = a;
     RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
@@ -1413,7 +1448,7 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
                                      w.dd.status, lim, /*packed=*/false);
         if (rc) return rc;
 #ifdef TSGPU_SIMT
-        simt_flip_decoded(ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, bt.c0, nb);
+        simt_flip("TSGPU_SIMT_FLIP_DECODED", ChunksOut{w.d_orig, w.dd.a_off, w.dd.v_len}, bt.c0, nb);
 #endif
     }
     // The segment word and the records over the L bytes the index gives: a batch that decodes to another length fails first.
@@ -1424,21 +1459,21 @@ static int source_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, const Batch& bt,
         if (rc) return rc;
     }
     if (flags) {
-        RT(rt::d2h(out, w.dd.a_len, 4ull * nb, st));
-        RT(rt::d2h(out + nb, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.back.src_sizes, w.dd.a_len, 4ull * nb, st));
+        RT(rt::d2h(w.back.src_status, w.dd.status, 4ull * nb, st));
     }
-    RT(rt::d2h(out + 2 * nb, pcrc_of<W>(w).d_cuts, 2 * sizeof(W), st));
+    RT(rt::d2h(w.back.words, pcrc_of<W>(w).d_cuts, 2 * sizeof(W), st));
     return TSGPU_OK;
 }
 
-// A drained batch in object order (`out` as source_stage filled it): every chunk's tag, frame and decoded size, then the record
-// verdict, then the CRC words extend the carry.
+// A drained batch in object order (as source_stage left it): every chunk's tag, frame and decoded size, then the record verdict,
+// then the CRC words extend the carry.
 template <typename W>
-static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const uint32_t* out, CheckCarry<W>& cur) {
+static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, CheckCarry<W>& cur) {
     Work& w = *bt.w;
     const uint32_t nb = bt.nb;
-    const uint32_t* got = out;
-    const uint32_t* status = out + nb;
+    const uint32_t* got = w.back.src_sizes;
+    const uint32_t* status = w.back.src_status;
     const ChunkLayout& index = q.index;
     uint64_t L = 0, obj = 0;
     for (uint32_t i = 0; i < nb; i++) {
@@ -1454,8 +1489,7 @@ static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const
         obj += q.tsizes[bt.c0 + i];
     }
     if (q.records) { int rc = records_resolve(c, w, cur.rec); if (rc) return rc; }
-    W words[2];                                                        // 4-byte aligned only
-    memcpy(words, out + 2 * nb, sizeof words);
+    const W* words = reinterpret_cast<const W*>(w.back.words);
     const W seg_word = words[1], obj_word = q.flags ? words[0] : seg_word;
     cur.obj_raw = crc_shift(cur.obj_raw, obj, 0) ^ obj_word;
     cur.seg_raw = crc_shift(cur.seg_raw, L, 0) ^ seg_word;
@@ -1493,18 +1527,15 @@ static int check_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64
                          cur.chunks, q);
     if (rc) return rc;
     if (q.n) {
-        uint64_t in_off = 0;                                     // batches are issued in order: in_off walks src with them
-        rc = run_batches(c, q.n,
+        rc = run_batches(c, q.n, transformed_sizes,
             [&](const Batch& bt) {
                 Work& w = *bt.w;
                 RT(rt::set_device(w.device));
-                const int r = source_stage<W>(c, w, w.stream, bt, q, src + in_off, cur.chunks, /*to_frames=*/false, w.h_sizes);
-                for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
-                if (r) return r;
+                { int r = source_stage<W>(c, w, w.stream, bt, q, cur.chunks, /*to_frames=*/false); if (r) return r; }
                 RT(rt::event_record(w.ev_sizes, w.stream));
                 return TSGPU_OK;
             },
-            [&](const Batch& bt) { return source_drain(c, bt, q, bt.w->h_sizes, cur); });
+            [&](const Batch& bt) { return source_drain(c, bt, q, cur); });
         if (rc) return rc;
     }
     if ((rc = source_finish(q, cur, object_ends_here))) return rc;
@@ -1549,21 +1580,9 @@ template <typename W> struct RewriteCarry {
 static_assert(sizeof(RewriteCarry<uint32_t>) == sizeof(tsgpu_rewrite_cursor) && sizeof(RewriteCarry<uint64_t>) == sizeof(tsgpu_rewrite_cursor),
               "the cursor holds the carry");
 
-// The new object's side of a rewrite.
-struct TargetReq {
-    uint32_t flags;                  // ZSTD, modifiers and AES of the new object
-    bool verify, kept;               // kept: the source frames go into the new object as they are
-    uint32_t reframe;                // TSGPU_FLAG_REFRAME: the ZSTD_DENSE and ZSTD_CHECKSUM bits that act on the kept frames, else 0
-    Aes256RoundKeys rk;
-    const uint8_t* aad; uint32_t aad_len;
-    const uint8_t* ivs;
-};
-
-// One batch of a rewrite: the target's IVs and AAD, the source half, the target half, the D2H of the new sizes.  h_sizes:
-// [0, nb) new sizes, [nb, 3 nb) the verify stage's verdicts (verify_verdict), [3 nb, 5 nb + 2 sizeof(W) / 4) the source half's
-// out (its two CRC words take 2 or 4 of the 16 words h_sizes has beyond 5 nb).
+// One batch of a rewrite: the target's IVs and AAD, the source half, the target half, the D2H of the new sizes.
 template <typename W>
-static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const TargetReq& t, const uint8_t* src, uint64_t g0) {
+static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const TargetReq& t, uint64_t g0) {
     Work& w = *bt.w;
     const uint32_t nb = bt.nb;
     RT(rt::set_device(w.device));
@@ -1581,16 +1600,16 @@ static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, cons
             RT(rt::h2d(k.d_aad, k.h_aad, t.aad_len, st));
         }
     }
-    { int rc = source_stage<W>(c, w, st, bt, q, src, g0, /*to_frames=*/q.flags == TSGPU_FLAG_ZSTD, w.h_sizes + 3 * nb); if (rc) return rc; }
+    { int rc = source_stage<W>(c, w, st, bt, q, g0, /*to_frames=*/q.flags == TSGPU_FLAG_ZSTD); if (rc) return rc; }
     uint64_t frames_max = 0;                 // the largest kept frame, by the object's sizes
     for (uint32_t i = 0; i < nb; i++) {
         const uint32_t ts = q.tsizes[bt.c0 + i];
         frames_max = std::max<uint64_t>(frames_max, (q.flags & TSGPU_FLAG_AES) ? (ts >= 28 ? ts - 28 : 0) : ts);
     }
     ChunksOut fin;
-    { int rc = target_stage(c, w, k, st, t.flags, t.verify, /*parts=*/(int)sizeof(W), bt.c0, nb, q.index.ocs, t.rk, t.aad_len,
-                            ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len}, t.kept, frames_max, fin, t.reframe); if (rc) return rc; }
-    RT(rt::d2h(w.h_sizes, fin.len, 4ull * nb, st));
+    { int rc = target_stage<W>(c, w, k, st, t, /*parts=*/true, bt.c0, nb, q.index.ocs, ChunksIn{w.d_orig, w.dd.a_off, w.dd.v_len},
+                               frames_max, fin); if (rc) return rc; }
+    RT(rt::d2h(w.back.sizes, fin.len, 4ull * nb, st));
     RT(rt::event_record(w.ev_sizes, st));
     return TSGPU_OK;
 }
@@ -1622,10 +1641,7 @@ static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src,
     if (kept && !reframe && (to_flags & ZSTD_MODIFIERS))
         return fail(TSGPU_E_ARG, "to_flags %u: the source frames are kept as they are, so TSGPU_FLAG_ZSTD_DENSE and "
                     "TSGPU_FLAG_ZSTD_CHECKSUM have nothing to act on", to_flags);
-    if ((to_flags & TSGPU_FLAG_AES) && (!to_key || (n_chunks && !to_ivs)))
-        return fail(TSGPU_E_ARG, "to_key and to_ivs are required for encryption");
-    if ((to_flags & TSGPU_FLAG_AES) && to_aad_len > MAX_AAD) return fail(TSGPU_E_ARG, "to_aad longer than %u bytes", MAX_AAD);
-    if ((to_flags & TSGPU_FLAG_AES) && to_aad_len && !to_aad) return fail(TSGPU_E_ARG, "to_aad cannot be null");
+    if (int rc = aes_args_ok(to_flags, AES_TO, to_key, !n_chunks || to_ivs, to_aad, to_aad_len)) return rc;
     if (n_chunks && !new_transformed_sizes) return fail(TSGPU_E_ARG, "new_transformed_sizes cannot be null");
     RewriteCarry<W> cur;
     memcpy(&cur, cursor, sizeof cur);
@@ -1677,8 +1693,9 @@ static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src,
         frames += frame + seal + ((to_flags & TSGPU_FLAG_AES) ? 28 : 0);
     }
     const uint64_t bound = !q.n ? 0 : kept ? frames : tsgpu_transform_bound(to_flags, L, original_chunk_size);
-    const PartsReq<W> pq{part_size, &cur.out, part_crc, part_cap, n_parts, object_crc};
-    if ((rc = parts_args_ok(pq, to_flags, bound, object_ends_here))) return rc;
+    PartsRun<W> run;
+    if ((rc = parts_begin(run, PartsReq<W>{part_size, &cur.out, part_crc, part_cap, n_parts, object_crc}, to_flags, bound,
+                          object_ends_here))) return rc;
 
     TargetReq t{};
     t.flags = to_flags & ~(TSGPU_FLAG_VERIFY | TSGPU_FLAG_REFRAME);
@@ -1688,42 +1705,23 @@ static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src,
     t.reframe = reframe ? to_flags & ZSTD_MODIFIERS : 0;
     if (to_flags & TSGPU_FLAG_AES) t.rk = aes256_expand_key(to_key);
     t.aad = to_aad; t.aad_len = to_aad_len; t.ivs = to_ivs;
-    PartsRun<W> run;
-    PartsCarry<W> out0;
-    memcpy(&out0, &cur.out, sizeof out0);
-    run.part_size = part_size; run.obj0 = out0.obj_len;
     if (q.n) {
         std::vector<uint32_t> len(q.n);                          // the window's original sizes (verify_verdict's messages)
         for (uint32_t i = 0; i < q.n; i++) len[i] = q.index.size(cur.src.chunks + i);
-        run.batches.assign((q.n + c->max_batch - 1) / c->max_batch, PcrcBatch<W>{});
-        uint64_t in_off = 0, dst_off = 0;                        // batches are issued in order: in_off walks src with them
-        rc = run_batches(c, q.n,
+        uint64_t dst_off = 0;
+        rc = run_batches(c, q.n, transformed_sizes,
+            [&](const Batch& bt) { return rewrite_issue<W>(c, bt, q, t, cur.src.chunks); },
             [&](const Batch& bt) {
-                const int r = rewrite_issue<W>(c, bt, q, t, src + in_off, cur.src.chunks);
-                for (uint32_t i = 0; i < bt.nb; i++) in_off += transformed_sizes[bt.c0 + i];
-                return r;
-            },
-            [&](const Batch& bt) {
-                Work& w = *bt.w;
-                { int r = source_drain(c, bt, q, w.h_sizes + 3 * bt.nb, cur.src); if (r) return r; }
+                { int r = source_drain(c, bt, q, cur.src); if (r) return r; }
                 if (t.verify) { int r = verify_verdict(bt, len.data(), cur.src.chunks); if (r) return r; }
-                uint64_t total = 0;
-                for (uint32_t i = 0; i < bt.nb; i++) { new_transformed_sizes[bt.c0 + i] = w.h_sizes[i]; total += w.h_sizes[i]; }
-                if (dst_off + total <= dst_cap) {
-                    int r = parts_drain(c, w, run, bt.c0 / c->max_batch, run.obj0 + dst_off, total);
-                    if (r) return r;
-                }
-                return copy_out(w, w.d_pack, total, dst, dst_cap, dst_off);
+                return target_drain(c, bt, new_transformed_sizes, &run, dst, dst_cap, dst_off);
             },
-            [&](const std::vector<Work*>& slots, int rcb) {          // the last batches' part prefixes, once all is idle
-                for (Work* w : slots) { if (rcb == TSGPU_OK) parts_collect(*w, run); pcrc_of<W>(*w).pending = -1; }
-                return rcb;
-            });
+            [&](const std::vector<Work*>& slots, int rcb) { return parts_idle(&run, slots, rcb); });
         if (rc) return rc;
     }
     if ((rc = source_finish(q, cur.src, object_ends_here))) return rc;
     if (n_chunks && !q.n) new_transformed_sizes[0] = 0;                    // the empty segment's one empty chunk stays one
-    parts_finish(pq, out0, q.n ? &run : nullptr, object_ends_here);       // writes cur.out and the part CRCs
+    parts_finish(run, object_ends_here);                                   // writes cur.out and the part CRCs
     if (object_ends_here) {
         *source_crc = crc_finish(cur.src.obj_raw, cur.src.obj_len, 0);
         *segment_crc = crc_finish(cur.src.seg_raw, cur.src.seg_len, 0);
@@ -1802,7 +1800,7 @@ extern "C" int tsgpu_transform_device(tsgpu_ctx* c, int device_index, uint32_t f
     const uint64_t n64 = chunk_size ? (src_len + chunk_size - 1) / chunk_size : 0;
     int rc = dev_args_ok(c, device_index, flags, chunk_size, n64, slot_stride);
     if (rc || n64 == 0) return rc;
-    if ((flags & TSGPU_FLAG_AES) && (!key || !ivs || aad_len > MAX_AAD)) return fail(TSGPU_E_ARG, "key/ivs/aad invalid");
+    if ((rc = aes_args_ok(flags, AES_ENC, key, ivs != nullptr, aad, aad_len))) return rc;
     const uint32_t nb = (uint32_t)n64, cs = chunk_size;
     Aes256RoundKeys rk{};
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
@@ -1812,9 +1810,8 @@ extern "C" int tsgpu_transform_device(tsgpu_ctx* c, int device_index, uint32_t f
         for (uint32_t i = 0; i < nb; i++) {
             w.hd.a_off[i] = (uint64_t)i * cs;
             w.hd.a_len[i] = (uint32_t)std::min<uint64_t>(cs, src_len - (uint64_t)i * cs);
-            w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
-            w.hd.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD;
         }
+        slot_layout(c, w.hd, nb, slot_stride);
         if (flags & TSGPU_FLAG_AES) {
             memcpy(w.hd.ivs, ivs, (size_t)nb * TSGPU_IV_SIZE);
             if (aad_len) memcpy(w.hd.aad, aad, aad_len);
@@ -1836,18 +1833,15 @@ extern "C" int tsgpu_detransform_device(tsgpu_ctx* c, int device_index, uint32_t
     int rc = dev_args_ok(c, device_index, flags, chunk_size, n_chunks, slot_stride);
     if (rc || n_chunks == 0) return rc;
     flags &= ~ZSTD_MODIFIERS;                                // how a frame was compressed does not matter to the reader
-    if ((flags & TSGPU_FLAG_AES) && (!key || aad_len > MAX_AAD)) return fail(TSGPU_E_ARG, "key/aad invalid");
+    if ((rc = aes_args_ok(flags, AES_DEC, key, true, aad, aad_len))) return rc;
     if (!d_slots || !d_transformed_sizes || !d_dst || !d_original_sizes || !d_status) return fail(TSGPU_E_ARG, "null device pointer");
     Aes256RoundKeys rk{};
     if (flags & TSGPU_FLAG_AES) rk = aes256_expand_key(key);
     rt::stream_t st = (rt::stream_t)stream;
     SlotClaim claim;
     rc = dev_call_begin(c, device_index, st, claim, [&](Work& w) {
-        for (uint32_t i = 0; i < n_chunks; i++) {
-            w.hd.c_off[i] = (uint64_t)i * slot_stride + TSGPU_SLOT_HEAD;
-            w.hd.b_off[i] = (uint64_t)i * c->frame_stride;
-            w.hd.a_off[i] = (uint64_t)i * chunk_size;        // original side: chunk i at i * chunk_size
-        }
+        slot_layout(c, w.hd, n_chunks, slot_stride);
+        for (uint32_t i = 0; i < n_chunks; i++) w.hd.a_off[i] = (uint64_t)i * chunk_size;     // original side: chunk i at i * chunk_size
         if ((flags & TSGPU_FLAG_AES) && aad_len) memcpy(w.hd.aad, aad, aad_len);
     });
     if (rc) return rc;
