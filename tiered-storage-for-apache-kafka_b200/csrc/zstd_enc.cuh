@@ -199,17 +199,17 @@ __device__ __forceinline__ void ze_seq_hist(const uint2* __restrict__ seqs, uint
 
 // ze_build_kind for one sequence code, k = 0 LL, 1 OF, 2 ML (the order of the descriptions in the stream), from the histograms
 // in cnt (LL, ML, OF back to back) with the predefined tables as the Predefined_Mode choice.  CT: ZeCTab or a smaller table
-// set with the same members.
+// set with the same members.  Returns ze_build_kind's packed result.
 template <class CT>
 __device__ __forceinline__ uint32_t ze_build_seq_kind(uint32_t k, uint32_t* cnt, uint32_t N, CT* ct, uint8_t* scratch, uint8_t* desc,
-                                                      ZeKind* kind, uint32_t lane) {
+                                                      uint32_t lane) {
     const zf::PredefinedCTables& pre = g_pre_ctables;
     if (k == 0) return ze_build_kind(cnt, ZE_NSYM_LL, N, zf::LL_MAX_LOG, zf::LL_DEFAULT_LOG, pre.ll.state, pre.ll.sym,
-                                     ct->st_ll, ct->sy_ll, scratch, desc, kind, true, lane);
+                                     ct->st_ll, ct->sy_ll, scratch, desc, true, lane);
     if (k == 1) return ze_build_kind(cnt + ZE_NSYM_LL + ZE_NSYM_ML, ZE_NSYM_OF, N, zf::OF_MAX_LOG, zf::OF_DEFAULT_LOG, pre.of.state,
-                                     pre.of.sym, ct->st_of, ct->sy_of, scratch, desc, kind, true, lane);
+                                     pre.of.sym, ct->st_of, ct->sy_of, scratch, desc, true, lane);
     return ze_build_kind(cnt + ZE_NSYM_LL, ZE_NSYM_ML, N, zf::ML_MAX_LOG, zf::ML_DEFAULT_LOG, pre.ml.state, pre.ml.sym,
-                         ct->st_ml, ct->sy_ml, scratch, desc, kind, true, lane);
+                         ct->st_ml, ct->sy_ml, scratch, desc, true, lane);
 }
 
 // Number_of_Sequences field: its size, and the field itself (one lane; returns the size)
@@ -651,11 +651,11 @@ __global__ void __launch_bounds__(ZE_THREADS, 2) zstd_enc_regions_kernel(const _
         if (w == 0) {
             ze_huf_build(S->hist, S->ctab, (uint32_t*)fin_area, nlit_total, &S->huf, lane);
         } else if (w <= 3 && nseq_total) {
-            ZeKind k;
-            const uint32_t dn = ze_build_seq_kind(w - 1, S->cnt, nseq_total, &S->ct, fin_area + 8192 + (w - 1) * ZE_KIND_SCRATCH,
-                                                  S->desc[w - 1], &k, lane);
+            const uint32_t r = ze_build_seq_kind(w - 1, S->cnt, nseq_total, &S->ct, fin_area + 8192 + (w - 1) * ZE_KIND_SCRATCH,
+                                                 S->desc[w - 1], lane);
+            const ZeKind k = ze_kind_of(r);
             if (lane == 0) {
-                S->desc_len[w - 1] = dn;
+                S->desc_len[w - 1] = ze_kind_bytes(r);
                 if (w == 1) R->kll = k; else if (w == 2) R->kof = k; else R->kml = k;
             }
         }

@@ -4,7 +4,7 @@
 // different trade: every 8 KiB block is self-contained (own Huffman tree, own FSE tables, no match leaves the block), so a
 // 1 GiB segment is 131,072 independent warps with no barrier between them, 20 warps per SM.  That is the round-1 kernel with
 // the streamlined FSE chains and the backwards growth of taken matches ("catch up"); it compresses the K corpus ~3.1 : 1 at
-// ~14.9 ms per GiB on an H100, where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
+// ~13.8 ms per GiB on an H100 (700 W), where the region kernel of zstd_enc.cuh reaches ~3.5 : 1 at about twice the time (one 64 KiB
 // window and one set of tables per 8 blocks).  TSGPU_FLAG_ZSTD picks this kernel, TSGPU_FLAG_ZSTD | TSGPU_FLAG_ZSTD_DENSE the region kernel;
 // the decoder reads both through the same region path (zstd_dec.cuh).
 //   zstd_enc_blocks_kernel    one WARP per block: block staged in shared memory; 32 positions hashed and verified per step
@@ -51,6 +51,8 @@ constexpr uint32_t ZB_SMEM_WARP = ZB + ZB_BUF_PAD + ZB_HSIZE * 2;   // buf, ht
 constexpr uint32_t ZB_SMEM_WARP_AL = (ZB_SMEM_WARP + 15) & ~15u;
 // the sequence bit stream is staged in `buf`, its per-tile FSE scratch at ZE_SEQ_AUX_OFF in the tail
 static_assert(ZE_SEQ_AUX_OFF + 3 * 32 * 8 + 3 * 32 * 4 <= ZB + ZB_BUF_PAD, "FSE tile scratch must fit the block buffer");
+static_assert(ZE_SEQ_AUX_OFF % 16 == 0 && 2048 + 3 * 128 <= ZE_SEQ_AUX_OFF, "the bit stream area is cleared in 16-byte stores; "
+              "the three table descriptions are staged in it");
 struct ZbCTab {                                // per-warp FSE encoding tables (logs <= 7 for <= 1024 sequences); aliases the hash-table area
     uint16_t st_ll[128], st_ml[128], st_of[128];
     zf::FseCSym sy_ll[ZE_NSYM_LL], sy_ml[ZE_NSYM_ML], sy_of[ZE_NSYM_OF];
@@ -231,31 +233,158 @@ __device__ __forceinline__ uint32_t zb_encode_literals(const uint8_t* __restrict
 }
 
 
+// Bit stream of one block's sequences, staged in the word buffer `bits` (shared, zeroed below ZE_SEQ_AUX_OFF), with the
+// per-tile scratch at ZE_SEQ_AUX_OFF.  Returns its size in bytes.  Warp-uniform, N >= 1.  Per tile of 32 sequences every lane
+// stages the transforms of its sequence's three codes; lanes 0-2 walk the three state chains (OF, ML, LL) and record only the
+// state each symbol is encoded from (one 8-byte load, two shifts, an add, one store, one table load per symbol); every lane
+// then derives its fields' bit counts from those states and the transforms it kept, and packs its field.  An RLE kind comes
+// with st[0] = 0 and a zero transform for its code, so its chain stays at state 0 and emits nothing, without a branch.  The
+// `seq:` markers split the section into the parts whose static instructions scripts/seq_section_sass.py counts.
+__device__ __forceinline__ uint32_t zb_encode_seq_bits(const uint2* __restrict__ seqs, uint32_t N, uint32_t* bits, const ZbCTab* ct,
+                                                       const ZeCodeTabs* tabs, uint32_t log_ll, uint32_t log_of, uint32_t log_ml,
+                                                       uint32_t lane) {
+    uint2* pk = (uint2*)((uint8_t*)bits + ZE_SEQ_AUX_OFF);   // [3][32] OF, ML, LL: delta_nb_bits, index base in `st`
+    uint16_t* sb = (uint16_t*)(pk + 96);                     // [3][32] the state each symbol is encoded from
+    const uint16_t* st = ct->st_ll;                          // st_ll, st_ml, st_of back to back
+    const uint2* mypk = pk + min(lane, 2u) * 32;
+    uint16_t* mysb = sb + min(lane, 2u) * 32;
+    uint32_t state = 0, bitpos = 0;                          // lanes 0..2: OF, ML, LL chains
+    uint2 pre = lane < N ? seqs[N - 1 - lane] : make_uint2(0, 0);
+    for (uint32_t t0 = 0; t0 < N; t0 += 32) {
+        // seq: fill
+        const uint32_t j = t0 + lane;                        // stream order: j = 0 is the LAST sequence
+        const bool have = j < N;
+        const uint2 s = pre;
+        if (j + 32 < N) pre = seqs[N - 1 - (j + 32)];
+        const uint32_t ll = s.x & 0xffff, mlb = s.x >> 16, offb = s.y + 3;     // mlb = matchLength - 3, offb = offset + 3 (no repcodes)
+        const uint32_t llc = ze_ll_code_s(tabs, ll), mlc = ze_ml_code_s(tabs, mlb), ofc = (uint32_t)zf::highbit32(offb);
+        const zf::FseCSym a = ct->sy_of[ofc], b = ct->sy_ml[mlc], c = ct->sy_ll[llc];
+        pk[lane] = make_uint2((uint32_t)a.delta_nb_bits, (uint32_t)a.delta_find_state + 256u);
+        pk[32 + lane] = make_uint2((uint32_t)b.delta_nb_bits, (uint32_t)b.delta_find_state + 128u);
+        pk[64 + lane] = make_uint2((uint32_t)c.delta_nb_bits, (uint32_t)c.delta_find_state);
+        __syncwarp();
+        // seq: chain
+        if (lane < 3) {
+            if (t0 == 0) {                                   // FSE_initCState2 is one encoding step from this state (its bits are dropped)
+                const uint32_t x = mypk[0].x;
+                state = (((x + (1u << 15)) >> 16) << 16) - x;
+            }
+            if (N - t0 >= 32) {
+                _Pragma("unroll")
+                for (uint32_t i = 0; i < 32; i++) {          // FSE_encodeSymbol
+                    const uint2 e = mypk[i];
+                    const uint32_t nb = (state + e.x) >> 16;
+                    mysb[i] = (uint16_t)state;
+                    state = st[(state >> nb) + e.y];
+                }
+            } else {
+                // seq: chain_tail
+                for (uint32_t i = 0; i < N - t0; i++) {
+                    const uint2 e = mypk[i];
+                    const uint32_t nb = (state + e.x) >> 16;
+                    mysb[i] = (uint16_t)state;
+                    state = st[(state >> nb) + e.y];
+                }
+            }
+        }
+        // seq: chain_sync
+        __syncwarp();
+        // seq: pack
+        // order inside a field (first written = lowest bits): OF state, ML state, LL state, LL extra, ML extra, OF extra.
+        // (No rendezvous after the tile: the next tile's stores to pk come after this tile's chains, and its chains store to
+        // sb only after a rendezvous that every lane reaches once it has packed.)
+        uint64_t field = 0; uint32_t nb = 0;
+        if (have) {
+            const uint32_t keep = j ? 0xffffffffu : 0u;     // the first symbol's states (initCState2) emit nothing
+            const uint32_t s0 = sb[lane], s1 = sb[32 + lane], s2 = sb[64 + lane];
+            const uint32_t n0 = ((s0 + (uint32_t)a.delta_nb_bits) >> 16) & keep, n1 = ((s1 + (uint32_t)b.delta_nb_bits) >> 16) & keep,
+                           n2 = ((s2 + (uint32_t)c.delta_nb_bits) >> 16) & keep;
+            uint32_t sv = s0 & ~zb_ones_from(n0);
+            sv |= (s1 & ~zb_ones_from(n1)) << n0; nb = n0 + n1;
+            sv |= (s2 & ~zb_ones_from(n2)) << nb; nb += n2;  // at most 3 x 7 bits
+            const uint32_t llb = tabs->ll_bits[llc], mlbits = tabs->ml_bits[mlc];
+            field = sv | (uint64_t)(ll & ~zb_ones_from(llb)) << nb; nb += llb;
+            field |= (uint64_t)(mlb & ~zb_ones_from(mlbits)) << nb; nb += mlbits;
+            field |= (uint64_t)(offb & ~zb_ones_from(ofc)) << nb; nb += ofc;
+        }
+        const uint32_t inc = warp_inclusive_scan_u32(nb, lane);
+        ze_put_bits(bits, bitpos + inc - nb, field, nb);
+        bitpos += __shfl_sync(TS_FULL, inc, 31);
+    }
+    // seq: flush
+    // FSE_flushCState x3 (ML, OF, LL) then the closing 1 bit
+    const uint32_t st_of = __shfl_sync(TS_FULL, state, 0), st_ml = __shfl_sync(TS_FULL, state, 1),
+                   st_ll = __shfl_sync(TS_FULL, state, 2);
+    if (lane == 0) {
+        uint64_t f = st_ml & ((1u << log_ml) - 1);
+        uint32_t nb = log_ml;
+        f |= (uint64_t)(st_of & ((1u << log_of) - 1)) << nb; nb += log_of;
+        f |= (uint64_t)(st_ll & ((1u << log_ll) - 1)) << nb; nb += log_ll;
+        f |= 1ull << nb; nb += 1;
+        ze_put_bits(bits, bitpos, f, nb);
+    }
+    bitpos += log_ml + log_of + log_ll + 1;
+    __syncwarp();
+    return (bitpos + 7) >> 3;
+    // seq: end
+}
+
 // Encodes the sequences section (everything after the Number_of_Sequences field): the modes byte and table
 // descriptions go straight to `hdr_out` (global), the bit stream is staged in the word buffer `bits` (shared).
 // Returns the bit-stream bytes; *desc_bytes = 1 (modes byte) + table descriptions.  Warp-uniform, N >= 1.
 __device__ __forceinline__ uint32_t zb_encode_sequences(const uint2* __restrict__ seqs, uint32_t N, uint32_t* bits, ZbCTab* ct,
                                                         const ZeCodeTabs* tabs, uint8_t* hdr_out, uint32_t* desc_bytes,
                                                         uint32_t lane ZB_PH_PARAM) {
+    // seq: hist
     // code histograms (then normalised counts), in the word buffer beyond ze_build_kind's own scratch
     uint32_t* cnt = bits + 256;
     for (uint32_t i = lane; i < ZE_NSYM_LL + ZE_NSYM_ML + ZE_NSYM_OF; i += 32) cnt[i] = 0;
     __syncwarp();
     ze_seq_hist(seqs, N, cnt, tabs, lane);
     __syncwarp();
-    // tables (descriptions in stream order LL, OF, ML); `bits` doubles as scratch until it is cleared
-    ZeKind kll, kof, kml;
-    uint8_t* desc = hdr_out + 1;
-    uint32_t dn = ze_build_seq_kind(0, cnt, N, ct, (uint8_t*)bits, desc, &kll, lane);
-    dn += ze_build_seq_kind(1, cnt, N, ct, (uint8_t*)bits, desc + dn, &kof, lane);
-    dn += ze_build_seq_kind(2, cnt, N, ct, (uint8_t*)bits, desc + dn, &kml, lane);
-    if (lane == 0) hdr_out[0] = (uint8_t)((kll.mode << 6) | (kof.mode << 4) | (kml.mode << 2));
-    *desc_bytes = 1 + dn;
+    // seq: tables
+    // the three tables; `bits` doubles as scratch until it is cleared.  The descriptions are left to the lanes below.
+    const uint32_t rll = ze_build_seq_kind(0, cnt, N, ct, (uint8_t*)bits, nullptr, lane);
+    const uint32_t rof = ze_build_seq_kind(1, cnt, N, ct, (uint8_t*)bits, nullptr, lane);
+    const uint32_t rml = ze_build_seq_kind(2, cnt, N, ct, (uint8_t*)bits, nullptr, lane);
+    // seq: desc
+    // lane k writes description k (LL, OF, ML: their order in the stream) into its own 128 bytes of `bits`, the three at
+    // once, then the warp copies them out back to back
+    uint8_t* dstage = (uint8_t*)bits + 2048;
+    uint32_t dn = 0;
+    if (lane < 3) {
+        const uint32_t r = lane == 0 ? rll : lane == 1 ? rof : rml;
+        const ZeKind k = ze_kind_of(r);
+        const uint32_t max_sym = ze_kind_max_sym(r);
+        uint8_t* o = dstage + lane * 128;
+        if (k.mode == 2) {
+            dn = ze_write_ncount(o, cnt + (lane == 0 ? 0 : lane == 1 ? ZE_NSYM_LL + ZE_NSYM_ML : ZE_NSYM_LL), max_sym + 1, k.log);
+        } else if (k.mode == 1) {
+            o[0] = (uint8_t)max_sym;
+            dn = 1;
+            zf::FseCSym* sy = lane == 0 ? ct->sy_ll : lane == 1 ? ct->sy_of : ct->sy_ml;
+            uint16_t* stk = lane == 0 ? ct->st_ll : lane == 1 ? ct->st_of : ct->st_ml;
+            sy[max_sym] = zf::FseCSym{0, 0};                 // see zb_encode_seq_bits
+            stk[0] = 0;
+        }
+    }
     __syncwarp();
-    for (uint32_t i = lane; i < (ZB + ZB_BUF_PAD) / 4; i += 32) bits[i] = 0;
+    const uint32_t n_ll = __shfl_sync(TS_FULL, dn, 0), n_of = __shfl_sync(TS_FULL, dn, 1), n_ml = __shfl_sync(TS_FULL, dn, 2);
+    uint8_t* desc = hdr_out + 1;
+    for (uint32_t i = lane; i < n_ll; i += 32) desc[i] = dstage[i];
+    for (uint32_t i = lane; i < n_of; i += 32) desc[n_ll + i] = dstage[128 + i];
+    for (uint32_t i = lane; i < n_ml; i += 32) desc[n_ll + n_of + i] = dstage[256 + i];
+    const ZeKind kll = ze_kind_of(rll), kof = ze_kind_of(rof), kml = ze_kind_of(rml);
+    if (lane == 0) hdr_out[0] = (uint8_t)((kll.mode << 6) | (kof.mode << 4) | (kml.mode << 2));
+    *desc_bytes = 1 + n_ll + n_of + n_ml;
+    __syncwarp();
+    // seq: clear
+    // the bit stream ends below ZE_SEQ_AUX_OFF (zstd_enc.cuh): only that part is cleared, 16 bytes per store
+    for (uint32_t i = lane; i < ZE_SEQ_AUX_OFF / 16; i += 32) ((uint4*)bits)[i] = make_uint4(0, 0, 0, 0);
     __syncwarp();
     ZB_MARK(5);
-    return ze_encode_seq_bits(seqs, N, bits, ct, tabs, kll, kof, kml, lane);
+    return zb_encode_seq_bits(seqs, N, bits, ct, tabs, kll.log, kof.log, kml.log, lane);
+    // seq: end
 }
 
 __global__ void __launch_bounds__(ZB_WPB * 32, 5) zstd_enc_blocks_kernel(const __grid_constant__ ZstdBlkArgs A) {

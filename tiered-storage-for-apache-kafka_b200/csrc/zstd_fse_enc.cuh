@@ -32,6 +32,11 @@ struct ZeKind {                                   // uniform per-kind parameters
     uint32_t mode;                                // 0 predefined, 1 RLE, 2 FSE compressed
     uint32_t log;                                 // table log (0 for RLE)
 };
+// ze_build_kind's result in one register (no stack frame for an out-parameter of the non-inlined call):
+// description bytes | mode << 8 | log << 12 | largest present code << 16
+__device__ __forceinline__ uint32_t ze_kind_bytes(uint32_t r) { return r & 0xff; }
+__device__ __forceinline__ ZeKind ze_kind_of(uint32_t r) { return ZeKind{(r >> 8) & 3, (r >> 12) & 15}; }
+__device__ __forceinline__ uint32_t ze_kind_max_sym(uint32_t r) { return r >> 16; }
 
 // ---- table description, libzstd FSE_writeNCount layout.  One lane.  Returns bytes written.
 __device__ TS_NOINLINE uint32_t ze_write_ncount(uint8_t* out, const uint32_t* norm, uint32_t alphabet, uint32_t log) {
@@ -73,26 +78,25 @@ __device__ TS_NOINLINE uint32_t ze_write_ncount(uint8_t* out, const uint32_t* no
 
 // ---- choose the mode of one kind and build its encoding tables.  Warp-uniform.
 // cnt[alphabet]: histogram on entry, normalised counts on exit (FSE mode).  scratch: >= 512 + 4*68 bytes of shared memory.
-// Returns the bytes of table description written at desc (global).
+// Writes the table description at desc (the RLE byte, or FSE_writeNCount on lane 0) unless desc is null, when the caller
+// writes it.  Returns the packed result above.
 __device__ TS_NOINLINE uint32_t ze_build_kind(uint32_t* cnt, uint32_t alphabet, uint32_t N, uint32_t max_log, uint32_t default_log,
                                                   const uint16_t* pre_state, const zf::FseCSym* pre_sym, uint16_t* st, zf::FseCSym* sy,
-                                                  uint8_t* scratch, uint8_t* desc, ZeKind* kind, bool allow_predefined, uint32_t lane) {
+                                                  uint8_t* scratch, uint8_t* desc, bool allow_predefined, uint32_t lane) {
     const uint32_t c0 = lane < alphabet ? cnt[lane] : 0, c1 = lane + 32 < alphabet ? cnt[lane + 32] : 0;
     const uint32_t used0 = __ballot_sync(TS_FULL, c0 != 0), used1 = __ballot_sync(TS_FULL, c1 != 0);
     const uint32_t nused = (uint32_t)__popc(used0) + (uint32_t)__popc(used1);
     const uint32_t max_sym = used1 ? 32 + (31 - (uint32_t)__clz((int)used1)) : 31 - (uint32_t)__clz((int)used0);
     if (nused == 1) {                                        // RLE_Mode: one byte, states carry no bits
-        if (lane == 0) desc[0] = (uint8_t)max_sym;
-        kind->mode = 1; kind->log = 0;
-        return 1;
+        if (lane == 0 && desc) desc[0] = (uint8_t)max_sym;
+        return 1u | 1u << 8 | max_sym << 16;
     }
     if (allow_predefined && N < ZE_PREDEF_BELOW) {           // Predefined_Mode
         const uint32_t size = 1u << default_log;
         for (uint32_t i = lane; i < size; i += 32) st[i] = pre_state[i];
         for (uint32_t i = lane; i < alphabet; i += 32) sy[i] = pre_sym[i];
-        kind->mode = 0; kind->log = default_log;
         __syncwarp();
-        return 0;
+        return default_log << 12 | max_sym << 16;
     }
     // ---- FSE_Compressed_Mode.  Table log as FSE_optimalTableLog picks it.
     uint32_t log = max_log;
@@ -162,11 +166,12 @@ __device__ TS_NOINLINE uint32_t ze_build_kind(uint32_t* cnt, uint32_t alphabet, 
         __syncwarp();
     }
     uint32_t bytes = 0;
-    if (lane == 0) bytes = ze_write_ncount(desc, cnt, max_sym + 1, log);
-    bytes = __shfl_sync(TS_FULL, bytes, 0);
-    kind->mode = 2; kind->log = log;
+    if (desc) {
+        if (lane == 0) bytes = ze_write_ncount(desc, cnt, max_sym + 1, log);
+        bytes = __shfl_sync(TS_FULL, bytes, 0);
+    }
     __syncwarp();
-    return bytes;
+    return bytes | 2u << 8 | log << 12 | max_sym << 16;
 }
 
 }  // namespace ts

@@ -190,9 +190,10 @@ __device__ __forceinline__ uint32_t ze_huf_tree_desc(const uint32_t* ctab, uint3
     __syncwarp();
     uint32_t tree_bytes = nweights <= 128 ? 1 + (nweights + 1) / 2 : ZE_NO_TREE;
     if (nweights >= 2 && (ZE_FSE_WEIGHTS_ALWAYS || nweights > 128)) {
-        ZeKind wk;
-        const uint32_t dsz = ze_build_kind(wcnt, 13, nweights, zf::HUFW_MAX_LOG, zf::HUFW_MAX_LOG, nullptr, nullptr, wst, wsy,
-                                           wscratch, desc + 1, &wk, false, lane);
+        const uint32_t wr = ze_build_kind(wcnt, 13, nweights, zf::HUFW_MAX_LOG, zf::HUFW_MAX_LOG, nullptr, nullptr, wst, wsy,
+                                          wscratch, desc + 1, false, lane);
+        const uint32_t dsz = ze_kind_bytes(wr);
+        const ZeKind wk = ze_kind_of(wr);
         if (wk.mode == 2) {
             uint32_t fsz = 0;
             if (lane == 0) {                                              // two interleaved states, last weight first
