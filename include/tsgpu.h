@@ -376,6 +376,59 @@ int tsgpu_rewrite_object_crc64(tsgpu_ctx* ctx,
                                uint64_t* source_crc64, uint64_t* object_crc64, uint64_t* segment_crc64);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * tsgpu_rekey_object — the AES-GCM chunks of a stored object re-encrypted under a new data key with nothing decoded: for replacing
+ * an exposed key.  Each chunk (IV || CT || TAG) is read once; one GPU pass computes CT ^ E_old(ctr) ^ E_new(ctr), checks the old
+ * tag and writes the new IV and tag.  The plaintext exists only in registers.  The call serves both objects of an encrypted
+ * segment: the .log object (its chunks by the chunk index) and the .indexes object (its blobs at their SegmentIndexesV1 positions
+ * and sizes).  Sizes do not change, so the chunk index and SegmentIndexesV1 stay as they are and only the manifest's encryption
+ * metadata changes.  Unlike tsgpu_rewrite_object this proves only that every chunk is authentic under the old key: nothing checks
+ * that the object decodes to a valid segment.
+ *
+ *   flags          TSGPU_FLAG_VERIFY only; any other bit fails with TSGPU_E_ARG.  TSGPU_VERIFY=1 turns VERIFY on.  With VERIFY every
+ *                  batch is decrypted again by the separate decrypt kernels, the source under the old key and the output under
+ *                  the new one, and the two plaintexts are compared on the GPU before any byte of the batch is released; a
+ *                  difference fails with TSGPU_E_VERIFY naming the chunk and the first differing byte.
+ *   src, src_len, transformed_sizes, n_chunks   the window's chunks back to back.  A chunk of 0 bytes passes through as 0 bytes
+ *                  (an empty index blob, the empty segment's one chunk) and takes no IV; a chunk of 1 to 27 bytes fails its tag
+ *                  (TSGPU_E_AUTH); a chunk larger than the context's transformed slot (what tsgpu_detransform takes) fails with
+ *                  TSGPU_E_ARG before any GPU work.
+ *   from_key, from_aad   the old data key and AAD; to_key, to_aad, to_ivs   the new ones and one 12-byte IV per chunk.  The IV
+ *                  rules and messages are those of tsgpu_rewrite_object: no two non-empty chunks of the window may get the same
+ *                  IV, and when to_key equals from_key no new IV may equal a source chunk's IV (TSGPU_E_ARG, before any GPU work).
+ *   dst, dst_cap   receive exactly sum(transformed_sizes) bytes: chunk i keeps its size and gets to_ivs[i].  A smaller dst_cap
+ *                  fails with TSGPU_E_SHORT before any GPU work.
+ *   part_size, part_crc32c, part_cap, n_parts   as tsgpu_transform_parts, with an exact bound: part_cap >= floor((carried +
+ *                  sum(transformed_sizes)) / part_size) + (object_ends_here ? 1 : 0); a smaller part_cap fails with TSGPU_E_SHORT
+ *                  before any GPU work.
+ *   cursor         64 bytes, zeroed at the start of the object, passed to every window in order: the parts cursor, the source
+ *                  object's running CRC and length, and the chunk count (messages name a chunk by its number in the object).
+ *                  Updated on success, without a defined value after a failure.
+ *   object_ends_here  != 0 on the last window (which may be empty): then *source_crc32c is the CRC-32C of the old object and
+ *                  *object_crc32c that of the new object (FULL_OBJECT).  Neither is written before the end or on failure.
+ * Returns the first failure in object order; within a batch: the first bad tag (TSGPU_E_AUTH, "Tag mismatch in chunk <k>"), then
+ * VERIFY (TSGPU_E_VERIFY).  No byte of a failing batch reaches dst; earlier batches may already be there.  A failed call writes no
+ * CRC.  Buffers and cost: DESIGN.md §3, §4.1, §8.
+ * --------------------------------------------------------------------------------------------------------- */
+typedef struct tsgpu_rekey_cursor { uint64_t opaque[8]; } tsgpu_rekey_cursor;
+int tsgpu_rekey_object(tsgpu_ctx* ctx, uint32_t flags,
+                       const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes, uint32_t n_chunks,
+                       const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                       const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len, const uint8_t* to_ivs,
+                       uint8_t* dst, uint64_t dst_cap,
+                       uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
+                       tsgpu_rekey_cursor* cursor, int object_ends_here,
+                       uint32_t* source_crc32c, uint32_t* object_crc32c);
+/* The CRC-64/NVME twin: the same arguments, rules, errors and output bytes, with 64-bit part, source and object words. */
+int tsgpu_rekey_object_crc64(tsgpu_ctx* ctx, uint32_t flags,
+                             const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes, uint32_t n_chunks,
+                             const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                             const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len, const uint8_t* to_ivs,
+                             uint8_t* dst, uint64_t dst_cap,
+                             uint64_t part_size, uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts,
+                             tsgpu_rekey_cursor* cursor, int object_ends_here,
+                             uint64_t* source_crc64, uint64_t* object_crc64);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Device-resident variants (inputs and outputs already in HBM of device `device_index` of the context; used by
  * bench.py for the kernel-side throughput and by callers that keep segments on the GPU).  Layouts:
  *   original side     contiguous, chunk i at i * chunk_size

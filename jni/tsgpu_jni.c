@@ -3,7 +3,7 @@
  * There is no JDK in this repository's build image: the tests compile this file against a test-only stand-in for
  * <jni.h> and drive it through a fake JNIEnv (tests/cpp/test_jni_shim.c).  Build on the broker host with
  *   gcc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude jni/tsgpu_jni.c -L<pkg> -ltsgpu -o libtsgpu_jni.so
- * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,RewriteCursor,Crc64,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
+ * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,RewriteCursor,RekeyCursor,Crc64,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
  * (implement TransformChunkEnumeration / DetransformChunkEnumeration of the reference, core/M/transform/TransformChunkEnumeration.java:28-42,
  * DetransformChunkEnumeration.java:28-29) and jni/io/aiven/kafka/tieredstorage/fetch/gpu/GpuChunkManager.java (ChunkManager, fetch/ChunkManager.java).
  *
@@ -441,4 +441,113 @@ JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_Crc64_rew
     np[0] = (jint)nParts;
     (*env)->ReleaseIntArrayElements(env, nPartsOut, np, 0);
     if (objectEndsHere) { out[0] = crcs[0]; out[1] = crcs[1]; out[2] = crcs[2]; }
+}
+
+/* ---------------------------------------------------------------------------------------------------------------------------
+ * Key rotation (RekeyCursor.java): one window of a stored object's AES-GCM chunks re-encrypted under a new key with nothing
+ * decoded (tsgpu_rekey_object[_crc64]).  `cursor` a direct ByteBuffer of at least 64 bytes holding the tsgpu_rekey_cursor (zeros
+ * at the start of the object), updated in place; dst a direct ByteBuffer receiving exactly the window's bytes (every chunk keeps
+ * its size); toIvs 12 bytes per chunk of the window (an empty chunk takes none, its 12 bytes are not read). */
+
+/* The arguments both widths check the same way; the key, AAD and IV arrays pinned.  Returns -1 with an exception pending. */
+typedef struct {
+    uint8_t* s; uint8_t* d; tsgpu_rekey_cursor* cur; uint32_t n;
+    jint* ts; jbyte* fk; jbyte* fa; jint falen; jbyte* tk; jbyte* ta; jint talen; jbyte* iv;
+} rekey_args;
+static int rekey_begin(JNIEnv* env, jobject src, jlong srcLen, jintArray transformedSizes, jbyteArray fromKey, jbyteArray fromAad,
+                       jbyteArray toKey, jbyteArray toAad, jbyteArray toIvs, jobject dst, jlong dstCap, jlong partSize,
+                       jintArray nPartsOut, jobject cursor, rekey_args* r) {
+    jlong ccap = 0;
+    r->s = srcLen ? direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer") : NULL;
+    if (srcLen && !r->s) return -1;
+    r->d = dstCap ? direct(env, dst, dstCap, NULL, "dst must be a direct ByteBuffer") : NULL;
+    if (dstCap && !r->d) return -1;
+    r->cur = (tsgpu_rekey_cursor*)direct(env, cursor, 0, &ccap, "rekey cursor must be a direct ByteBuffer of 64 bytes");
+    if (!r->cur) return -1;
+    if (ccap < (jlong)sizeof(tsgpu_rekey_cursor)) { throw_arg(env, "rekey cursor must be a direct ByteBuffer of 64 bytes"); return -1; }
+    if (!transformedSizes) { throw_arg(env, "chunks cannot be null"); return -1; }
+    r->n = (uint32_t)(*env)->GetArrayLength(env, transformedSizes);
+    if (!nPartsOut || (*env)->GetArrayLength(env, nPartsOut) < 1) { throw_arg(env, "nPartsOut must hold 1 int"); return -1; }
+    if (partSize < 1) { throw_arg(env, "partSize must be positive"); return -1; }
+    if ((fromKey && (*env)->GetArrayLength(env, fromKey) != 32) || (toKey && (*env)->GetArrayLength(env, toKey) != 32)) {
+        throw_arg(env, "data key must be 32 bytes"); return -1;
+    }
+    if (toIvs && (uint32_t)(*env)->GetArrayLength(env, toIvs) < 12 * r->n) { throw_arg(env, "toIvs must hold 12 bytes per chunk"); return -1; }
+    r->fk = fromKey ? (*env)->GetByteArrayElements(env, fromKey, NULL) : NULL;
+    r->fa = fromAad ? (*env)->GetByteArrayElements(env, fromAad, NULL) : NULL;
+    r->falen = fromAad ? (*env)->GetArrayLength(env, fromAad) : 0;
+    r->tk = toKey ? (*env)->GetByteArrayElements(env, toKey, NULL) : NULL;
+    r->ta = toAad ? (*env)->GetByteArrayElements(env, toAad, NULL) : NULL;
+    r->talen = toAad ? (*env)->GetArrayLength(env, toAad) : 0;
+    r->iv = toIvs ? (*env)->GetByteArrayElements(env, toIvs, NULL) : NULL;
+    r->ts = (*env)->GetIntArrayElements(env, transformedSizes, NULL);
+    return 0;
+}
+/* Releases what rekey_begin pinned; on success nPartsOut[0] receives the count of completed parts. */
+static void rekey_end(JNIEnv* env, jintArray transformedSizes, jbyteArray fromKey, jbyteArray fromAad, jbyteArray toKey,
+                      jbyteArray toAad, jbyteArray toIvs, jintArray nPartsOut, rekey_args* r, int rc, uint32_t nParts) {
+    (*env)->ReleaseIntArrayElements(env, transformedSizes, r->ts, JNI_ABORT);
+    if (r->fk) (*env)->ReleaseByteArrayElements(env, fromKey, r->fk, JNI_ABORT);
+    if (r->fa) (*env)->ReleaseByteArrayElements(env, fromAad, r->fa, JNI_ABORT);
+    if (r->tk) (*env)->ReleaseByteArrayElements(env, toKey, r->tk, JNI_ABORT);
+    if (r->ta) (*env)->ReleaseByteArrayElements(env, toAad, r->ta, JNI_ABORT);
+    if (r->iv) (*env)->ReleaseByteArrayElements(env, toIvs, r->iv, JNI_ABORT);
+    if (rc) { throw_rt(env, rc); return; }
+    jint* np = (*env)->GetIntArrayElements(env, nPartsOut, NULL);
+    np[0] = (jint)nParts;
+    (*env)->ReleaseIntArrayElements(env, nPartsOut, np, 0);
+}
+
+/* RekeyCursor.rekeyObject: partCrcs (int[], its length is part_cap) receives the CRC-32C of the upload parts the window completes;
+ * crcsOut (int[2]) receives, on the object's last window, the CRC-32C of the old object and of the new object. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RekeyCursor_rekeyObject(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray transformedSizes, jbyteArray fromKey,
+    jbyteArray fromAad, jbyteArray toKey, jbyteArray toAad, jbyteArray toIvs, jobject dst, jlong dstCap, jlong partSize,
+    jintArray partCrcs, jintArray nPartsOut, jobject cursor, jboolean objectEndsHere, jintArray crcsOut) {
+    if (!partCrcs) { throw_arg(env, "partCrcs cannot be null"); return; }
+    if (!crcsOut || (*env)->GetArrayLength(env, crcsOut) < 2) { throw_arg(env, "crcsOut must hold 2 ints"); return; }
+    rekey_args r;
+    if (rekey_begin(env, src, srcLen, transformedSizes, fromKey, fromAad, toKey, toAad, toIvs, dst, dstCap, partSize, nPartsOut,
+                    cursor, &r)) return;
+    const uint32_t cap = (uint32_t)(*env)->GetArrayLength(env, partCrcs);
+    jint* pc = (*env)->GetIntArrayElements(env, partCrcs, NULL);
+    uint32_t nParts = 0, crcs[2] = {0, 0};
+    int rc = tsgpu_rekey_object((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, r.s, (uint64_t)srcLen, (const uint32_t*)r.ts, r.n,
+                                (const uint8_t*)r.fk, (const uint8_t*)r.fa, (uint32_t)r.falen, (const uint8_t*)r.tk, (const uint8_t*)r.ta,
+                                (uint32_t)r.talen, (const uint8_t*)r.iv, r.d, (uint64_t)dstCap, (uint64_t)partSize, (uint32_t*)pc, cap,
+                                &nParts, r.cur, objectEndsHere ? 1 : 0, &crcs[0], &crcs[1]);
+    (*env)->ReleaseIntArrayElements(env, partCrcs, pc, rc ? JNI_ABORT : 0);
+    rekey_end(env, transformedSizes, fromKey, fromAad, toKey, toAad, toIvs, nPartsOut, &r, rc, nParts);
+    if (!rc && objectEndsHere) {
+        jint* out = (*env)->GetIntArrayElements(env, crcsOut, NULL);
+        out[0] = (jint)crcs[0]; out[1] = (jint)crcs[1];
+        (*env)->ReleaseIntArrayElements(env, crcsOut, out, 0);
+    }
+}
+
+/* RekeyCursor.rekeyObjectCrc64: rekeyObject with CRC-64/NVME.  partCrc64 (direct, 8 bytes per part: its capacity / 8 is
+ * part_cap) receives the CRCs of the upload parts the window completes; crcsOut (direct, 16 bytes) receives, on the object's last
+ * window, the CRC-64/NVME of the old object and of the new object. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RekeyCursor_rekeyObjectCrc64(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray transformedSizes, jbyteArray fromKey,
+    jbyteArray fromAad, jbyteArray toKey, jbyteArray toAad, jbyteArray toIvs, jobject dst, jlong dstCap, jlong partSize,
+    jobject partCrc64, jintArray nPartsOut, jobject cursor, jboolean objectEndsHere, jobject crcsOut) {
+    jlong pcap = 0, wcap = 0;
+    uint64_t* pc = (uint64_t*)direct(env, partCrc64, 0, &pcap, "partCrc64 must be a direct ByteBuffer");
+    if (!pc) return;
+    uint64_t* out = (uint64_t*)direct(env, crcsOut, 0, &wcap, "crcsOut must be a direct ByteBuffer of 16 bytes");
+    if (!out) return;
+    if (wcap < 16) { throw_arg(env, "crcsOut must be a direct ByteBuffer of 16 bytes"); return; }
+    rekey_args r;
+    if (rekey_begin(env, src, srcLen, transformedSizes, fromKey, fromAad, toKey, toAad, toIvs, dst, dstCap, partSize, nPartsOut,
+                    cursor, &r)) return;
+    uint32_t nParts = 0;
+    uint64_t crcs[2] = {0, 0};
+    int rc = tsgpu_rekey_object_crc64((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, r.s, (uint64_t)srcLen, (const uint32_t*)r.ts, r.n,
+                                      (const uint8_t*)r.fk, (const uint8_t*)r.fa, (uint32_t)r.falen, (const uint8_t*)r.tk,
+                                      (const uint8_t*)r.ta, (uint32_t)r.talen, (const uint8_t*)r.iv, r.d, (uint64_t)dstCap,
+                                      (uint64_t)partSize, pc, (uint32_t)(pcap / 8), &nParts, r.cur, objectEndsHere ? 1 : 0, &crcs[0],
+                                      &crcs[1]);
+    rekey_end(env, transformedSizes, fromKey, fromAad, toKey, toAad, toIvs, nPartsOut, &r, rc, nParts);
+    if (!rc && objectEndsHere) { out[0] = crcs[0]; out[1] = crcs[1]; }
 }

@@ -28,6 +28,7 @@ CURSOR_SIZE = 64         # tsgpu_records_cursor
 PARTS_CURSOR_SIZE = 32   # tsgpu_parts_cursor
 CHECK_CURSOR_SIZE = 128  # tsgpu_check_cursor
 REWRITE_CURSOR_SIZE = 192  # tsgpu_rewrite_cursor
+REKEY_CURSOR_SIZE = 64   # tsgpu_rekey_cursor
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",
@@ -38,6 +39,7 @@ SYMBOLS = [
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
     "tsgpu_transform_cursor", "tsgpu_transform_parts", "tsgpu_check_object", "tsgpu_rewrite_object",
     "tsgpu_transform_parts_crc64", "tsgpu_check_object_crc64", "tsgpu_rewrite_object_crc64",
+    "tsgpu_rekey_object", "tsgpu_rekey_object_crc64",
 ]
 
 
@@ -84,6 +86,9 @@ def load(path=None):
     L.tsgpu_transform_parts_crc64.argtypes = L.tsgpu_transform_parts.argtypes
     L.tsgpu_check_object_crc64.argtypes = L.tsgpu_check_object.argtypes
     L.tsgpu_rewrite_object_crc64.argtypes = L.tsgpu_rewrite_object.argtypes
+    L.tsgpu_rekey_object.argtypes = [vp, u32, vp, u64, vp, u32, vp, vp, u32, vp, vp, u32, vp, vp, u64, u64, vp, u32, vp, vp,
+                                     C.c_int, vp, vp]
+    L.tsgpu_rekey_object_crc64.argtypes = L.tsgpu_rekey_object.argtypes
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
     L.tsgpu_detransform_device.argtypes = [vp, C.c_int, u32, vp, u64, vp, u32, u32, vp, vp, u32, vp, vp, vp, vp]
     L.tsgpu_launch_count.restype = u64
@@ -355,6 +360,45 @@ class Context:
         sizes = sizes[:n]
         crc3 = (int(src_crc.value), int(obj_crc.value), int(seg_crc.value)) if object_ends_here else None
         return dst[:int(sizes.sum(dtype=np.uint64))], [int(x) for x in sizes], [int(x) for x in crcs[:n_parts.value]], crc3
+
+    def rekey_object(self, src, transformed_sizes, from_key, to_key, to_ivs, part_size, from_aad=b"", to_aad=b"", flags=0,
+                     cursor=None, object_ends_here=True, part_cap=None, dst_cap=None):
+        """Re-encrypts one window of a stored object's AES-GCM chunks under a new key with nothing decoded (tsgpu_rekey_object):
+        chunk i keeps its size and gets to_ivs[i].  `flags`: 0 or FLAG_VERIFY.  `cursor`: a 64-byte np.uint8 array (zeros at
+        the start of the object), updated in place on success; None rekeys a whole object.  Returns (new bytes, [CRC-32C of the
+        parts this call completed], (source, object) CRC-32C or None when the object does not end here)."""
+        return self._rekey_object(self.lib.tsgpu_rekey_object, C.c_uint32, src, transformed_sizes, from_key, to_key, to_ivs,
+                                  part_size, from_aad, to_aad, flags, cursor, object_ends_here, part_cap, dst_cap)
+
+    def rekey_object_crc64(self, src, transformed_sizes, from_key, to_key, to_ivs, part_size, from_aad=b"", to_aad=b"", flags=0,
+                           cursor=None, object_ends_here=True, part_cap=None, dst_cap=None):
+        """rekey_object with CRC-64/NVME part, source and object checksums (tsgpu_rekey_object_crc64): the same new bytes.  A
+        cursor carries one width: start and continue it with the same method."""
+        return self._rekey_object(self.lib.tsgpu_rekey_object_crc64, C.c_uint64, src, transformed_sizes, from_key, to_key,
+                                  to_ivs, part_size, from_aad, to_aad, flags, cursor, object_ends_here, part_cap, dst_cap)
+
+    def _rekey_object(self, fn, word, src, transformed_sizes, from_key, to_key, to_ivs, part_size, from_aad, to_aad, flags,
+                      cursor, object_ends_here, part_cap, dst_cap):
+        s = _u8(src)
+        if cursor is None:
+            cursor = np.zeros(REKEY_CURSOR_SIZE, np.uint8)
+        if not (isinstance(cursor, np.ndarray) and cursor.dtype == np.uint8 and cursor.size == REKEY_CURSOR_SIZE
+                and cursor.flags.c_contiguous):
+            raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % REKEY_CURSOR_SIZE)
+        ts = np.ascontiguousarray(transformed_sizes, dtype=np.uint32)
+        total = int(ts.sum(dtype=np.uint64))
+        dst = np.empty(total if dst_cap is None else dst_cap, dtype=np.uint8)
+        if part_cap is None:                                 # the exact bound: (carried + window) // part_size, + 1 at the end
+            part_cap = (int(np.frombuffer(cursor[:8].tobytes(), np.uint64)[0]) % max(part_size, 1) + total) // max(part_size, 1) + 1
+        crcs = np.zeros(max(part_cap, 1), dtype=_np_word(word))
+        n_parts, src_crc, obj_crc = C.c_uint32(0), word(0), word(0)
+        fk, fa, tk, ta, iv = _u8(from_key), _u8(from_aad), _u8(to_key), _u8(to_aad), _u8(to_ivs)
+        self._check(fn(
+            self._h, flags, _p(s), s.size, _p(ts), ts.size, _p(fk), _p(fa), fa.size, _p(tk), _p(ta), ta.size, _p(iv),
+            _p(dst), dst.size, part_size, _p(crcs), part_cap, C.addressof(n_parts), cursor.ctypes.data,
+            1 if object_ends_here else 0, C.addressof(src_crc), C.addressof(obj_crc)))
+        crc2 = (int(src_crc.value), int(obj_crc.value)) if object_ends_here else None
+        return dst[:total], [int(x) for x in crcs[:n_parts.value]], crc2
 
     # ---- device-resident API (raw device pointers as ints; bench.py passes torch data_ptr()) ----
     def slot_stride(self, flags, chunk_size):

@@ -15,6 +15,10 @@
 //                          shared-memory table; emits one 16-byte partial per range
 //   gcm_finalize_kernel    one warp per chunk: combines the range partials with H-powers, adds AAD and the
 //                          length block, computes/verifies the tag, writes IV and TAG, sizes and status
+//   gcm_rekey_kernel       the main kernel's grid over IV||CT||TAG chunks, re-encrypted in place under a second key: per block
+//                          ct_new = ct_old ^ E_old(ctr) ^ E_new(ctr), ct_old folded into the old GHASH and ct_new into the new
+//                          one (one H^256 table per key in shared memory); two partials per range
+//   gcm_rekey_finalize_kernel  one warp per chunk: checks the old tag, writes the new IV and tag and the status
 // Integer/byte arithmetic only; no tensor cores (nothing here is a dense contraction).
 #pragma once
 #include "ts_common.cuh"
@@ -32,6 +36,7 @@ constexpr uint32_t GCM_IV = 12, GCM_TAG = 16;
 constexpr uint32_t GCM_SMEM_TE = 256 * 64 * 4;   // 64 KiB
 constexpr uint32_t GCM_SMEM_HTAB = 16 * 256 * 16;  // 64 KiB
 constexpr uint32_t GCM_SMEM_BYTES = GCM_SMEM_TE + GCM_SMEM_HTAB;
+constexpr uint32_t GCM_REKEY_SMEM_BYTES = GCM_SMEM_TE + 2 * GCM_SMEM_HTAB;   // 192 KiB: one CTA per SM, as gcm_main_kernel
 
 struct GcmKeyCtx {
     uint4 hsq[GH_NSQ];            // hsq[k] = H^(2^k)
@@ -210,6 +215,96 @@ __device__ __forceinline__ uint32_t ld_le32_bytes(const uint8_t* p) {
     return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
 }
 
+// ------------------------------------------------------------------------------------------ shared kernel pieces
+// gcm_main_kernel / gcm_finalize_kernel and the rekey kernels share these pieces as macros, not functions: the compiler optimizes
+// a function on its own before it inlines it, which reorders the instructions of its callers.  As text the pieces leave
+// gcm_main_kernel and gcm_finalize_kernel compiling to the SASS they had before the rekey kernels shared them.
+
+// The lane-replicated round tables into the first GCM_SMEM_TE bytes of shared memory.
+#define GCM_FILL_TE(smem, tid)                                                                                                 \
+    for (uint32_t i = tid; i < 256 * 64; i += GH_T) {                                                                          \
+        const uint32_t t0 = g_aes_tables.te0[i >> 6];                                                                          \
+        ((uint32_t*)smem)[i] = (i & 32) ? __byte_perm(t0, 0, 0x1032) : t0;       /* second half of a row: Te2 = rotl16(Te0) */ \
+    }
+
+// Block `off` (a multiple of 16) of an n-byte run: declares d = its bytes at src + off, the pad zeroed (one 128-bit load when the
+// run is aligned and the block full), and o = d ^ (k0, k1, k2, k3), stored at dst + off (only the bytes inside the run) and left
+// with its pad zeroed, as GHASH takes it.
+#define GCM_XOR_BLOCK(src, dst, off, n, aligned, full, k0, k1, k2, k3, d, o)                                                   \
+    uint4 d;                                                                                                                   \
+    if (aligned && full) {                                                                                                     \
+        d = ldg128_stream((const uint4*)(src + off));                                                                          \
+    } else {                                                                                                                   \
+        uint32_t w[4] = {0, 0, 0, 0};                                                                                          \
+        uint32_t k = full ? 16 : n - (uint32_t)off;                                                                            \
+        for (uint32_t q = 0; q < k; q++) w[q >> 2] |= (uint32_t)src[off + q] << (8 * (q & 3));                                 \
+        d = make_uint4(w[0], w[1], w[2], w[3]);                                                                                \
+    }                                                                                                                          \
+    uint4 o = make_uint4(d.x ^ k0, d.y ^ k1, d.z ^ k2, d.w ^ k3);                                                              \
+    if (aligned && full) {                                                                                                     \
+        stg128_stream((uint4*)(dst + off), o);                                                                                 \
+    } else {                                                                                                                   \
+        uint32_t w[4] = { o.x, o.y, o.z, o.w };                                                                                \
+        uint32_t k = full ? 16 : n - (uint32_t)off;                                                                            \
+        for (uint32_t q = 0; q < k; q++) dst[off + q] = (uint8_t)(w[q >> 2] >> (8 * (q & 3)));                                 \
+        if (!full) {                                  /* zero the pad bytes of the ciphertext block for GHASH */               \
+            for (uint32_t q = k; q < 16; q++) w[q >> 2] &= ~(0xffu << (8 * (q & 3)));                                          \
+            o = make_uint4(w[0], w[1], w[2], w[3]);                                                                            \
+        }                                                                                                                      \
+    }
+
+// A lane's GHASH accumulator `acc` (last block `last`, 0xffffffff if none) aligned to the range end b1 and XOR-reduced over the
+// CTA through `red` (GH_T / 32 entries, one __syncthreads); thread 0 stores the range's partial to `partial`.
+#define GCM_RANGE_PARTIAL(kc, acc, last, b1, red, tid, partial)                                                                \
+    if (last != 0xffffffffu) acc = gf_mul(acc, kc->hpow[b1 - last]);   /* align the lane to the range end */                   \
+                                                                                                                               \
+    /* XOR-reduce the 256 lanes */                                                                                             \
+    for (int o = 16; o; o >>= 1) {                                                                                             \
+        acc.x ^= __shfl_xor_sync(TS_FULL, acc.x, o); acc.y ^= __shfl_xor_sync(TS_FULL, acc.y, o);                              \
+        acc.z ^= __shfl_xor_sync(TS_FULL, acc.z, o); acc.w ^= __shfl_xor_sync(TS_FULL, acc.w, o);                              \
+    }                                                                                                                          \
+    if ((tid & 31) == 0) red[tid >> 5] = acc;                                                                                  \
+    __syncthreads();                                                                                                           \
+    if (tid == 0) {                                                                                                            \
+        uint4 p = red[0];                                                                                                      \
+        for (int w = 1; w < GH_T / 32; w++) p = xor4(p, red[w]);                                                               \
+        partial = p;                                                                                                           \
+    }
+
+// Declares `term`: the GHASH of an m-block chunk before its length block, summed over the warp -- its nr range partials
+// P_r * H^(m - end_r) (at partials[chunk * max_ranges + r]) and the AAD's X_A * H^(m+1).
+#define GCM_HASH_TERMS(kc, partials, max_ranges, chunk, m, nr, aad, aad_len, lane, term)                                       \
+    uint4 term = make_uint4(0, 0, 0, 0);                                                                                       \
+    for (uint32_t r = lane; r < nr; r += 32) {             /* P_r * H^(m - end_r) */                                           \
+        uint32_t end_r = min((r + 1) * GH_RANGE_BLOCKS, m);                                                                    \
+        uint4 p = partials[(size_t)chunk * max_ranges + r];                                                                    \
+        uint32_t e = m - end_r;                                                                                                \
+        term = xor4(term, e ? gf_mul(p, gf_pow(kc, e)) : p);                                                                   \
+    }                                                                                                                          \
+    if (lane == 31 && aad_len) {                           /* X_A * H^(m+1) */                                                 \
+        uint4 x = make_uint4(0, 0, 0, 0);                                                                                      \
+        const uint4 H = kc->hpow[1];                                                                                           \
+        for (uint32_t off = 0; off < aad_len; off += 16) {                                                                     \
+            uint32_t w[4] = {0, 0, 0, 0};                                                                                      \
+            uint32_t k = min(16u, aad_len - off);                                                                              \
+            for (uint32_t q = 0; q < k; q++) w[q >> 2] |= (uint32_t)aad[off + q] << (8 * (q & 3));                             \
+            x = off ? gf_mul(x, H) : x;                                                                                        \
+            x = xor4(x, make_uint4(w[0], w[1], w[2], w[3]));                                                                   \
+        }                                                                                                                      \
+        term = xor4(term, gf_mul(x, gf_pow(kc, m + 1)));                                                                       \
+    }                                                                                                                          \
+    for (int o = 16; o; o >>= 1) {                                                                                             \
+        term.x ^= __shfl_xor_sync(TS_FULL, term.x, o); term.y ^= __shfl_xor_sync(TS_FULL, term.y, o);                          \
+        term.z ^= __shfl_xor_sync(TS_FULL, term.z, o); term.w ^= __shfl_xor_sync(TS_FULL, term.w, o);                          \
+    }
+
+// Declares S = (term ^ length block) * H for an n-byte ciphertext: the tag is S ^ E_K(J0).
+#define GCM_TAG_S(kc, term, aad_len, n, S)                                                                                     \
+    const uint64_t abits = (uint64_t)aad_len * 8, cbits = (uint64_t)n * 8;                                                     \
+    uint4 L = make_uint4(bswap32((uint32_t)(abits >> 32)), bswap32((uint32_t)abits),                                           \
+                         bswap32((uint32_t)(cbits >> 32)), bswap32((uint32_t)cbits));                                          \
+    uint4 S = gf_mul(xor4(term, L), kc->hpow[1]);
+
 // ------------------------------------------------------------------------------------------ main kernel
 template <bool ENC>
 __global__ void __launch_bounds__(GH_T, 1)
@@ -238,10 +333,7 @@ gcm_main_kernel(const __grid_constant__ Aes256RoundKeys rk, const GcmKeyCtx* __r
     if (tid == 0) mbar_init(&bar, 1);
     uint64_t* barp = &bar;
 #endif
-    for (uint32_t i = tid; i < 256 * 64; i += GH_T) {
-        const uint32_t t0 = g_aes_tables.te0[i >> 6];
-        ((uint32_t*)smem)[i] = (i & 32) ? __byte_perm(t0, 0, 0x1032) : t0;       // second half of a row: Te2 = rotl16(Te0)
-    }
+    GCM_FILL_TE(smem, tid)
     __syncthreads();
     block_bulk_load(htab, kc->htab, GCM_SMEM_HTAB, barp, 0);   // TMA bulk copy of the H^256 table
     __syncthreads();
@@ -262,45 +354,12 @@ gcm_main_kernel(const __grid_constant__ Aes256RoundKeys rk, const GcmKeyCtx* __r
         aes256_encrypt_te(rk, te, off0, off2, s0, s1, s2, s3);
         const size_t off = (size_t)i << 4;
         const bool full = off + 16 <= n;
-        uint4 d;
-        if (aligned && full) {
-            d = ldg128_stream((const uint4*)(src + off));
-        } else {
-            uint32_t w[4] = {0, 0, 0, 0};
-            uint32_t k = full ? 16 : n - (uint32_t)off;
-            for (uint32_t q = 0; q < k; q++) w[q >> 2] |= (uint32_t)src[off + q] << (8 * (q & 3));
-            d = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-        uint4 o = make_uint4(d.x ^ s0, d.y ^ s1, d.z ^ s2, d.w ^ s3);
-        if (aligned && full) {
-            stg128_stream((uint4*)(dst + off), o);
-        } else {
-            uint32_t w[4] = { o.x, o.y, o.z, o.w };
-            uint32_t k = full ? 16 : n - (uint32_t)off;
-            for (uint32_t q = 0; q < k; q++) dst[off + q] = (uint8_t)(w[q >> 2] >> (8 * (q & 3)));
-            if (!full) {                                  // zero the pad bytes of the ciphertext block for GHASH
-                for (uint32_t q = k; q < 16; q++) w[q >> 2] &= ~(0xffu << (8 * (q & 3)));
-                o = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-        }
+        GCM_XOR_BLOCK(src, dst, off, n, aligned, full, s0, s1, s2, s3, d, o)
         const uint4 ct = ENC ? o : d;                     // (DEC: d was zero padded on load)
         acc = xor4(gf_mul_tab(htab, acc), ct);
         last = i;
     }
-    if (last != 0xffffffffu) acc = gf_mul(acc, kc->hpow[b1 - last]);   // align the lane to the range end
-
-    // XOR-reduce the 256 lanes
-    for (int o = 16; o; o >>= 1) {
-        acc.x ^= __shfl_xor_sync(TS_FULL, acc.x, o); acc.y ^= __shfl_xor_sync(TS_FULL, acc.y, o);
-        acc.z ^= __shfl_xor_sync(TS_FULL, acc.z, o); acc.w ^= __shfl_xor_sync(TS_FULL, acc.w, o);
-    }
-    if ((tid & 31) == 0) red[tid >> 5] = acc;
-    __syncthreads();
-    if (tid == 0) {
-        uint4 p = red[0];
-        for (int w = 1; w < GH_T / 32; w++) p = xor4(p, red[w]);
-        B.partials[(size_t)chunk * B.max_ranges + range] = p;
-    }
+    GCM_RANGE_PARTIAL(kc, acc, last, b1, red, tid, B.partials[(size_t)chunk * B.max_ranges + range])
 }
 
 // ------------------------------------------------------------------------------------------ finalize
@@ -319,34 +378,9 @@ gcm_finalize_kernel(const __grid_constant__ Aes256RoundKeys rk, const GcmKeyCtx*
     const uint8_t* in = B.in_base + B.in_off[chunk];
     uint8_t* out = B.out_base + B.out_off[chunk];
 
-    uint4 term = make_uint4(0, 0, 0, 0);
-    for (uint32_t r = lane; r < nr; r += 32) {             // P_r * H^(m - end_r)
-        uint32_t end_r = min((r + 1) * GH_RANGE_BLOCKS, m);
-        uint4 p = B.partials[(size_t)chunk * B.max_ranges + r];
-        uint32_t e = m - end_r;
-        term = xor4(term, e ? gf_mul(p, gf_pow(kc, e)) : p);
-    }
-    if (lane == 31 && B.aad_len) {                         // X_A * H^(m+1)
-        uint4 x = make_uint4(0, 0, 0, 0);
-        const uint4 H = kc->hpow[1];
-        for (uint32_t off = 0; off < B.aad_len; off += 16) {
-            uint32_t w[4] = {0, 0, 0, 0};
-            uint32_t k = min(16u, B.aad_len - off);
-            for (uint32_t q = 0; q < k; q++) w[q >> 2] |= (uint32_t)B.aad[off + q] << (8 * (q & 3));
-            x = off ? gf_mul(x, H) : x;
-            x = xor4(x, make_uint4(w[0], w[1], w[2], w[3]));
-        }
-        term = xor4(term, gf_mul(x, gf_pow(kc, m + 1)));
-    }
-    for (int o = 16; o; o >>= 1) {
-        term.x ^= __shfl_xor_sync(TS_FULL, term.x, o); term.y ^= __shfl_xor_sync(TS_FULL, term.y, o);
-        term.z ^= __shfl_xor_sync(TS_FULL, term.z, o); term.w ^= __shfl_xor_sync(TS_FULL, term.w, o);
-    }
+    GCM_HASH_TERMS(kc, B.partials, B.max_ranges, chunk, m, nr, B.aad, B.aad_len, lane, term)
     if (lane == 0) {
-        const uint64_t abits = (uint64_t)B.aad_len * 8, cbits = (uint64_t)n * 8;
-        uint4 L = make_uint4(bswap32((uint32_t)(abits >> 32)), bswap32((uint32_t)abits),
-                             bswap32((uint32_t)(cbits >> 32)), bswap32((uint32_t)cbits));
-        uint4 S = gf_mul(xor4(term, L), kc->hpow[1]);
+        GCM_TAG_S(kc, term, B.aad_len, n, S)
         const uint8_t* ivp = ENC ? B.ivs + (size_t)chunk * GCM_IV : in;
         uint4 j0 = make_uint4(0, 0, 0, 0x01000000u);
         if (!malformed) { j0.x = ld_le32_bytes(ivp); j0.y = ld_le32_bytes(ivp + 4); j0.z = ld_le32_bytes(ivp + 8); }
@@ -363,6 +397,120 @@ gcm_finalize_kernel(const __grid_constant__ Aes256RoundKeys rk, const GcmKeyCtx*
             B.status[chunk] = diff ? 1u : 0u;
             B.out_len[chunk] = n;
         }
+    }
+}
+
+// ------------------------------------------------------------------------------------------ re-encryption under a new key
+// tsgpu_rekey_object: IV || CT || TAG chunks re-encrypted in place, the plaintext only in registers.  A chunk keeps its size.
+struct GcmRekeyBatch {
+    uint8_t* base; const uint64_t* off; const uint32_t* len;   // chunk i: len[i] bytes at base + off[i], 16 + off[i] 16-byte aligned
+    const uint8_t* ivs;              // the new IVs, 12 bytes per chunk
+    const uint8_t* aad_old; uint32_t aad_old_len;
+    const uint8_t* aad_new; uint32_t aad_new_len;
+    uint4* partials_old; uint4* partials_new; uint32_t max_ranges;   // [chunk * max_ranges + range]
+    uint32_t* status;                // 0 ok or empty; 1 old tag mismatch, or a chunk of 1 to 27 bytes
+    uint32_t n_chunks;
+};
+
+__global__ void __launch_bounds__(GH_T, 1)
+gcm_rekey_kernel(const __grid_constant__ Aes256RoundKeys rk_old, const GcmKeyCtx* __restrict__ kc_old,
+                 const __grid_constant__ Aes256RoundKeys rk_new, const GcmKeyCtx* __restrict__ kc_new,
+                 const __grid_constant__ GcmRekeyBatch B) {
+    TS_DYN_SMEM(smem);
+    __shared__ uint4 red_old[GH_T / 32], red_new[GH_T / 32];
+#if TS_DEVICE_ASM
+    __shared__ __align__(8) uint64_t bar;
+#else
+    uint64_t bar_dummy = 0; uint64_t* barp = &bar_dummy;
+#endif
+    const uint8_t* te = smem;
+    uint4* htab_old = (uint4*)(smem + GCM_SMEM_TE);
+    uint4* htab_new = (uint4*)(smem + GCM_SMEM_TE + GCM_SMEM_HTAB);
+
+    const uint32_t chunk = blockIdx.y, range = blockIdx.x, tid = threadIdx.x;
+    const uint32_t len = B.len[chunk];
+    const uint32_t n = len >= GCM_IV + GCM_TAG ? len - (GCM_IV + GCM_TAG) : 0;
+    const uint32_t m = (n + 15) >> 4;
+    const uint32_t b0 = range * GH_RANGE_BLOCKS;
+    if (b0 >= m) return;                                   // uniform for the CTA
+    const uint32_t b1 = min(b0 + GH_RANGE_BLOCKS, m);
+
+#if TS_DEVICE_ASM
+    if (tid == 0) mbar_init(&bar, 1);
+    uint64_t* barp = &bar;
+#endif
+    GCM_FILL_TE(smem, tid)
+    __syncthreads();
+    block_bulk_load(htab_old, kc_old->htab, GCM_SMEM_HTAB, barp, 0);
+    __syncthreads();             // every thread has seen phase 0 complete before phase 1 starts: parity 0 cannot come round again
+    block_bulk_load(htab_new, kc_new->htab, GCM_SMEM_HTAB, barp, 1);
+    __syncthreads();
+
+    uint8_t* chunk_p = B.base + B.off[chunk];
+    uint8_t* ct = chunk_p + GCM_IV;
+    const uint8_t* ivn = B.ivs + (size_t)chunk * GCM_IV;
+    const uint32_t iv0 = ld_le32_bytes(chunk_p), iv1 = ld_le32_bytes(chunk_p + 4), iv2 = ld_le32_bytes(chunk_p + 8);
+    const uint32_t jv0 = ld_le32_bytes(ivn), jv1 = ld_le32_bytes(ivn + 4), jv2 = ld_le32_bytes(ivn + 8);
+    const bool aligned = (((uintptr_t)ct) & 15) == 0;
+    const uint32_t off0 = (tid & 31) * 4, off2 = 128 + off0;
+
+    uint4 acc_old = make_uint4(0, 0, 0, 0), acc_new = make_uint4(0, 0, 0, 0);
+    uint32_t last = 0xffffffffu;
+    for (uint32_t i = b0 + tid; i < b1; i += GH_T) {
+        uint32_t s0 = iv0, s1 = iv1, s2 = iv2, s3 = bswap32(i + 2);
+        aes256_encrypt_te(rk_old, te, off0, off2, s0, s1, s2, s3);
+        uint32_t t0 = jv0, t1 = jv1, t2 = jv2, t3 = bswap32(i + 2);
+        aes256_encrypt_te(rk_new, te, off0, off2, t0, t1, t2, t3);
+        const size_t off = (size_t)i << 4;
+        const bool full = off + 16 <= n;
+        GCM_XOR_BLOCK(ct, ct, off, n, aligned, full, (s0 ^ t0), (s1 ^ t1), (s2 ^ t2), (s3 ^ t3), d, o)   // d: ct_old, o: ct_new
+        acc_old = xor4(gf_mul_tab(htab_old, acc_old), d);
+        acc_new = xor4(gf_mul_tab(htab_new, acc_new), o);
+        last = i;
+    }
+    { GCM_RANGE_PARTIAL(kc_old, acc_old, last, b1, red_old, tid, B.partials_old[(size_t)chunk * B.max_ranges + range]) }
+    { GCM_RANGE_PARTIAL(kc_new, acc_new, last, b1, red_new, tid, B.partials_new[(size_t)chunk * B.max_ranges + range]) }
+}
+
+__global__ void __launch_bounds__(128)
+gcm_rekey_finalize_kernel(const __grid_constant__ Aes256RoundKeys rk_old, const GcmKeyCtx* __restrict__ kc_old,
+                          const __grid_constant__ Aes256RoundKeys rk_new, const GcmKeyCtx* __restrict__ kc_new,
+                          const __grid_constant__ GcmRekeyBatch B) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t chunk = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (chunk >= B.n_chunks) return;                       // whole warp leaves together
+    const uint32_t len = B.len[chunk];
+    if (len < GCM_IV + GCM_TAG) {                          // an empty chunk passes through; a shorter one cannot hold IV and tag
+        if (lane == 0) B.status[chunk] = len ? 1u : 0u;
+        return;
+    }
+    const uint32_t n = len - (GCM_IV + GCM_TAG);
+    const uint32_t m = (n + 15) >> 4;
+    const uint32_t nr = (m + GH_RANGE_BLOCKS - 1) / GH_RANGE_BLOCKS;
+    uint8_t* p = B.base + B.off[chunk];
+    uint4 told = make_uint4(0, 0, 0, 0), tnew = told;      // lane 0: the old tag (recomputed) and the new one
+    const uint8_t* ivn = B.ivs + (size_t)chunk * GCM_IV;
+    {
+        GCM_HASH_TERMS(kc_old, B.partials_old, B.max_ranges, chunk, m, nr, B.aad_old, B.aad_old_len, lane, term)
+        if (lane == 0) {
+            GCM_TAG_S(kc_old, term, B.aad_old_len, n, S)
+            told = xor4(S, aes256_encrypt_slow(rk_old, make_uint4(ld_le32_bytes(p), ld_le32_bytes(p + 4), ld_le32_bytes(p + 8), 0x01000000u)));
+        }
+    }
+    {
+        GCM_HASH_TERMS(kc_new, B.partials_new, B.max_ranges, chunk, m, nr, B.aad_new, B.aad_new_len, lane, term)
+        if (lane == 0) {
+            GCM_TAG_S(kc_new, term, B.aad_new_len, n, S)
+            tnew = xor4(S, aes256_encrypt_slow(rk_new, make_uint4(ld_le32_bytes(ivn), ld_le32_bytes(ivn + 4), ld_le32_bytes(ivn + 8), 0x01000000u)));
+        }
+    }
+    if (lane == 0) {
+        const uint32_t tw[4] = { told.x, told.y, told.z, told.w }, nw[4] = { tnew.x, tnew.y, tnew.z, tnew.w };
+        uint32_t diff = 0;
+        for (int q = 0; q < 16; q++) diff |= (uint32_t)(p[GCM_IV + n + q] ^ (uint8_t)(tw[q >> 2] >> (8 * (q & 3))));
+        B.status[chunk] = diff ? 1u : 0u;
+        for (int q = 0; q < 12; q++) p[q] = ivn[q];
+        for (int q = 0; q < 16; q++) p[GCM_IV + n + q] = (uint8_t)(nw[q >> 2] >> (8 * (q & 3)));
     }
 }
 

@@ -123,14 +123,14 @@ struct Work {
     bool out_pending = false;              // a copy-out on out_stream still reads this slot's final buffer
     bool ready = false;
     bool claimed = false;                  // owned by a call in progress (guarded by tsgpu_ctx::mu)
-    GcmKeys keys[2];               // [0] every call's; [1] the new key of tsgpu_rewrite_object (allocated on first use)
+    GcmKeys keys[2];               // [0] every call's; [1] the new key of tsgpu_rewrite_object / tsgpu_rekey_object (allocated on first use)
     uint8_t* d_orig = nullptr;     // max_batch * chunk_cap
     uint8_t* d_frames = nullptr;   // max_batch * frame_stride        (zstd frames, 16-byte aligned slots)
     uint8_t* d_xf = nullptr;       // max_batch * slot_stride         (transformed slots)
     uint8_t* d_pack = nullptr;     // max_batch * slot_stride         (transformed chunks back to back: what one D2H takes home)
     uint8_t* d_desc = nullptr;  uint8_t* h_desc = nullptr;  size_t desc_bytes = 0;
     Desc dd{}, hd{};               // device / pinned-host views of the descriptor block
-    uint4* d_partials = nullptr;  uint32_t max_ranges = 0;
+    uint4* d_partials = nullptr;  uint32_t max_ranges = 0;   // 2 * max_ranges * max_batch: [0] every GCM stage's, [1] the rekey's new key
     ZstdEncScratch zenc{};         // region kernel (TSGPU_FLAG_ZSTD_DENSE), allocated on first use
     ZstdBlkScratch zblk{};         // block kernel (default), allocated on first use
     ZstdDecScratch zdec{};
@@ -223,7 +223,7 @@ static int work_init_impl(tsgpu_ctx* c, Work& w, int device) {
     RT(rt::malloc_host((void**)&w.h_back, w.back_bytes));
     carve_back(w.h_back, c->max_batch, w.back);
     w.max_ranges = (uint32_t)((frame_bound(c->chunk_cap) / 16 + GH_RANGE_BLOCKS) / GH_RANGE_BLOCKS) + 1;
-    RT(rt::malloc_device((void**)&w.d_partials, sizeof(uint4) * (size_t)w.max_ranges * nb));
+    RT(rt::malloc_device((void**)&w.d_partials, 2 * sizeof(uint4) * (size_t)w.max_ranges * nb));   // the rekey takes two sets
     RT(rt::malloc_device((void**)&w.keys[0].ctx, sizeof(GcmKeyCtx)));
     w.keys[0].d_aad = w.dd.aad;
     const char* e = zstd_dec_scratch_alloc(w.zdec, c->chunk_cap, c->max_batch);
@@ -299,6 +299,7 @@ extern "C" int tsgpu_create(const int* device_ids, int n_devices, uint32_t max_c
         rt::set_device(ids[l]);
         const char* e = rt::allow_smem(gcm_main_kernel<true>, GCM_SMEM_BYTES);
         if (!e) e = rt::allow_smem(gcm_main_kernel<false>, GCM_SMEM_BYTES);
+        if (!e) e = rt::allow_smem(gcm_rekey_kernel, GCM_REKEY_SMEM_BYTES);
         if (e) { tsgpu_destroy(c); return fail(TSGPU_E_CUDA, "gcm kernel attributes: %s", e); }
         e = zstd_kernels_configure();
         if (e) { tsgpu_destroy(c); return fail(TSGPU_E_CUDA, "zstd kernel attributes: %s", e); }
@@ -372,15 +373,22 @@ static int zstd_stage(tsgpu_ctx* c, Work& w, rt::stream_t st, uint32_t flags, Ch
 // with one segment's data key skip the set-up kernel.  Host and device calls share slot 0's tables; that is safe because device
 // calls are ordered behind each other by events (dev_call_begin) and a host call takes the slot only once device work on it has
 // completed.
-template <bool ENC>
-static int gcm_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, const Aes256RoundKeys& rk, ChunksIn in, ChunksOut out,
-                     uint32_t aad_len, uint32_t* d_status, uint32_t n_chunks, uint32_t max_payload, uint32_t out_cap) {
+// The key tables of `rk` in k.ctx: the set-up kernel unless they are there already.  k.valid stays false until the caller has
+// enqueued the kernels that read them.
+static int gcm_key_tables(tsgpu_ctx* c, GcmKeys& k, rt::stream_t st, const Aes256RoundKeys& rk) {
     const bool key_ready = k.valid && memcmp(&k.rk, &rk, sizeof rk) == 0;
     k.rk = rk; k.valid = false;                              // valid again once the whole stage has been enqueued
     if (!key_ready) {
         TS_LAUNCH_P(c->prof, "gcm_key_setup", gcm_key_setup_kernel, dim3(1), dim3(GH_T), 0, st, rk, k.ctx);
         CHECK_LAUNCH("gcm_key_setup_kernel");
     }
+    return TSGPU_OK;
+}
+
+template <bool ENC>
+static int gcm_stage(tsgpu_ctx* c, Work& w, GcmKeys& k, rt::stream_t st, const Aes256RoundKeys& rk, ChunksIn in, ChunksOut out,
+                     uint32_t aad_len, uint32_t* d_status, uint32_t n_chunks, uint32_t max_payload, uint32_t out_cap) {
+    { int rc = gcm_key_tables(c, k, st, rk); if (rc) return rc; }
     GcmBatch B;
     B.in_base = in.base; B.in_off = in.off; B.in_len = in.len;
     B.out_base = out.base; B.out_off = out.off; B.out_len = out.len;
@@ -863,6 +871,8 @@ static void parts_finish(const PartsRun<W>& pr, int segment_ends_here) {
 //   TSGPU_SIMT_FLIP_DECODED: the chunk's decoded bytes in d_orig right after the source decode of tsgpu_check_object /
 //     tsgpu_rewrite_object -- a decoder that misread the chunk.  tests/test_simt_reframe.py drives it: TSGPU_FLAG_REFRAME must
 //     not stamp the checksum of such a chunk.
+//   TSGPU_SIMT_FLIP_REKEYED: the chunk's re-encrypted bytes in its d_xf slot right after the rekey kernels of tsgpu_rekey_object
+//     -- a rekey that wrote a wrong byte.  tests/test_simt_rekey.py drives it: TSGPU_FLAG_VERIFY must catch it.
 static void simt_flip(const char* var, ChunksOut chunks, uint32_t c0, uint32_t nb) {
     const char* e = getenv(var);
     long k = 0, at = 0;
@@ -1012,14 +1022,14 @@ static int verify_verdict(const Batch& bt, const uint32_t* len, uint64_t first =
     return TSGPU_OK;
 }
 
-// The drain of a batch whose target half ran (transform, rewrite), once its verdicts have passed: its new sizes go to the
-// caller's `sizes`, [its part prefixes are cut,] and its bytes leave.
+// The drain of a batch whose target half ran (transform, rewrite, rekey), once its verdicts have passed: its new sizes go to the
+// caller's `sizes` (nullptr: the caller knows them), [its part prefixes are cut,] and its bytes leave.
 template <typename W>
 static int target_drain(tsgpu_ctx* c, const Batch& bt, uint32_t* sizes, PartsRun<W>* parts, uint8_t* dst, uint64_t dst_cap,
                         uint64_t& dst_off) {
     Work& w = *bt.w;
     uint64_t total = 0;
-    for (uint32_t i = 0; i < bt.nb; i++) { sizes[bt.c0 + i] = w.back.sizes[i]; total += w.back.sizes[i]; }
+    for (uint32_t i = 0; i < bt.nb; i++) { if (sizes) sizes[bt.c0 + i] = w.back.sizes[i]; total += w.back.sizes[i]; }
     if (parts && dst_off + total <= dst_cap) {
         int rc = parts_drain(c, w, *parts, bt.c0 / c->max_batch, dst_off, total);
         if (rc) return rc;
@@ -1580,6 +1590,39 @@ template <typename W> struct RewriteCarry {
 static_assert(sizeof(RewriteCarry<uint32_t>) == sizeof(tsgpu_rewrite_cursor) && sizeof(RewriteCarry<uint64_t>) == sizeof(tsgpu_rewrite_cursor),
               "the cursor holds the carry");
 
+// GCM breaks when one key encrypts two plaintexts under one IV: no two chunks of a window of n chunks may share a new IV, nor,
+// with same_key (the new key is the old one), a new IV an old chunk of the window has (an old chunk's IV is its first 12 bytes of
+// `src`).  `first`: the object's number of the window's first chunk.  skip_empty: a chunk of 0 bytes takes no new IV.
+static int new_ivs_ok(const uint8_t* to_ivs, uint32_t n, const uint8_t* src, const uint32_t* tsizes, bool same_key, uint64_t first,
+                      bool skip_empty) {
+    struct Iv { std::array<uint8_t, TSGPU_IV_SIZE> b; uint32_t i; bool old; };
+    std::vector<Iv> ivs;
+    for (uint32_t i = 0; i < n; i++) {
+        if (skip_empty && tsizes[i] == 0) continue;
+        Iv v{{}, i, false};
+        memcpy(v.b.data(), to_ivs + (size_t)i * TSGPU_IV_SIZE, TSGPU_IV_SIZE);
+        ivs.push_back(v);
+    }
+    if (same_key) {
+        uint64_t at = 0;
+        for (uint32_t i = 0; i < n; at += tsizes[i++]) {
+            if (tsizes[i] < TSGPU_IV_SIZE) continue;
+            Iv v{{}, i, true};
+            memcpy(v.b.data(), src + at, TSGPU_IV_SIZE);
+            ivs.push_back(v);
+        }
+    }
+    std::sort(ivs.begin(), ivs.end(), [](const Iv& x, const Iv& y) { return x.b != y.b ? x.b < y.b : x.old < y.old; });
+    for (size_t j = 1; j < ivs.size(); j++) {
+        const Iv &x = ivs[j - 1], &y = ivs[j];
+        if (x.b != y.b || (x.old && y.old)) continue;           // two old chunks sharing an IV is the old object's business
+        if (y.old) return fail(TSGPU_E_ARG, "to_ivs[%u] repeats the IV of chunk %llu under the same key", x.i,
+                               (unsigned long long)(first + y.i));
+        return fail(TSGPU_E_ARG, "to_ivs[%u] repeats to_ivs[%u]", std::min(x.i, y.i), std::max(x.i, y.i));
+    }
+    return TSGPU_OK;
+}
+
 // One batch of a rewrite: the target's IVs and AAD, the source half, the target half, the D2H of the new sizes.
 template <typename W>
 static int rewrite_issue(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, const TargetReq& t, uint64_t g0) {
@@ -1650,33 +1693,9 @@ static int rewrite_object(tsgpu_ctx* c, uint32_t from_flags, const uint8_t* src,
                          from_key, from_aad, from_aad_len, cur.src.chunks, q);
     if (rc) return rc;
     if (q.n && !dst) return fail(TSGPU_E_ARG, "dst cannot be null");
-    // GCM breaks when one key encrypts two plaintexts under one IV: no two chunks of the window may share a new IV, nor, under
-    // the old key, a new IV an old chunk of the window has (an old chunk's IV is its first 12 bytes)
     if ((to_flags & TSGPU_FLAG_AES) && q.n) {
-        struct Iv { std::array<uint8_t, TSGPU_IV_SIZE> b; uint32_t i; bool old; };
-        std::vector<Iv> ivs;
-        for (uint32_t i = 0; i < q.n; i++) {
-            Iv v{{}, i, false};
-            memcpy(v.b.data(), to_ivs + (size_t)i * TSGPU_IV_SIZE, TSGPU_IV_SIZE);
-            ivs.push_back(v);
-        }
-        if ((q.flags & TSGPU_FLAG_AES) && memcmp(from_key, to_key, 32) == 0) {
-            uint64_t at = 0;
-            for (uint32_t i = 0; i < q.n; at += transformed_sizes[i++]) {
-                if (transformed_sizes[i] < TSGPU_IV_SIZE) continue;
-                Iv v{{}, i, true};
-                memcpy(v.b.data(), src + at, TSGPU_IV_SIZE);
-                ivs.push_back(v);
-            }
-        }
-        std::sort(ivs.begin(), ivs.end(), [](const Iv& x, const Iv& y) { return x.b != y.b ? x.b < y.b : x.old < y.old; });
-        for (size_t j = 1; j < ivs.size(); j++) {
-            const Iv &x = ivs[j - 1], &y = ivs[j];
-            if (x.b != y.b || (x.old && y.old)) continue;           // two old chunks sharing an IV is the old object's business
-            if (y.old) return fail(TSGPU_E_ARG, "to_ivs[%u] repeats the IV of chunk %llu under the same key", x.i,
-                                   (unsigned long long)(cur.src.chunks + y.i));
-            return fail(TSGPU_E_ARG, "to_ivs[%u] repeats to_ivs[%u]", std::min(x.i, y.i), std::max(x.i, y.i));
-        }
+        const bool same_key = (q.flags & TSGPU_FLAG_AES) && memcmp(from_key, to_key, 32) == 0;
+        if ((rc = new_ivs_ok(to_ivs, q.n, src, transformed_sizes, same_key, cur.src.chunks, /*skip_empty=*/false))) return rc;
     }
     // part_cap: the transform bound of the window's length by the chunk index, or of its kept frames (4 bytes more each when
     // TSGPU_FLAG_REFRAME seals them: a dense frame replaces one only when it is smaller)
@@ -1754,6 +1773,230 @@ extern "C" int tsgpu_rewrite_object_crc64(tsgpu_ctx* c, uint32_t from_flags, con
     return rewrite_object(c, from_flags, src, src_len, transformed_sizes, n_chunks, original_chunk_size, original_file_size, from_key,
                           from_aad, from_aad_len, to_flags, to_key, to_aad, to_aad_len, to_ivs, dst, dst_cap, new_transformed_sizes,
                           part_size, part_crc64, part_cap, n_parts, cursor, object_ends_here, source_crc64, object_crc64, segment_crc64);
+}
+
+// ------------------------------------------------------------------------------------------ object rekey (host)
+// tsgpu_rekey_object: a stored object's IV || CT || TAG chunks re-encrypted under a new key with nothing decoded.  Per batch, on the
+// compute stream: the chunks into the d_xf slots, pcrc over them where they sit (the source word), [VERIFY: the DEC kernels
+// decrypt them under the old key into the d_frames slots,] the rekey kernels in place, [VERIFY: the DEC kernels decrypt the new
+// chunks under the new key into d_pack at the frame slots' offsets and verify_compare compares the two plaintexts,] pack_chunks
+// into d_pack and pcrc_tiles over it.  No original chunk, frame or decoder is involved, and without VERIFY neither the d_frames
+// slots nor d_orig are touched.  At the drain, in object order: the old tags, the verify verdict, then the source word extends the
+// carry and target_drain cuts the part prefixes and copies the batch out.
+
+// The state of a rekey between calls: the public tsgpu_rekey_cursor (64 bytes, zero = start of the object).
+template <typename W> struct RekeyCarry {
+    tsgpu_parts_cursor out;    // the new object's parts (a PartsCarry<W>)
+    uint64_t chunks;           // chunks rekeyed so far
+    uint64_t src_len;          // source object bytes so far
+    W src_raw;                 // raw CRC of the source object so far
+    uint64_t reserved;
+};
+static_assert(sizeof(RekeyCarry<uint32_t>) == sizeof(tsgpu_rekey_cursor) && sizeof(RekeyCarry<uint64_t>) == sizeof(tsgpu_rekey_cursor),
+              "the cursor holds the carry");
+
+struct RekeyReq {
+    bool verify;
+    const uint8_t* src; const uint32_t* tsizes;
+    Aes256RoundKeys rk_old, rk_new;
+    const uint8_t* aad_old; uint32_t aad_old_len;
+    const uint8_t* aad_new; uint32_t aad_new_len;
+    const uint8_t* ivs;
+};
+
+template <typename W>
+static int rekey_issue(tsgpu_ctx* c, const Batch& bt, const RekeyReq& q) {
+    Work& w = *bt.w;
+    const uint32_t c0 = bt.c0, nb = bt.nb;
+    RT(rt::set_device(w.device));
+    rt::stream_t st = w.stream;
+    GcmKeys &ko = w.keys[0], &kn = w.keys[1];
+    if (!kn.ctx) {
+        RT(rt::malloc_device((void**)&kn.ctx, sizeof(GcmKeyCtx)));
+        RT(rt::malloc_device((void**)&kn.d_aad, MAX_AAD));
+        RT(rt::malloc_host((void**)&kn.h_aad, MAX_AAD));
+    }
+    if (q.aad_new_len) {                 // the slot's previous batch has drained: its upload of h_aad is done
+        memcpy(kn.h_aad, q.aad_new, q.aad_new_len);
+        RT(rt::h2d(kn.d_aad, kn.h_aad, q.aad_new_len, st));
+    }
+    memcpy(w.hd.ivs, q.ivs + (size_t)c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
+    if (q.aad_old_len) memcpy(w.hd.aad, q.aad_old, q.aad_old_len);
+    slot_layout(c, w.hd, nb, c->slot_stride);
+    uint64_t at = bt.in_off, obj = 0;
+    uint32_t max_t = 0;
+    for (uint32_t i = 0; i < nb; i++) {  // the sizes were bounded by the slot before any GPU work
+        const uint32_t t = q.tsizes[c0 + i];
+        w.hd.c_len[i] = t;
+        w.back.sizes[i] = t;             // a chunk keeps its size
+        if (t) RT(rt::h2d(w.d_xf + w.hd.c_off[i], q.src + at, t, st));
+        at += t; obj += t;
+        max_t = std::max(max_t, t);
+    }
+    RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
+    // the slot's previous batch may still be copying d_pack out, its part prefixes read from the pcrc scratch this batch rewrites
+    { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
+    const ChunksIn in{w.d_xf, w.dd.c_off, w.dd.c_len};
+    { int rc = check_crc_word<W, true>(c, w, st, in.base, in.off, in.len, nb, obj, 0); if (rc) return rc; }
+    RT(rt::d2h(w.back.words, pcrc_of<W>(w).d_cuts, sizeof(W), st));
+    const uint32_t payload = max_t >= 28 ? max_t - 28 : 0, room = (uint32_t)(c->frame_stride - 16);
+    if (q.verify) {                      // the old plaintext, for the comparison below
+        RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
+        int rc = gcm_stage<false>(c, w, ko, st, q.rk_old, in, ChunksOut{w.d_frames, w.dd.b_off, w.dd.b_len}, q.aad_old_len, w.dd.status,
+                                  nb, max_t, room);
+        if (rc) return rc;
+    }
+    { int rc = gcm_key_tables(c, ko, st, q.rk_old); if (!rc) rc = gcm_key_tables(c, kn, st, q.rk_new); if (rc) return rc; }
+    GcmRekeyBatch R;
+    R.base = w.d_xf; R.off = w.dd.c_off; R.len = w.dd.c_len; R.ivs = w.dd.ivs;
+    R.aad_old = ko.d_aad; R.aad_old_len = q.aad_old_len; R.aad_new = kn.d_aad; R.aad_new_len = q.aad_new_len;
+    R.partials_old = w.d_partials; R.partials_new = w.d_partials + (size_t)w.max_ranges * c->max_batch; R.max_ranges = w.max_ranges;
+    R.status = w.dd.status; R.n_chunks = nb;
+    const uint32_t ranges = (uint32_t)(((uint64_t)payload + 15) / 16 + GH_RANGE_BLOCKS - 1) / GH_RANGE_BLOCKS;
+    if (ranges) {
+        TS_LAUNCH_P(c->prof, "gcm_rekey", gcm_rekey_kernel, dim3(ranges, nb), dim3(GH_T), GCM_REKEY_SMEM_BYTES, st, q.rk_old, ko.ctx,
+                    q.rk_new, kn.ctx, R);
+        CHECK_LAUNCH("gcm_rekey_kernel");
+    }
+    TS_LAUNCH_P(c->prof, "gcm_rekey_finalize", gcm_rekey_finalize_kernel, dim3((nb + 3) / 4), dim3(128), 0, st, q.rk_old, ko.ctx,
+                q.rk_new, kn.ctx, R);
+    CHECK_LAUNCH("gcm_rekey_finalize_kernel");
+    ko.valid = kn.valid = true;
+    RT(rt::d2h(w.back.src_status, w.dd.status, 4ull * nb, st));
+#ifdef TSGPU_SIMT
+    simt_flip("TSGPU_SIMT_FLIP_REKEYED", ChunksOut{w.d_xf, w.dd.c_off, w.dd.c_len}, c0, nb);
+#endif
+    if (q.verify) {                      // the new chunks read back under the new key
+        RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
+        RT(rt::memset_async(w.dd.v_diff, 0xff, 4ull * nb, st));
+        int rc = gcm_stage<false>(c, w, kn, st, q.rk_new, in, ChunksOut{w.d_pack, w.dd.b_off, w.dd.v_len}, q.aad_new_len, w.dd.status,
+                                  nb, max_t, room);
+        if (rc) return rc;
+        VerifyArgs V;
+        V.orig = w.d_frames; V.orig_off = w.dd.b_off; V.orig_len = w.dd.b_len;
+        V.back = w.d_pack; V.back_off = w.dd.b_off; V.back_len = w.dd.v_len;
+        V.status = w.dd.status; V.diff = w.dd.v_diff;
+        TS_LAUNCH_P(c->prof, "verify_compare", verify_compare_kernel, dim3(std::max(1u, (payload + VERIFY_PIECE - 1) / VERIFY_PIECE), nb),
+                    dim3(VERIFY_T), 0, st, V);
+        CHECK_LAUNCH("verify_compare_kernel");
+        RT(rt::d2h(w.back.status, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.back.diff, w.dd.v_diff, 4ull * nb, st));
+    }
+    PackArgs P;
+    P.base = w.d_xf; P.stride = c->slot_stride; P.head = TSGPU_SLOT_HEAD; P.len = w.dd.c_len; P.n = nb; P.out = w.d_pack;
+    TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3(std::max(1u, (max_t + PACK_PIECE - 1) / PACK_PIECE), nb), dim3(PACK_T),
+                0, st, P);
+    CHECK_LAUNCH("pack_chunks_kernel");
+    { int rc = parts_stage<W>(c, w, st, w.dd.c_len, nb, obj); if (rc) return rc; }
+    RT(rt::event_record(w.ev_sizes, st));
+    return TSGPU_OK;
+}
+
+// A drained batch's verdicts in object order: every old tag, then (VERIFY) every read-back.  `first`: the object's number of the
+// call's first chunk.
+static int rekey_verdict(const Batch& bt, const RekeyReq& q, uint64_t first) {
+    const Back& b = bt.w->back;
+    for (uint32_t i = 0; i < bt.nb; i++)
+        if (b.src_status[i]) return fail(TSGPU_E_AUTH, "Tag mismatch in chunk %llu", (unsigned long long)(first + bt.c0 + i));
+    if (!q.verify) return TSGPU_OK;
+    for (uint32_t i = 0; i < bt.nb; i++) {
+        const unsigned long long g = first + bt.c0 + i;
+        if (q.tsizes[bt.c0 + i] == 0) continue;          // nothing to read back (the DEC kernels call an empty chunk malformed)
+        if (b.status[i] == 1) return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back under the new key: tag check failed", g);
+        if (b.status[i] != 0) return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back under the new key: size check failed", g);
+        if (b.diff[i] != VERIFY_NO_DIFF)
+            return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back under the new key: plaintext differs from byte %u", g, b.diff[i]);
+    }
+    return TSGPU_OK;
+}
+
+template <typename W>
+static int rekey_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                        uint32_t n_chunks, const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                        const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len, const uint8_t* to_ivs,
+                        uint8_t* dst, uint64_t dst_cap, uint64_t part_size, W* part_crc, uint32_t part_cap, uint32_t* n_parts,
+                        tsgpu_rekey_cursor* cursor, int object_ends_here, W* source_crc, W* object_crc) try {
+    if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
+    if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
+    if (object_ends_here && (!source_crc || !object_crc))
+        return fail(TSGPU_E_ARG, "source_%s/object_%s cannot be null", crc_arg<W>(), crc_arg<W>());
+    if (flags & ~TSGPU_FLAG_VERIFY) return fail(TSGPU_E_ARG, "unknown flags %u: only TSGPU_FLAG_VERIFY applies to a rekey", flags);
+    if (n_chunks && !transformed_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
+    if (int rc = aes_args_ok(TSGPU_FLAG_AES, AES_DEC, from_key, true, from_aad, from_aad_len)) return rc;
+    if ((uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
+        return fail(TSGPU_E_ARG, "part checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
+                    (unsigned long long)c->slot_stride);
+    RekeyCarry<W> cur;
+    memcpy(&cur, cursor, sizeof cur);
+    uint64_t need = 0;
+    for (uint32_t i = 0; i < n_chunks; i++) {
+        // a chunk goes into one transformed slot (what tsgpu_detransform reads one into)
+        if (transformed_sizes[i] > c->slot_stride - TSGPU_SLOT_HEAD - 16)
+            return fail(TSGPU_E_ARG, "chunk %llu: transformed chunk of %u bytes exceeds the context's capacity",
+                        (unsigned long long)(cur.chunks + i), transformed_sizes[i]);
+        need += transformed_sizes[i];
+    }
+    if (int rc = aes_args_ok(TSGPU_FLAG_AES, AES_TO, to_key, !need || to_ivs, to_aad, to_aad_len)) return rc;   // empty chunks take no IV
+    if (need && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
+    if (need > src_len) return fail(TSGPU_E_SHORT, "Stream has fewer bytes than expected");
+    if (need && !dst) return fail(TSGPU_E_ARG, "dst cannot be null");
+    if (need > dst_cap) return fail(TSGPU_E_SHORT, "dst too small: the window's chunks are %llu bytes, dst_cap is %llu",
+                                    (unsigned long long)need, (unsigned long long)dst_cap);
+    if (need) {
+        if (int rc = new_ivs_ok(to_ivs, n_chunks, src, transformed_sizes, memcmp(from_key, to_key, 32) == 0, cur.chunks,
+                                /*skip_empty=*/true)) return rc;
+    }
+    PartsRun<W> run;
+    if (int rc = parts_begin(run, PartsReq<W>{part_size, &cur.out, part_crc, part_cap, n_parts, object_crc}, TSGPU_FLAG_AES, need,
+                             object_ends_here)) return rc;
+    RekeyReq q;
+    q.verify = (flags & TSGPU_FLAG_VERIFY) || c->verify_default;
+    q.src = src; q.tsizes = transformed_sizes;
+    q.rk_old = aes256_expand_key(from_key); q.rk_new = aes256_expand_key(to_key);
+    q.aad_old = from_aad; q.aad_old_len = from_aad_len; q.aad_new = to_aad; q.aad_new_len = to_aad_len;
+    q.ivs = to_ivs;
+    if (need) {                                                            // a window of empty chunks writes nothing
+        uint64_t dst_off = 0;
+        const int rc = run_batches(c, n_chunks, transformed_sizes,
+            [&](const Batch& bt) { return rekey_issue<W>(c, bt, q); },
+            [&](const Batch& bt) {
+                { int r = rekey_verdict(bt, q, cur.chunks); if (r) return r; }
+                uint64_t obj = 0;
+                for (uint32_t i = 0; i < bt.nb; i++) obj += transformed_sizes[bt.c0 + i];
+                cur.src_raw = crc_shift(cur.src_raw, obj, 0) ^ reinterpret_cast<const W*>(bt.w->back.words)[0];
+                return target_drain<W>(c, bt, nullptr, &run, dst, dst_cap, dst_off);
+            },
+            [&](const std::vector<Work*>& slots, int rcb) { return parts_idle(&run, slots, rcb); });
+        if (rc) return rc;
+    }
+    cur.chunks += n_chunks;
+    cur.src_len += need;
+    parts_finish(run, object_ends_here);                                   // writes cur.out and the part CRCs
+    if (object_ends_here) *source_crc = crc_finish(cur.src_raw, cur.src_len, 0);
+    memcpy(cursor, &cur, sizeof cur);
+    return TSGPU_OK;
+} catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
+
+extern "C" int tsgpu_rekey_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* transformed_sizes,
+                                  uint32_t n_chunks, const uint8_t from_key[32], const uint8_t* from_aad, uint32_t from_aad_len,
+                                  const uint8_t to_key[32], const uint8_t* to_aad, uint32_t to_aad_len, const uint8_t* to_ivs,
+                                  uint8_t* dst, uint64_t dst_cap, uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap,
+                                  uint32_t* n_parts, tsgpu_rekey_cursor* cursor, int object_ends_here, uint32_t* source_crc32c,
+                                  uint32_t* object_crc32c) {
+    return rekey_object(c, flags, src, src_len, transformed_sizes, n_chunks, from_key, from_aad, from_aad_len, to_key, to_aad,
+                        to_aad_len, to_ivs, dst, dst_cap, part_size, part_crc32c, part_cap, n_parts, cursor, object_ends_here,
+                        source_crc32c, object_crc32c);
+}
+
+extern "C" int tsgpu_rekey_object_crc64(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len,
+                                        const uint32_t* transformed_sizes, uint32_t n_chunks, const uint8_t from_key[32],
+                                        const uint8_t* from_aad, uint32_t from_aad_len, const uint8_t to_key[32], const uint8_t* to_aad,
+                                        uint32_t to_aad_len, const uint8_t* to_ivs, uint8_t* dst, uint64_t dst_cap, uint64_t part_size,
+                                        uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts, tsgpu_rekey_cursor* cursor,
+                                        int object_ends_here, uint64_t* source_crc64, uint64_t* object_crc64) {
+    return rekey_object(c, flags, src, src_len, transformed_sizes, n_chunks, from_key, from_aad, from_aad_len, to_key, to_aad,
+                        to_aad_len, to_ivs, dst, dst_cap, part_size, part_crc64, part_cap, n_parts, cursor, object_ends_here,
+                        source_crc64, object_crc64);
 }
 
 // ------------------------------------------------------------------------------------------ device-resident API
