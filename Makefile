@@ -84,3 +84,9 @@ tests/cpp/test_jni_rekey_simt: tests/cpp/test_jni_rekey.c jni/tsgpu_jni.c tests/
 # Host mirror of key rotation (RemoteSegmentRekeyer, tsgpu_rekey_object) on an oracle-written segment, on the emulator build
 tests/cpp/test_rekey_mirror_simt: tests/cpp/test_rekey_mirror.cpp $(PKG)/host/chunk_transform.hpp $(PKG)/host/segment_upload.hpp $(PKG)/host/segment_rekey.hpp include/tsgpu.h tests/simt/libtsgpu_simt.so oracle
 	g++ -O1 -g -std=c++17 -o $@ tests/cpp/test_rekey_mirror.cpp -Ltests/simt -ltsgpu_simt -Loracle -ltsoracle -Wl,-rpath,'$$ORIGIN/../simt' -Wl,-rpath,'$$ORIGIN/../../oracle'
+# JNI glue's encryption path (EncryptCursor.encryptObject, encryptObjectCrc64) on an oracle-written object, same fake JNIEnv
+tests/cpp/test_jni_encrypt_simt: tests/cpp/test_jni_encrypt.c jni/tsgpu_jni.c tests/jni_stub/jni.h include/tsgpu.h tests/simt/libtsgpu_simt.so oracle
+	gcc -O1 -g -std=gnu11 -Wall -Wno-unused-parameter -Wno-unused-function -Itests/jni_stub -Iinclude -o $@ tests/cpp/test_jni_encrypt.c -Ltests/simt -ltsgpu_simt -Loracle -ltsoracle -Wl,-rpath,'$$ORIGIN/../simt' -Wl,-rpath,'$$ORIGIN/../../oracle'
+# Host mirror of encryption (RemoteSegmentEncryptor, tsgpu_encrypt_object) on an oracle-written segment, on the emulator build
+tests/cpp/test_encrypt_mirror_simt: tests/cpp/test_encrypt_mirror.cpp $(PKG)/host/chunk_transform.hpp $(PKG)/host/segment_upload.hpp $(PKG)/host/segment_encrypt.hpp include/tsgpu.h tests/simt/libtsgpu_simt.so oracle
+	g++ -O1 -g -std=c++17 -o $@ tests/cpp/test_encrypt_mirror.cpp -Ltests/simt -ltsgpu_simt -Loracle -ltsoracle -Wl,-rpath,'$$ORIGIN/../simt' -Wl,-rpath,'$$ORIGIN/../../oracle'

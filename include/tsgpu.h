@@ -429,6 +429,70 @@ int tsgpu_rekey_object_crc64(tsgpu_ctx* ctx, uint32_t flags,
                              uint64_t* source_crc64, uint64_t* object_crc64);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * tsgpu_encrypt_object — the chunks of a stored unencrypted object encrypted with AES-GCM and nothing decoded: for turning
+ * encryption on for a segment already in the bucket.  A stored chunk, compressed or plain, is exactly the plaintext that
+ * EncryptionChunkEnumeration encrypts, so the new chunk i is IV_i || AES-256-GCM(key, IV_i, aad, chunk i) || TAG, 28 bytes longer,
+ * and the frames stay byte for byte what they were (a Content_Checksum they carry included): the new object decodes to the same
+ * segment.  One GCM pass per byte; no decoder runs.  The call serves both objects of a segment: the .log object (its chunks by the
+ * chunk index) and the .indexes object (its blobs at their SegmentIndexesV1 positions and sizes).
+ *
+ *   flags          TSGPU_FLAG_ZSTD when the object is compressed (the manifest's `compression`), and TSGPU_FLAG_VERIFY; any other
+ *                  bit fails with TSGPU_E_ARG, TSGPU_FLAG_AES with a message that points at tsgpu_rekey_object (the object is
+ *                  already encrypted).  TSGPU_VERIFY=1 turns VERIFY on; TSGPU_ZSTD_MODE and TSGPU_ZSTD_CHECKSUM have nothing to act
+ *                  on.  With VERIFY every new chunk of a batch is decrypted again by the separate decrypt kernels and compared
+ *                  with its source chunk on the GPU before any byte of the batch is released; a difference fails with
+ *                  TSGPU_E_VERIFY naming the chunk and the first differing byte.
+ *   src, src_len, chunk_sizes, n_chunks   the window's chunks back to back.
+ *   original_chunk_size, original_file_size   the chunk index of a .log object (> 0): the chunks are walked as tsgpu_check_object
+ *                  walks them, chunk k holding the size the index gives it, and at object_ends_here the chunk count must be the
+ *                  index's (an empty segment's object is its one chunk of 0 bytes).  Without ZSTD each chunk's size must be its
+ *                  index size.  With ZSTD each non-empty chunk must be one frame that the decoder's index stage accepts: the magic
+ *                  number, no Dictionary_ID, a Frame_Content_Size equal to the index size, a block walk that ends at a last block
+ *                  without a reserved type inside the chunk, and after the frame only the announced Content_Checksum and
+ *                  skippable frames.  The Content_Checksum is not verified: that needs the decoded bytes.  A failure is
+ *                  TSGPU_E_CORRUPT with tsgpu_check_object's messages ("Invalid zstd frame in chunk <k> (code 2)", "chunk <k>
+ *                  decoded to <n> bytes, the chunk index gives <m>": for a frame, n is its Frame_Content_Size).
+ *                  0 for an .indexes object: its chunks are the index blobs, only the size bound below applies, and ZSTD fails
+ *                  with TSGPU_E_ARG.
+ *   key, aad, ivs  the data key and AAD, and one 12-byte IV per chunk.  No two non-empty chunks of the window may get the same IV
+ *                  (TSGPU_E_ARG, before any GPU work: tsgpu_rewrite_object's message).
+ *   dst, dst_cap, new_transformed_sizes   receive exactly the sum of the new sizes: new_transformed_sizes[i] = chunk_sizes[i] + 28,
+ *                  or 0 for a chunk of 0 bytes, which passes through as 0 bytes and takes no IV (an empty index blob, the empty
+ *                  segment's chunk: what transformIndex writes for an empty index).  A smaller dst_cap fails with TSGPU_E_SHORT,
+ *                  and a chunk whose new size does not fit the context's transformed slot (what tsgpu_detransform takes) with
+ *                  TSGPU_E_ARG, both before any GPU work.
+ *   part_size, part_crc32c, part_cap, n_parts   as tsgpu_transform_parts, with an exact bound: part_cap >= floor((carried +
+ *                  sum(new sizes)) / part_size) + (object_ends_here ? 1 : 0); a smaller part_cap fails with TSGPU_E_SHORT before any
+ *                  GPU work.
+ *   cursor         64 bytes, zeroed at the start of the object, passed to every window in order: the parts cursor, the source
+ *                  object's running CRC and length, and the chunk count (messages name a chunk by its number in the object).
+ *                  Updated on success, without a defined value after a failure.
+ *   object_ends_here  != 0 on the last window (which may be empty): then *source_crc32c is the CRC-32C of the old object and
+ *                  *object_crc32c that of the new object (FULL_OBJECT).  Neither is written before the end or on failure.
+ * Returns the first failure in object order; within a batch: the frame and size checks (TSGPU_E_CORRUPT), then VERIFY
+ * (TSGPU_E_VERIFY).  No byte of a failing batch reaches dst; earlier batches may already be there.  A failed call writes no CRC.
+ * Buffers and cost: DESIGN.md §3, §8.
+ * --------------------------------------------------------------------------------------------------------- */
+typedef struct tsgpu_encrypt_cursor { uint64_t opaque[8]; } tsgpu_encrypt_cursor;
+int tsgpu_encrypt_object(tsgpu_ctx* ctx, uint32_t flags,
+                         const uint8_t* src, uint64_t src_len, const uint32_t* chunk_sizes, uint32_t n_chunks,
+                         uint32_t original_chunk_size, uint64_t original_file_size,
+                         const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                         uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                         uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
+                         tsgpu_encrypt_cursor* cursor, int object_ends_here,
+                         uint32_t* source_crc32c, uint32_t* object_crc32c);
+/* The CRC-64/NVME twin: the same arguments, rules, errors and output bytes, with 64-bit part, source and object words. */
+int tsgpu_encrypt_object_crc64(tsgpu_ctx* ctx, uint32_t flags,
+                               const uint8_t* src, uint64_t src_len, const uint32_t* chunk_sizes, uint32_t n_chunks,
+                               uint32_t original_chunk_size, uint64_t original_file_size,
+                               const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                               uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                               uint64_t part_size, uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts,
+                               tsgpu_encrypt_cursor* cursor, int object_ends_here,
+                               uint64_t* source_crc64, uint64_t* object_crc64);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Device-resident variants (inputs and outputs already in HBM of device `device_index` of the context; used by
  * bench.py for the kernel-side throughput and by callers that keep segments on the GPU).  Layouts:
  *   original side     contiguous, chunk i at i * chunk_size

@@ -3,7 +3,7 @@
  * There is no JDK in this repository's build image: the tests compile this file against a test-only stand-in for
  * <jni.h> and drive it through a fake JNIEnv (tests/cpp/test_jni_shim.c).  Build on the broker host with
  *   gcc -shared -fPIC -I$JAVA_HOME/include -I$JAVA_HOME/include/linux -Iinclude jni/tsgpu_jni.c -L<pkg> -ltsgpu -o libtsgpu_jni.so
- * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,RewriteCursor,RekeyCursor,Crc64,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
+ * Java side: jni/io/aiven/kafka/tieredstorage/transform/gpu/{TsGpu,RecordsCursor,PartsCursor,CheckCursor,RewriteCursor,RekeyCursor,EncryptCursor,Crc64,PinnedPool,GpuTransformChunkEnumeration,GpuDetransformChunkEnumeration}.java
  * (implement TransformChunkEnumeration / DetransformChunkEnumeration of the reference, core/M/transform/TransformChunkEnumeration.java:28-42,
  * DetransformChunkEnumeration.java:28-29) and jni/io/aiven/kafka/tieredstorage/fetch/gpu/GpuChunkManager.java (ChunkManager, fetch/ChunkManager.java).
  *
@@ -549,5 +549,111 @@ JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_RekeyCurs
                                       (uint64_t)partSize, pc, (uint32_t)(pcap / 8), &nParts, r.cur, objectEndsHere ? 1 : 0, &crcs[0],
                                       &crcs[1]);
     rekey_end(env, transformedSizes, fromKey, fromAad, toKey, toAad, toIvs, nPartsOut, &r, rc, nParts);
+    if (!rc && objectEndsHere) { out[0] = crcs[0]; out[1] = crcs[1]; }
+}
+
+/* ---------------------------------------------------------------------------------------------------------------------------
+ * Encryption of a stored unencrypted object (EncryptCursor.java): one window of its chunks encrypted with nothing decoded
+ * (tsgpu_encrypt_object[_crc64]).  `cursor` a direct ByteBuffer of at least 64 bytes holding the tsgpu_encrypt_cursor (zeros at
+ * the start of the object), updated in place; dst a direct ByteBuffer receiving exactly the window's new bytes (every non-empty
+ * chunk 28 bytes longer); newSizes (int[], one per chunk) the new chunk sizes; ivs 12 bytes per chunk of the window (an empty
+ * chunk takes none, its 12 bytes are not read). */
+
+/* The arguments both widths check the same way; the chunk sizes, key, AAD and IV arrays pinned.  Returns -1 with an exception
+ * pending. */
+typedef struct {
+    uint8_t* s; uint8_t* d; tsgpu_encrypt_cursor* cur; uint32_t n;
+    jint* cs; jint* ns; jbyte* k; jbyte* a; jint alen; jbyte* iv;
+} encrypt_args;
+static int encrypt_begin(JNIEnv* env, jobject src, jlong srcLen, jintArray chunkSizes, jbyteArray key, jbyteArray aad, jbyteArray ivs,
+                         jobject dst, jlong dstCap, jintArray newSizes, jlong partSize, jintArray nPartsOut, jobject cursor,
+                         encrypt_args* r) {
+    jlong ccap = 0;
+    r->s = srcLen ? direct(env, src, srcLen, NULL, "src must be a direct ByteBuffer") : NULL;
+    if (srcLen && !r->s) return -1;
+    r->d = dstCap ? direct(env, dst, dstCap, NULL, "dst must be a direct ByteBuffer") : NULL;
+    if (dstCap && !r->d) return -1;
+    r->cur = (tsgpu_encrypt_cursor*)direct(env, cursor, 0, &ccap, "encrypt cursor must be a direct ByteBuffer of 64 bytes");
+    if (!r->cur) return -1;
+    if (ccap < (jlong)sizeof(tsgpu_encrypt_cursor)) { throw_arg(env, "encrypt cursor must be a direct ByteBuffer of 64 bytes"); return -1; }
+    if (!chunkSizes) { throw_arg(env, "chunks cannot be null"); return -1; }
+    r->n = (uint32_t)(*env)->GetArrayLength(env, chunkSizes);
+    if (!newSizes || (uint32_t)(*env)->GetArrayLength(env, newSizes) < r->n) { throw_arg(env, "newSizes must hold 1 int per chunk"); return -1; }
+    if (!nPartsOut || (*env)->GetArrayLength(env, nPartsOut) < 1) { throw_arg(env, "nPartsOut must hold 1 int"); return -1; }
+    if (partSize < 1) { throw_arg(env, "partSize must be positive"); return -1; }
+    if (key && (*env)->GetArrayLength(env, key) != 32) { throw_arg(env, "data key must be 32 bytes"); return -1; }
+    if (ivs && (uint32_t)(*env)->GetArrayLength(env, ivs) < 12 * r->n) { throw_arg(env, "ivs must hold 12 bytes per chunk"); return -1; }
+    r->k = key ? (*env)->GetByteArrayElements(env, key, NULL) : NULL;
+    r->a = aad ? (*env)->GetByteArrayElements(env, aad, NULL) : NULL;
+    r->alen = aad ? (*env)->GetArrayLength(env, aad) : 0;
+    r->iv = ivs ? (*env)->GetByteArrayElements(env, ivs, NULL) : NULL;
+    r->cs = (*env)->GetIntArrayElements(env, chunkSizes, NULL);
+    r->ns = (*env)->GetIntArrayElements(env, newSizes, NULL);
+    return 0;
+}
+/* Releases what encrypt_begin pinned; on success newSizes keeps the new sizes and nPartsOut[0] receives the count of completed
+ * parts. */
+static void encrypt_end(JNIEnv* env, jintArray chunkSizes, jbyteArray key, jbyteArray aad, jbyteArray ivs, jintArray newSizes,
+                        jintArray nPartsOut, encrypt_args* r, int rc, uint32_t nParts) {
+    (*env)->ReleaseIntArrayElements(env, chunkSizes, r->cs, JNI_ABORT);
+    (*env)->ReleaseIntArrayElements(env, newSizes, r->ns, rc ? JNI_ABORT : 0);
+    if (r->k) (*env)->ReleaseByteArrayElements(env, key, r->k, JNI_ABORT);
+    if (r->a) (*env)->ReleaseByteArrayElements(env, aad, r->a, JNI_ABORT);
+    if (r->iv) (*env)->ReleaseByteArrayElements(env, ivs, r->iv, JNI_ABORT);
+    if (rc) { throw_rt(env, rc); return; }
+    jint* np = (*env)->GetIntArrayElements(env, nPartsOut, NULL);
+    np[0] = (jint)nParts;
+    (*env)->ReleaseIntArrayElements(env, nPartsOut, np, 0);
+}
+
+/* EncryptCursor.encryptObject: partCrcs (int[], its length is part_cap) receives the CRC-32C of the upload parts the window
+ * completes; crcsOut (int[2]) receives, on the object's last window, the CRC-32C of the old object and of the new object. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_EncryptCursor_encryptObject(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray chunkSizes, jint originalChunkSize,
+    jlong originalFileSize, jbyteArray key, jbyteArray aad, jbyteArray ivs, jobject dst, jlong dstCap, jintArray newSizes,
+    jlong partSize, jintArray partCrcs, jintArray nPartsOut, jobject cursor, jboolean objectEndsHere, jintArray crcsOut) {
+    if (!partCrcs) { throw_arg(env, "partCrcs cannot be null"); return; }
+    if (!crcsOut || (*env)->GetArrayLength(env, crcsOut) < 2) { throw_arg(env, "crcsOut must hold 2 ints"); return; }
+    encrypt_args r;
+    if (encrypt_begin(env, src, srcLen, chunkSizes, key, aad, ivs, dst, dstCap, newSizes, partSize, nPartsOut, cursor, &r)) return;
+    const uint32_t cap = (uint32_t)(*env)->GetArrayLength(env, partCrcs);
+    jint* pc = (*env)->GetIntArrayElements(env, partCrcs, NULL);
+    uint32_t nParts = 0, crcs[2] = {0, 0};
+    int rc = tsgpu_encrypt_object((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, r.s, (uint64_t)srcLen, (const uint32_t*)r.cs, r.n,
+                                  (uint32_t)originalChunkSize, (uint64_t)originalFileSize, (const uint8_t*)r.k, (const uint8_t*)r.a,
+                                  (uint32_t)r.alen, (const uint8_t*)r.iv, r.d, (uint64_t)dstCap, (uint32_t*)r.ns, (uint64_t)partSize,
+                                  (uint32_t*)pc, cap, &nParts, r.cur, objectEndsHere ? 1 : 0, &crcs[0], &crcs[1]);
+    (*env)->ReleaseIntArrayElements(env, partCrcs, pc, rc ? JNI_ABORT : 0);
+    encrypt_end(env, chunkSizes, key, aad, ivs, newSizes, nPartsOut, &r, rc, nParts);
+    if (!rc && objectEndsHere) {
+        jint* out = (*env)->GetIntArrayElements(env, crcsOut, NULL);
+        out[0] = (jint)crcs[0]; out[1] = (jint)crcs[1];
+        (*env)->ReleaseIntArrayElements(env, crcsOut, out, 0);
+    }
+}
+
+/* EncryptCursor.encryptObjectCrc64: encryptObject with CRC-64/NVME.  partCrc64 (direct, 8 bytes per part: its capacity / 8 is
+ * part_cap) receives the CRCs of the upload parts the window completes; crcsOut (direct, 16 bytes) receives, on the object's last
+ * window, the CRC-64/NVME of the old object and of the new object. */
+JNIEXPORT void JNICALL Java_io_aiven_kafka_tieredstorage_transform_gpu_EncryptCursor_encryptObjectCrc64(
+    JNIEnv* env, jclass c, jlong h, jint flags, jobject src, jlong srcLen, jintArray chunkSizes, jint originalChunkSize,
+    jlong originalFileSize, jbyteArray key, jbyteArray aad, jbyteArray ivs, jobject dst, jlong dstCap, jintArray newSizes,
+    jlong partSize, jobject partCrc64, jintArray nPartsOut, jobject cursor, jboolean objectEndsHere, jobject crcsOut) {
+    jlong pcap = 0, wcap = 0;
+    uint64_t* pc = (uint64_t*)direct(env, partCrc64, 0, &pcap, "partCrc64 must be a direct ByteBuffer");
+    if (!pc) return;
+    uint64_t* out = (uint64_t*)direct(env, crcsOut, 0, &wcap, "crcsOut must be a direct ByteBuffer of 16 bytes");
+    if (!out) return;
+    if (wcap < 16) { throw_arg(env, "crcsOut must be a direct ByteBuffer of 16 bytes"); return; }
+    encrypt_args r;
+    if (encrypt_begin(env, src, srcLen, chunkSizes, key, aad, ivs, dst, dstCap, newSizes, partSize, nPartsOut, cursor, &r)) return;
+    uint32_t nParts = 0;
+    uint64_t crcs[2] = {0, 0};
+    int rc = tsgpu_encrypt_object_crc64((tsgpu_ctx*)(intptr_t)h, (uint32_t)flags, r.s, (uint64_t)srcLen, (const uint32_t*)r.cs, r.n,
+                                        (uint32_t)originalChunkSize, (uint64_t)originalFileSize, (const uint8_t*)r.k,
+                                        (const uint8_t*)r.a, (uint32_t)r.alen, (const uint8_t*)r.iv, r.d, (uint64_t)dstCap,
+                                        (uint32_t*)r.ns, (uint64_t)partSize, pc, (uint32_t)(pcap / 8), &nParts, r.cur,
+                                        objectEndsHere ? 1 : 0, &crcs[0], &crcs[1]);
+    encrypt_end(env, chunkSizes, key, aad, ivs, newSizes, nPartsOut, &r, rc, nParts);
     if (!rc && objectEndsHere) { out[0] = crcs[0]; out[1] = crcs[1]; }
 }

@@ -29,6 +29,7 @@ PARTS_CURSOR_SIZE = 32   # tsgpu_parts_cursor
 CHECK_CURSOR_SIZE = 128  # tsgpu_check_cursor
 REWRITE_CURSOR_SIZE = 192  # tsgpu_rewrite_cursor
 REKEY_CURSOR_SIZE = 64   # tsgpu_rekey_cursor
+ENCRYPT_CURSOR_SIZE = 64  # tsgpu_encrypt_cursor
 
 SYMBOLS = [
     "tsgpu_last_error", "tsgpu_version", "tsgpu_create", "tsgpu_destroy", "tsgpu_host_alloc", "tsgpu_host_free",
@@ -39,7 +40,7 @@ SYMBOLS = [
     "tsgpu_decode_path_stats", "tsgpu_transformed_chunks_serialize_ctx", "tsgpu_chunk_index_json_ctx",
     "tsgpu_transform_cursor", "tsgpu_transform_parts", "tsgpu_check_object", "tsgpu_rewrite_object",
     "tsgpu_transform_parts_crc64", "tsgpu_check_object_crc64", "tsgpu_rewrite_object_crc64",
-    "tsgpu_rekey_object", "tsgpu_rekey_object_crc64",
+    "tsgpu_rekey_object", "tsgpu_rekey_object_crc64", "tsgpu_encrypt_object", "tsgpu_encrypt_object_crc64",
 ]
 
 
@@ -89,6 +90,9 @@ def load(path=None):
     L.tsgpu_rekey_object.argtypes = [vp, u32, vp, u64, vp, u32, vp, vp, u32, vp, vp, u32, vp, vp, u64, u64, vp, u32, vp, vp,
                                      C.c_int, vp, vp]
     L.tsgpu_rekey_object_crc64.argtypes = L.tsgpu_rekey_object.argtypes
+    L.tsgpu_encrypt_object.argtypes = [vp, u32, vp, u64, vp, u32, u32, u64, vp, vp, u32, vp, vp, u64, vp, u64, vp, u32, vp, vp,
+                                       C.c_int, vp, vp]
+    L.tsgpu_encrypt_object_crc64.argtypes = L.tsgpu_encrypt_object.argtypes
     L.tsgpu_transform_device.argtypes = [vp, C.c_int, u32, vp, u64, u32, vp, vp, u32, vp, vp, u64, vp, vp]
     L.tsgpu_detransform_device.argtypes = [vp, C.c_int, u32, vp, u64, vp, u32, u32, vp, vp, u32, vp, vp, vp, vp]
     L.tsgpu_launch_count.restype = u64
@@ -399,6 +403,48 @@ class Context:
             1 if object_ends_here else 0, C.addressof(src_crc), C.addressof(obj_crc)))
         crc2 = (int(src_crc.value), int(obj_crc.value)) if object_ends_here else None
         return dst[:total], [int(x) for x in crcs[:n_parts.value]], crc2
+
+    def encrypt_object(self, src, chunk_sizes, key, ivs, part_size, original_chunk_size=0, original_file_size=0, aad=b"",
+                       flags=0, cursor=None, object_ends_here=True, part_cap=None, dst_cap=None):
+        """Encrypts one window of a stored unencrypted object's chunks with nothing decoded (tsgpu_encrypt_object): chunk i
+        becomes ivs[i] || AES-GCM(key, aad, chunk i) || tag, an empty chunk stays empty.  `flags`: FLAG_ZSTD for a compressed
+        object, FLAG_VERIFY.  original_chunk_size / original_file_size: the chunk index of a .log object, 0 for an .indexes object.
+        `cursor`: a 64-byte np.uint8 array (zeros at the start of the object), updated in place on success; None encrypts a whole
+        object.  Returns (new bytes, [new sizes], [CRC-32C of the parts this call completed], (source, object) CRC-32C or None
+        when the object does not end here)."""
+        return self._encrypt_object(self.lib.tsgpu_encrypt_object, C.c_uint32, src, chunk_sizes, key, ivs, part_size,
+                                    original_chunk_size, original_file_size, aad, flags, cursor, object_ends_here, part_cap, dst_cap)
+
+    def encrypt_object_crc64(self, src, chunk_sizes, key, ivs, part_size, original_chunk_size=0, original_file_size=0, aad=b"",
+                             flags=0, cursor=None, object_ends_here=True, part_cap=None, dst_cap=None):
+        """encrypt_object with CRC-64/NVME part, source and object checksums (tsgpu_encrypt_object_crc64): the same new bytes.  A
+        cursor carries one width: start and continue it with the same method."""
+        return self._encrypt_object(self.lib.tsgpu_encrypt_object_crc64, C.c_uint64, src, chunk_sizes, key, ivs, part_size,
+                                    original_chunk_size, original_file_size, aad, flags, cursor, object_ends_here, part_cap, dst_cap)
+
+    def _encrypt_object(self, fn, word, src, chunk_sizes, key, ivs, part_size, original_chunk_size, original_file_size, aad, flags,
+                        cursor, object_ends_here, part_cap, dst_cap):
+        s = _u8(src)
+        if cursor is None:
+            cursor = np.zeros(ENCRYPT_CURSOR_SIZE, np.uint8)
+        if not (isinstance(cursor, np.ndarray) and cursor.dtype == np.uint8 and cursor.size == ENCRYPT_CURSOR_SIZE
+                and cursor.flags.c_contiguous):
+            raise TypeError("cursor must be a contiguous np.uint8 array of %d bytes" % ENCRYPT_CURSOR_SIZE)
+        cs = np.ascontiguousarray(chunk_sizes, dtype=np.uint32)
+        total = int(sum(int(x) + 28 for x in cs if x))
+        dst = np.empty(total if dst_cap is None else dst_cap, dtype=np.uint8)
+        sizes = np.zeros(max(cs.size, 1), dtype=np.uint32)
+        if part_cap is None:                                 # the exact bound: (carried + window) // part_size, + 1 at the end
+            part_cap = (int(np.frombuffer(cursor[:8].tobytes(), np.uint64)[0]) % max(part_size, 1) + total) // max(part_size, 1) + 1
+        crcs = np.zeros(max(part_cap, 1), dtype=_np_word(word))
+        n_parts, src_crc, obj_crc = C.c_uint32(0), word(0), word(0)
+        k, a, iv = _u8(key), _u8(aad), _u8(ivs)
+        self._check(fn(
+            self._h, flags, _p(s), s.size, _p(cs), cs.size, original_chunk_size, original_file_size, _p(k), _p(a), a.size, _p(iv),
+            _p(dst), dst.size, _p(sizes), part_size, _p(crcs), part_cap, C.addressof(n_parts), cursor.ctypes.data,
+            1 if object_ends_here else 0, C.addressof(src_crc), C.addressof(obj_crc)))
+        crc2 = (int(src_crc.value), int(obj_crc.value)) if object_ends_here else None
+        return dst[:total], [int(x) for x in sizes[:cs.size]], [int(x) for x in crcs[:n_parts.value]], crc2
 
     # ---- device-resident API (raw device pointers as ints; bench.py passes torch data_ptr()) ----
     def slot_stride(self, flags, chunk_size):

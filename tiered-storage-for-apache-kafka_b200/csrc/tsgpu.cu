@@ -36,6 +36,7 @@
 #include "zstd_enc_blk.cuh"
 #include "zstd_dec.cuh"
 #include "reframe.cuh"
+#include "frame_walk.cuh"
 #include "host_index.hpp"
 
 using namespace ts;
@@ -867,7 +868,7 @@ static void parts_finish(const PartsRun<W>& pr, int segment_ends_here) {
 // has finished when its launch returns).  The variable `var` = <chunk>:<offset> flips the low bit of one byte of that chunk of
 // the batch's chunks [c0, c0 + nb) in `chunks`.  A negative offset counts from the chunk's end.
 //   TSGPU_SIMT_FLIP: the chunk's transformed bytes -- frame, or IV || ciphertext || tag -- before they are packed and verified
-//     (-1: last tag byte).  tests/test_simt_verify.py drives it.
+//     (-1: last tag byte).  tests/test_simt_verify.py drives it, and tests/test_simt_encrypt.py for tsgpu_encrypt_object.
 //   TSGPU_SIMT_FLIP_DECODED: the chunk's decoded bytes in d_orig right after the source decode of tsgpu_check_object /
 //     tsgpu_rewrite_object -- a decoder that misread the chunk.  tests/test_simt_reframe.py drives it: TSGPU_FLAG_REFRAME must
 //     not stamp the checksum of such a chunk.
@@ -1345,6 +1346,25 @@ struct ChunkLayout {
     uint32_t size(uint64_t g) const { return g + 1 < count ? ocs : g + 1 == count ? (uint32_t)(ofs - g * ocs) : 0u; }
 };
 
+// Chunk g of the object reads to `got` bytes (decoded, or a frame's Frame_Content_Size): TSGPU_OK when the chunk index gives it
+// that many.
+static int index_size_ok(const ChunkLayout& index, unsigned long long g, uint32_t got) {
+    if (g >= index.count)
+        return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, but the chunk index (original chunk size %u, original file "
+                    "size %llu) has %llu chunks", g, got, index.ocs, (unsigned long long)index.ofs, (unsigned long long)index.count);
+    if (got != index.size(g))
+        return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, the chunk index gives %u", g, got, index.size(g));
+    return TSGPU_OK;
+}
+
+// At the object's end: TSGPU_OK when it had as many chunks as the chunk index.
+static int index_count_ok(const ChunkLayout& index, uint64_t chunks) {
+    if (chunks != index.count)
+        return fail(TSGPU_E_CORRUPT, "the object has %llu chunks, the chunk index (original chunk size %u, original file size %llu) "
+                    "has %llu", (unsigned long long)chunks, index.ocs, (unsigned long long)index.ofs, (unsigned long long)index.count);
+    return TSGPU_OK;
+}
+
 // One window of a stored object, its arguments checked (source_args).
 struct SourceReq {
     uint32_t flags;                  // ZSTD and AES of the object (0: plain)
@@ -1490,11 +1510,7 @@ static int source_drain(tsgpu_ctx* c, const Batch& bt, const SourceReq& q, Check
         const unsigned long long g = cur.chunks + bt.c0 + i;
         if (status[i] == 1) return fail(TSGPU_E_AUTH, "Tag mismatch in chunk %llu", g);
         if (status[i] > 1) return fail(TSGPU_E_CORRUPT, "Invalid zstd frame in chunk %llu (code %u)", g, status[i]);
-        if (g >= index.count)
-            return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, but the chunk index (original chunk size %u, original file "
-                        "size %llu) has %llu chunks", g, got[i], index.ocs, (unsigned long long)index.ofs, (unsigned long long)index.count);
-        if (got[i] != index.size(g))
-            return fail(TSGPU_E_CORRUPT, "chunk %llu decoded to %u bytes, the chunk index gives %u", g, got[i], index.size(g));
+        if (int rc = index_size_ok(index, g, got[i])) return rc;
         L += got[i];
         obj += q.tsizes[bt.c0 + i];
     }
@@ -1514,9 +1530,7 @@ static int source_finish(const SourceReq& q, CheckCarry<W>& cur, int object_ends
     cur.obj_len += q.need;
     for (uint32_t i = 0; i < q.n; i++) cur.seg_len += q.index.size(cur.chunks - q.n + i);
     if (!object_ends_here) return TSGPU_OK;
-    if (cur.chunks != q.index.count)
-        return fail(TSGPU_E_CORRUPT, "the object has %llu chunks, the chunk index (original chunk size %u, original file size %llu) "
-                    "has %llu", (unsigned long long)cur.chunks, q.index.ocs, (unsigned long long)q.index.ofs, (unsigned long long)q.index.count);
+    if (int rc = index_count_ok(q.index, cur.chunks)) return rc;
     if (q.records) { int rc = records_segment_end(cur.rec); if (rc) return rc; }
     return TSGPU_OK;
 }
@@ -1997,6 +2011,232 @@ extern "C" int tsgpu_rekey_object_crc64(tsgpu_ctx* c, uint32_t flags, const uint
     return rekey_object(c, flags, src, src_len, transformed_sizes, n_chunks, from_key, from_aad, from_aad_len, to_key, to_aad,
                         to_aad_len, to_ivs, dst, dst_cap, part_size, part_crc64, part_cap, n_parts, cursor, object_ends_here,
                         source_crc64, object_crc64);
+}
+
+// ------------------------------------------------------------------------------------------ object encryption (host)
+// tsgpu_encrypt_object: a stored unencrypted object's chunks (frames or plain chunks) encrypted with nothing decoded.  Per batch,
+// on the compute stream: each chunk into its d_xf slot where its ciphertext goes (c_off + 12, a_off / a_len), [VERIFY: again
+// into its d_frames slot,] pcrc over them where they sit (the source word), [ZSTD: frame_walk over them,] the GCM encrypt stage
+// in place (each 16-byte block is read once, by the thread that then writes its ciphertext over it), IV and tag around it, [VERIFY:
+// the DEC kernels decrypt the new chunks into d_pack at the frame slots' offsets and verify_compare compares them with the copy,]
+// pack_chunks into d_pack and pcrc_tiles over it.  d_orig, the decoder and the compressor are never involved.  At the drain, in
+// object order: the frame statuses and the sizes against the chunk index, the verify verdict, then the source word extends the
+// carry and target_drain cuts the part prefixes and copies the batch out.
+
+// The encrypt cursor holds what the rekey cursor holds: the new object's parts, the chunk count and the source's CRC and length.
+static_assert(sizeof(RekeyCarry<uint32_t>) == sizeof(tsgpu_encrypt_cursor) && sizeof(RekeyCarry<uint64_t>) == sizeof(tsgpu_encrypt_cursor),
+              "the cursor holds the carry");
+
+struct EncryptReq {
+    bool zstd, verify;
+    bool indexed;                    // a .log object: its chunks are checked against the chunk index
+    ChunkLayout index;
+    const uint8_t* src; const uint32_t* tsizes;
+    Aes256RoundKeys rk;
+    const uint8_t* aad; uint32_t aad_len;
+    const uint8_t* ivs;
+};
+
+template <typename W>
+static int encrypt_issue(tsgpu_ctx* c, const Batch& bt, const EncryptReq& q) {
+    Work& w = *bt.w;
+    const uint32_t c0 = bt.c0, nb = bt.nb;
+    RT(rt::set_device(w.device));
+    rt::stream_t st = w.stream;
+    memcpy(w.hd.ivs, q.ivs + (size_t)c0 * TSGPU_IV_SIZE, (size_t)nb * TSGPU_IV_SIZE);
+    if (q.aad_len) memcpy(w.hd.aad, q.aad, q.aad_len);
+    slot_layout(c, w.hd, nb, c->slot_stride);
+    uint64_t at = bt.in_off, obj = 0, out = 0;
+    uint32_t max_t = 0;
+    for (uint32_t i = 0; i < nb; i++) {  // the sizes were bounded by the slot before any GPU work
+        const uint32_t t = q.tsizes[c0 + i];
+        w.hd.a_off[i] = w.hd.c_off[i] + TSGPU_IV_SIZE;
+        w.hd.a_len[i] = t;
+        w.hd.c_len[i] = w.back.sizes[i] = t ? t + TSGPU_IV_SIZE + TSGPU_TAG_SIZE : 0;   // an empty chunk stays empty
+        if (t) {
+            RT(rt::h2d(w.d_xf + w.hd.a_off[i], q.src + at, t, st));
+            if (q.verify) RT(rt::h2d(w.d_frames + w.hd.b_off[i], q.src + at, t, st));
+        }
+        at += t; obj += t; out += w.hd.c_len[i];
+        max_t = std::max(max_t, t);
+    }
+    RT(rt::h2d(w.d_desc, w.h_desc, w.desc_bytes, st));
+    // the slot's previous batch may still be copying d_pack out, its part prefixes read from the pcrc scratch this batch rewrites
+    { int rcw = wait_copies_out(w, st); if (rcw) return rcw; }
+    const ChunksIn in{w.d_xf, w.dd.a_off, w.dd.a_len};
+    { int rc = check_crc_word<W, true>(c, w, st, in.base, in.off, in.len, nb, obj, 0); if (rc) return rc; }
+    RT(rt::d2h(w.back.words, pcrc_of<W>(w).d_cuts, sizeof(W), st));
+    if (q.zstd) {
+        FrameWalkArgs F;
+        F.base = in.base; F.off = in.off; F.len = in.len; F.status = w.dd.status; F.fcs = w.dd.v_len; F.n = nb;
+        TS_LAUNCH_P(c->prof, "frame_walk", frame_walk_kernel, dim3((nb + FW_T - 1) / FW_T), dim3(FW_T), 0, st, F);
+        CHECK_LAUNCH("frame_walk_kernel");
+        RT(rt::d2h(w.back.src_status, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.back.src_sizes, w.dd.v_len, 4ull * nb, st));
+    }
+    // the GCM stage writes every chunk's IV || CT || TAG, an empty chunk's 28 bytes included; c_len (what pack, the part checksums
+    // and VERIFY read) keeps the sizes the chunks leave with, and the stage's own sizes go to b_len, which nothing reads after it
+    { int rc = gcm_stage<true>(c, w, w.keys[0], st, q.rk, in, ChunksOut{w.d_xf, w.dd.c_off, w.dd.b_len}, q.aad_len, w.dd.status, nb,
+                               max_t, 0xffffffffu); if (rc) return rc; }
+    const ChunksOut fin{w.d_xf, w.dd.c_off, w.dd.c_len};
+#ifdef TSGPU_SIMT
+    simt_flip("TSGPU_SIMT_FLIP", fin, c0, nb);
+#endif
+    if (q.verify) {                      // the new chunks read back, against the copy of their source in the frame slots
+        RT(rt::memset_async(w.dd.status, 0, 4ull * nb, st));
+        RT(rt::memset_async(w.dd.v_diff, 0xff, 4ull * nb, st));
+        int rc = gcm_stage<false>(c, w, w.keys[0], st, q.rk, fin, ChunksOut{w.d_pack, w.dd.b_off, w.dd.v_len}, q.aad_len, w.dd.status,
+                                  nb, max_t + TSGPU_IV_SIZE + TSGPU_TAG_SIZE, (uint32_t)(c->frame_stride - 16));
+        if (rc) return rc;
+        VerifyArgs V;
+        V.orig = w.d_frames; V.orig_off = w.dd.b_off; V.orig_len = w.dd.a_len;
+        V.back = w.d_pack; V.back_off = w.dd.b_off; V.back_len = w.dd.v_len;
+        V.status = w.dd.status; V.diff = w.dd.v_diff;
+        TS_LAUNCH_P(c->prof, "verify_compare", verify_compare_kernel, dim3(std::max(1u, (max_t + VERIFY_PIECE - 1) / VERIFY_PIECE), nb),
+                    dim3(VERIFY_T), 0, st, V);
+        CHECK_LAUNCH("verify_compare_kernel");
+        RT(rt::d2h(w.back.status, w.dd.status, 4ull * nb, st));
+        RT(rt::d2h(w.back.diff, w.dd.v_diff, 4ull * nb, st));
+    }
+    PackArgs P;
+    P.base = w.d_xf; P.stride = c->slot_stride; P.head = TSGPU_SLOT_HEAD; P.len = w.dd.c_len; P.n = nb; P.out = w.d_pack;
+    const uint32_t longest = max_t + TSGPU_IV_SIZE + TSGPU_TAG_SIZE;
+    TS_LAUNCH_P(c->prof, "pack_chunks", pack_chunks_kernel, dim3((longest + PACK_PIECE - 1) / PACK_PIECE, nb), dim3(PACK_T), 0, st, P);
+    CHECK_LAUNCH("pack_chunks_kernel");
+    { int rc = parts_stage<W>(c, w, st, w.dd.c_len, nb, out); if (rc) return rc; }
+    RT(rt::event_record(w.ev_sizes, st));
+    return TSGPU_OK;
+}
+
+// A drained batch's verdicts in object order: every chunk's frame and size against the chunk index, then (VERIFY) every
+// read-back.  `first`: the object's number of the call's first chunk.
+static int encrypt_verdict(const Batch& bt, const EncryptReq& q, uint64_t first) {
+    const Back& b = bt.w->back;
+    if (q.indexed) {
+        for (uint32_t i = 0; i < bt.nb; i++) {
+            const unsigned long long g = first + bt.c0 + i;
+            const uint32_t t = q.tsizes[bt.c0 + i];
+            if (q.zstd && t && b.src_status[i]) return fail(TSGPU_E_CORRUPT, "Invalid zstd frame in chunk %llu (code %u)", g, b.src_status[i]);
+            if (int rc = index_size_ok(q.index, g, q.zstd && t ? b.src_sizes[i] : t)) return rc;
+        }
+    }
+    if (!q.verify) return TSGPU_OK;
+    for (uint32_t i = 0; i < bt.nb; i++) {
+        const unsigned long long g = first + bt.c0 + i;
+        if (q.tsizes[bt.c0 + i] == 0) continue;          // nothing to read back (the DEC kernels call an empty chunk malformed)
+        if (b.status[i] == 1) return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: tag check failed", g);
+        if (b.status[i] != 0) return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: size check failed", g);
+        if (b.diff[i] != VERIFY_NO_DIFF)
+            return fail(TSGPU_E_VERIFY, "verify: chunk %llu did not read back: bytes differ from offset %u", g, b.diff[i]);
+    }
+    return TSGPU_OK;
+}
+
+template <typename W>
+static int encrypt_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* chunk_sizes,
+                          uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size, const uint8_t key[32],
+                          const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs, uint8_t* dst, uint64_t dst_cap,
+                          uint32_t* new_transformed_sizes, uint64_t part_size, W* part_crc, uint32_t part_cap, uint32_t* n_parts,
+                          tsgpu_encrypt_cursor* cursor, int object_ends_here, W* source_crc, W* object_crc) try {
+    if (!c) return fail(TSGPU_E_ARG, "ctx cannot be null");
+    if (!cursor) return fail(TSGPU_E_ARG, "cursor cannot be null");
+    if (object_ends_here && (!source_crc || !object_crc))
+        return fail(TSGPU_E_ARG, "source_%s/object_%s cannot be null", crc_arg<W>(), crc_arg<W>());
+    if (flags & TSGPU_FLAG_AES)
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_AES: the object is already encrypted; tsgpu_rekey_object re-encrypts it under a new key");
+    if (flags & ~(TSGPU_FLAG_ZSTD | TSGPU_FLAG_VERIFY))
+        return fail(TSGPU_E_ARG, "unknown flags %u: only TSGPU_FLAG_ZSTD and TSGPU_FLAG_VERIFY apply to an encryption", flags);
+    if ((flags & TSGPU_FLAG_ZSTD) && original_chunk_size == 0)
+        return fail(TSGPU_E_ARG, "TSGPU_FLAG_ZSTD needs the chunk index (original_chunk_size > 0): an .indexes object is not compressed");
+    if (n_chunks && !chunk_sizes) return fail(TSGPU_E_ARG, "chunks cannot be null");
+    if (n_chunks && !new_transformed_sizes) return fail(TSGPU_E_ARG, "new_transformed_sizes cannot be null");
+    if ((uint64_t)c->max_batch * c->slot_stride > 0xffffff00ull)
+        return fail(TSGPU_E_ARG, "part checksums need batches below 4 GiB: max_batch %u x slot stride %llu is more", c->max_batch,
+                    (unsigned long long)c->slot_stride);
+    RekeyCarry<W> cur;
+    memcpy(&cur, cursor, sizeof cur);
+    uint64_t need = 0, out = 0;
+    for (uint32_t i = 0; i < n_chunks; i++) {
+        const uint32_t t = chunk_sizes[i];
+        // the new chunk goes into one transformed slot (what tsgpu_detransform reads one into)
+        if ((uint64_t)t + TSGPU_IV_SIZE + TSGPU_TAG_SIZE > c->slot_stride - TSGPU_SLOT_HEAD - 16)
+            return fail(TSGPU_E_ARG, "chunk %llu: a chunk of %u bytes encrypted exceeds the context's capacity",
+                        (unsigned long long)(cur.chunks + i), t);
+        need += t;
+        out += t ? (uint64_t)t + TSGPU_IV_SIZE + TSGPU_TAG_SIZE : 0;
+    }
+    if (int rc = aes_args_ok(TSGPU_FLAG_AES, AES_ENC, key, !need || ivs, aad, aad_len)) return rc;   // empty chunks take no IV
+    if (need && !src) return fail(TSGPU_E_ARG, "inputStream cannot be null");
+    if (need > src_len) return fail(TSGPU_E_SHORT, "Stream has fewer bytes than expected");
+    if (need && !dst) return fail(TSGPU_E_ARG, "dst cannot be null");
+    if (out > dst_cap) return fail(TSGPU_E_SHORT, "dst too small: the window's new chunks are %llu bytes, dst_cap is %llu",
+                                   (unsigned long long)out, (unsigned long long)dst_cap);
+    if (need) {
+        if (int rc = new_ivs_ok(ivs, n_chunks, src, chunk_sizes, /*same_key=*/false, cur.chunks, /*skip_empty=*/true)) return rc;
+    }
+    PartsRun<W> run;
+    if (int rc = parts_begin(run, PartsReq<W>{part_size, &cur.out, part_crc, part_cap, n_parts, object_crc}, TSGPU_FLAG_AES, out,
+                             object_ends_here)) return rc;
+    EncryptReq q;
+    q.zstd = flags & TSGPU_FLAG_ZSTD;
+    q.verify = (flags & TSGPU_FLAG_VERIFY) || c->verify_default;
+    q.indexed = original_chunk_size > 0;
+    q.index = ChunkLayout{original_chunk_size, original_file_size,
+                          original_chunk_size ? (original_file_size + original_chunk_size - 1) / original_chunk_size : 0};
+    q.src = src; q.tsizes = chunk_sizes;
+    q.rk = aes256_expand_key(key);
+    q.aad = aad; q.aad_len = aad_len; q.ivs = ivs;
+    // The index of an empty segment materialises one chunk of 0 bytes: a caller that walks it passes that chunk.
+    uint32_t n = n_chunks;
+    if (q.indexed && q.index.count == 0 && cur.chunks == 0 && n == 1 && chunk_sizes[0] == 0) n = 0;
+    if (q.indexed && !need) {                                              // no GPU work: the sizes are checked here
+        for (uint32_t i = 0; i < n; i++) if (int rc = index_size_ok(q.index, cur.chunks + i, 0)) return rc;
+    }
+    if (need) {                                                            // a window of empty chunks writes nothing
+        uint64_t dst_off = 0;
+        const int rc = run_batches(c, n, chunk_sizes,
+            [&](const Batch& bt) { return encrypt_issue<W>(c, bt, q); },
+            [&](const Batch& bt) {
+                { int r = encrypt_verdict(bt, q, cur.chunks); if (r) return r; }
+                uint64_t obj = 0;
+                for (uint32_t i = 0; i < bt.nb; i++) obj += chunk_sizes[bt.c0 + i];
+                cur.src_raw = crc_shift(cur.src_raw, obj, 0) ^ reinterpret_cast<const W*>(bt.w->back.words)[0];
+                return target_drain<W>(c, bt, nullptr, &run, dst, dst_cap, dst_off);
+            },
+            [&](const std::vector<Work*>& slots, int rcb) { return parts_idle(&run, slots, rcb); });
+        if (rc) return rc;
+    }
+    cur.chunks += n;
+    cur.src_len += need;
+    if (object_ends_here && q.indexed) { if (int rc = index_count_ok(q.index, cur.chunks)) return rc; }
+    for (uint32_t i = 0; i < n_chunks; i++)
+        new_transformed_sizes[i] = chunk_sizes[i] ? chunk_sizes[i] + TSGPU_IV_SIZE + TSGPU_TAG_SIZE : 0;
+    parts_finish(run, object_ends_here);                                   // writes cur.out and the part CRCs
+    if (object_ends_here) *source_crc = crc_finish(cur.src_raw, cur.src_len, 0);
+    memcpy(cursor, &cur, sizeof cur);
+    return TSGPU_OK;
+} catch (const std::bad_alloc&) { return fail(TSGPU_E_NOMEM, "out of memory"); }
+
+extern "C" int tsgpu_encrypt_object(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* chunk_sizes,
+                                    uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
+                                    const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                                    uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                                    uint64_t part_size, uint32_t* part_crc32c, uint32_t part_cap, uint32_t* n_parts,
+                                    tsgpu_encrypt_cursor* cursor, int object_ends_here, uint32_t* source_crc32c, uint32_t* object_crc32c) {
+    return encrypt_object(c, flags, src, src_len, chunk_sizes, n_chunks, original_chunk_size, original_file_size, key, aad, aad_len,
+                          ivs, dst, dst_cap, new_transformed_sizes, part_size, part_crc32c, part_cap, n_parts, cursor, object_ends_here,
+                          source_crc32c, object_crc32c);
+}
+
+extern "C" int tsgpu_encrypt_object_crc64(tsgpu_ctx* c, uint32_t flags, const uint8_t* src, uint64_t src_len, const uint32_t* chunk_sizes,
+                                          uint32_t n_chunks, uint32_t original_chunk_size, uint64_t original_file_size,
+                                          const uint8_t key[32], const uint8_t* aad, uint32_t aad_len, const uint8_t* ivs,
+                                          uint8_t* dst, uint64_t dst_cap, uint32_t* new_transformed_sizes,
+                                          uint64_t part_size, uint64_t* part_crc64, uint32_t part_cap, uint32_t* n_parts,
+                                          tsgpu_encrypt_cursor* cursor, int object_ends_here, uint64_t* source_crc64, uint64_t* object_crc64) {
+    return encrypt_object(c, flags, src, src_len, chunk_sizes, n_chunks, original_chunk_size, original_file_size, key, aad, aad_len,
+                          ivs, dst, dst_cap, new_transformed_sizes, part_size, part_crc64, part_cap, n_parts, cursor, object_ends_here,
+                          source_crc64, object_crc64);
 }
 
 // ------------------------------------------------------------------------------------------ device-resident API

@@ -173,6 +173,24 @@ struct SegmentLogUpload {
     std::optional<uint32_t> objectCrc32c;                // with partChecksums: CRC-32C of the whole object (S3 FULL_OBJECT, GCS crc32c)
     std::optional<uint64_t> objectCrc64nvme;             // with partChecksums and crc64Parts: CRC-64/NVME of the whole object (S3 CRC64NVME)
 };
+// The chunk index TransformFinisher builds for a segment of n original bytes in chunks of ocs whose `got` transformed sizes are
+// `sizes`: fixed when every chunk has the same known transformed size (ocs, or ocs + 28 encrypted), variable after compression.
+inline std::shared_ptr<ChunkIndex> finisherChunkIndex(int ocs, int n, bool compressed, bool encrypted, const uint32_t* sizes,
+                                                      uint32_t got) {
+    if (got == 0) {                                      // nothing went through the finisher (TransformFinisher.java:112-132)
+        if (compressed || encrypted) throw IllegalStateException("Chunk index was not built, was finisher used?");
+        return FixedSizeChunkIndexBuilder(ocs, n, ocs).finish(0);
+    }
+    if (compressed) {
+        VariableSizeChunkIndexBuilder b(ocs, n);
+        for (uint32_t i = 0; i + 1 < got; i++) b.addChunk((int)sizes[i]);
+        return b.finish((int)sizes[got - 1]);
+    }
+    FixedSizeChunkIndexBuilder b(ocs, n, encrypted ? ocs + 28 : ocs);
+    for (uint32_t i = 0; i + 1 < got; i++) b.addChunk((int)sizes[i]);
+    return b.finish((int)sizes[got - 1]);
+}
+
 class SegmentLogUploader {
 public:
     using PartSink = std::function<void(const UploadPart&, const uint8_t* data)>;
@@ -246,22 +264,9 @@ public:
         }
         if (rc == TSGPU_E_RECORDS) throw InvalidRecordBatchException(tsgpu_last_error());
         if (rc) throw std::runtime_error(tsgpu_last_error());            // RuntimeException in the reference
-        // TransformFinisher: fixed index when every chunk has the same known transformed size, variable after compression
         const int ocs = chunkSize ? chunkSize : (int)n;
         for (uint32_t i = 0; i < got; i++) { r.transformedSizes.push_back((int32_t)sizes[i]); r.objectBytes += sizes[i]; }
-        if (got == 0) {                                      // nothing went through the finisher (TransformFinisher.java:112-132)
-            if (flags != 0) throw IllegalStateException("Chunk index was not built, was finisher used?");
-            r.chunkIndex = FixedSizeChunkIndexBuilder(ocs, (int)n, ocs).finish(0);
-        } else if (r.compressed) {
-            VariableSizeChunkIndexBuilder b(ocs, (int)n);
-            for (uint32_t i = 0; i + 1 < got; i++) b.addChunk((int)sizes[i]);
-            r.chunkIndex = b.finish((int)sizes[got - 1]);
-        } else {
-            const int tcs = encryptionEnabled ? ocs + 28 : ocs;
-            FixedSizeChunkIndexBuilder b(ocs, (int)n, tcs);
-            for (uint32_t i = 0; i + 1 < got; i++) b.addChunk((int)sizes[i]);
-            r.chunkIndex = b.finish((int)sizes[got - 1]);
-        }
+        r.chunkIndex = finisherChunkIndex(ocs, (int)n, r.compressed, encryptionEnabled, sizes.data(), got);
         std::vector<UploadPart> plan = multipartPlan(r.objectBytes, partSize);
         if (checksums && crc64Parts) {
             if (partCrcs64.size() != plan.size()) throw std::runtime_error("part checksums do not match the multipart plan");
